@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- MERLOT pretraining-step throughput on B200 (BASELINE.json metric: frame-caption segments/sec, fwd+bwd+AdamW).
+"""bench.py -- MERLOT pretraining-step throughput on H100 (BASELINE.json metric: frame-caption segments/sec, fwd+bwd+AdamW).
 
-  python bench.py --gpus N --steps K --warmup W            # this repo's sm_100a path (N>1: launched under torchrun)
+  python bench.py --gpus N --steps K --warmup W            # this repo's sm_90a path (N>1: launched under torchrun)
+  python bench.py ... --dump-outputs DIR                   # also write what the last timed step computed, as DIR/*.npy
   python bench.py --impl reference --gpus N --steps K ...  # the reference math on the box's host cores (oracle port;
                                                            # TF 1.15 cannot be installed here, see DESIGN.md)
 
@@ -39,7 +40,7 @@ STEM = "patch"  # --stem hybrid: merlot.yaml exactly as shipped (resnet_layers [
 
 
 def load_config():
-    """merlot.yaml's model/optimizer sections (restated here because /root/reference does not travel to the GPU box),
+    """merlot.yaml's model/optimizer sections (restated here so that the benchmark needs no reference checkout),
     with the patch-embed stem the north star names (SURVEY.md discrepancy 1)."""
     from merlot_b200.config import NeatConfig
     model = dict(transpose_input=True, num_chunks_in_group=4, masking_use_attn=True, masking_rate=0.2, masking_do_spanbert=True,
@@ -60,11 +61,13 @@ def load_config():
 
 
 def peaks():
+    """(sustained bf16 TFLOP/s, burst bf16 TFLOP/s, HBM GB/s, source).  Without a measured file: NVIDIA's H100 SXM data sheet
+    (dense bf16 989 TFLOP/s, HBM3 3.35 TB/s at up to 700 W) -- an upper bound, not a rate this card was seen to reach."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1400.0), d.get("bf16_tflops", 1590.0), d.get("hbm_gbs", 6650.0), "measured"
-    return 1400.0, 1590.0, 6650.0, "fallback"
+        return d.get("bf16_tflops_sustained", 989.0), d.get("bf16_tflops", 989.0), d.get("hbm_gbs", 3350.0), "measured"
+    return 989.0, 989.0, 3350.0, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -169,8 +172,10 @@ def run_reference(args):
         step()
     t0 = time.perf_counter()
     for _ in range(args.steps):
-        step()
+        total = step()
     dt = time.perf_counter() - t0
+    if args.dump_outputs:
+        dump_arrays(args.dump_outputs, {"loss": np_array([total], "float64")})
     val = segs * args.steps / dt
     cores = cpu_threads()
     line = {
@@ -236,6 +241,8 @@ def run_ours(args):
     sync_all()
     launches = int(lib.merlot_launch_count())
     log("timed region done")
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, spec, store)
     ms = torch.tensor([e0.elapsed_time(e1)], device=dev)
     if dist is not None:
         dist.dist.all_reduce(ms, op=dist.dist.ReduceOp.MAX)
@@ -333,14 +340,13 @@ def run_ours(args):
         sustained, burst, hbm, how = peaks()
         ach = fl.value / (tm.value * 1e-3) / 1e12
         dom = dominant_k1_instance(dev, sustained)
-        roof = {"bound": "tensor", "kernel": "gemm_bf16_kernel / gemm2_bf16_kernel (K1, tcgen05), all launches of a step", "achieved": ach,
+        roof = {"bound": "tensor", "kernel": "gemm_bf16_kernel (K1, wgmma), all launches of a step", "achieved": ach,
                 "peak": sustained, "unit": "TFLOP/s", "frac": ach / sustained, "traffic": dom.get("traffic"),
                 "traffic_of": dom.get("traffic_of"), "dominant_instance": dom, "peak_source": f"{how} bf16_tflops_sustained",
                 "launches_per_step": nl.value, "gemm_ms_per_step": tm.value, "gemm_share_of_step": tm.value / (ms_total / args.steps),
-                "note": "sum over all K1 launches (1-CTA and CTA-pair variants) of one single-stream step: sum(2MNK) / sum(CUDA-event "
-                        "duration on the launch stream). The event pairs switch off the PDL overlap between consecutive kernels and "
-                        "add ~2 us per launch, so this is a lower bound (CUPTI kernel times give ~9.5 ms of K1 per step); isolated "
-                        "per-shape rates are in profiles/r01_k1_epilogue_timings.txt"}
+                "note": "sum over all K1 launches of one single-stream step: sum(2MNK) / sum(CUDA-event duration on the launch "
+                        "stream). The event pairs switch off the PDL overlap between consecutive kernels and add a few us per "
+                        "launch, so this is a lower bound"}
     torch.cuda.synchronize()
     # ---- attention TFLOP/s as a share of the peak (second half of BASELINE.json's metric), rank 0, after the timed regions ----
     attn = attention_rates(dev) if rank == 0 else None
@@ -372,7 +378,7 @@ def run_ours(args):
                         "configs[1]'s 4-segment pretrain step, fwd+bwd+AdamW, hidden dropout 0.1 -- not the north-star workload"),
                        "global_batch": PER_GPU_BATCH * world, "segments_per_step": segs_per_rank * world,
                        "parallelism": f"dp{world}", "l2": "per-step working set (~6 GB activations + 2.7 GB parameter state) "
-                                                          "is far larger than the 126 MB L2; no explicit flush",
+                                                          "is far larger than the 50 MB L2; no explicit flush",
                        "params": store.num_params()},
             "clocks": clocks,
             "e2e": {"value": e2e_val, "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 12,
@@ -420,6 +426,7 @@ def run_other_config(args):
         def step():
             spec = model_fn(feats, None, "train", None)
             spec.train_op()
+            return spec
         what = ("configs[4] stress: 8 segments x 384-token captions, 192x352 frames, joint sequence 3608, pretrain step "
                 "fwd+bwd+AdamW, hidden dropout 0.1; max_position_embeddings overridden 1024 -> 3072")
         metric = METRIC
@@ -466,9 +473,14 @@ def run_other_config(args):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(args.steps):
-        step()
+        out = step()
     e1.record()
     torch.cuda.synchronize()
+    if args.dump_outputs and rank == 0:
+        if args.config == 5:
+            dump_outputs(args.dump_outputs, out, model_fn.store)
+        else:  # configs 1 / 4: the forward's output (hidden states / temporal probabilities)
+            dump_arrays(args.dump_outputs, {"output": sample_f32(out)})
     if dist is not None:
         dist.barrier()
     ms = torch.tensor([e0.elapsed_time(e1)], device=dev)
@@ -483,7 +495,7 @@ def run_other_config(args):
             "warmup": max(args.warmup, 3), "ms_per_step": t, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "bf16", "data": "synthetic",
             "config": {"workload": what, "global_batch": batch * world, "segments_per_step": segs * world, "parallelism": f"dp{world}",
-                       "l2": "working set far larger than the 126 MB L2; no explicit flush"},
+                       "l2": "working set far larger than the 50 MB L2; no explicit flush"},
             "clocks": clocks, "gpu_launches": int(L.lib().merlot_launch_count()),
             "roofline": {"bound": "tensor", "kernel": "whole step (algorithmic FLOPs of SURVEY 8(d) / step time)", "achieved": tf,
                          "peak": sustained, "unit": "TFLOP/s", "frac": tf / sustained, "traffic": None,
@@ -494,9 +506,8 @@ def run_other_config(args):
 
 
 def dominant_k1_instance(dev, sustained):
-    """The K1 instance with the largest share of the step (profiles/r02_launch_summary_final.txt: the split-K wgrad pair kernel,
-    15 %): its ViT FFN2 shape timed live with CUDA events, and its DRAM traffic per launch from the committed `ncu --set full`
-    capture (profiles/r02_ncu_kernels_final.json; algorithmic bytes: A 52.3 MB + B 13.1 MB + fp32 red.add output 9.4 MB)."""
+    """The split-K wgrad K1 instance of the ViT FFN2 (3072x768x8512), timed live with CUDA events; its traffic is the
+    algorithmic byte count (A 52.3 MB + B 13.1 MB + fp32 red.add output 9.4 MB)."""
     from merlot_b200 import ops
     M, H, I = 8512, 768, 3072
     g = torch.Generator().manual_seed(0)
@@ -515,20 +526,44 @@ def dominant_k1_instance(dev, sustained):
     torch.cuda.synchronize()
     us = e0.elapsed_time(e1) / 20 * 1e3
     tf = 2.0 * M * H * I / (us * 1e-6) / 1e12
-    out = {"kernel": "gemm2_bf16_kernel<256, A MN-major, B MN-major, split-K red.add f32> (ViT FFN2 wgrad 3072x768x8512)",
-           "us_per_launch": us, "achieved": tf, "frac": tf / sustained, "algorithmic_bytes": M * I * 2 + M * H * 2 + I * H * 4,
-           "inputs": "104 MB working set per launch pair alternates with nothing else: L2-resident repeats (the ncu capture is the cold figure)"}
-    try:
-        d = json.load(open(os.path.join(ROOT, "profiles", "r02_ncu_kernels_final.json")))
-        ls = [x for x in d["launches"] if "gemm2_bf16_kernel<256, 1, 1, 2, 1>" in x["kernel"]]
-        top = max(ls, key=lambda x: x.get("dram_read_bytes", 0))
-        out["traffic"] = top["dram_read_bytes"] + top["dram_write_bytes"]
-        out["traffic_of"] = "dram__bytes_read.sum + dram__bytes_write.sum of one launch of the dominant instance, ncu --set full (profiles/r02_ncu_kernels_final.json)"
-        out["ncu_tensor_pipe_pct"] = top.get("tensor_pipe_pct")
-    except Exception as e:  # the capture is evidence, never fatal
-        out["traffic"] = None
-        out["traffic_of"] = f"profiles/r02_ncu_kernels_final.json not readable: {e!r}"[:160]
-    return out
+    nbytes = M * I * 2 + M * H * 2 + I * H * 4
+    return {"kernel": "gemm_bf16_kernel<256, A MN-major, B MN-major> split-K red.add f32 (ViT FFN2 wgrad 3072x768x8512)",
+            "us_per_launch": us, "achieved": tf, "frac": tf / sustained, "algorithmic_bytes": nbytes,
+            "traffic": nbytes, "traffic_of": "algorithmic bytes of one launch (A + B + fp32 output)",
+            "inputs": "repeated launches on the same operands: partly L2-resident"}
+
+
+DUMP_PARAM_SAMPLE = 1 << 22  # 4 Mi parameters (16 MB fp32) of the updated parameter vector
+
+
+def np_array(values, dtype):
+    import numpy as np
+    return np.array(values, dtype=dtype)
+
+
+def sample_f32(x):
+    """x as a flat float32 array; above DUMP_PARAM_SAMPLE elements a fixed, seeded sample of it."""
+    x = x.detach().reshape(-1)
+    if x.numel() > DUMP_PARAM_SAMPLE:
+        idx = torch.randint(0, x.numel(), (DUMP_PARAM_SAMPLE,), generator=torch.Generator().manual_seed(1234))
+        x = x[idx.to(x.device)]
+    return x.float().cpu().numpy()
+
+
+def dump_arrays(out_dir, arrays):
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+    log(f"outputs of the last timed step written to {out_dir}: {', '.join(sorted(arrays))}")
+
+
+def dump_outputs(out_dir, spec, store):
+    """What a training step hands its caller, after the last timed step: the three losses (float64) and a fixed, seeded
+    sample of the fp32 parameters AdamW has just written (float32).  The inputs, weights and dropout seeds depend only on
+    the command-line arguments, so two builds run with the same arguments can be compared file by file."""
+    dump_arrays(out_dir, {"loss_parts": np_array([float(x) for x in spec.loss_parts], "float64"),
+                          "params_sample": sample_f32(store.p)})
 
 
 def attention_rates(dev):
@@ -576,6 +611,9 @@ def main():
     ap.add_argument("--config", type=int, default=2, choices=[1, 2, 4, 5],
                     help="BASELINE.json configs, 1-based as SURVEY 8 numbers them: 2 (default) = the headline 4-segment pretrain step")
     ap.add_argument("--batch", type=int, default=0, help="per-GPU batch override for --config 1/4/5")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step computed as DIR/*.npy: losses and a seeded sample of the updated "
+                         "parameters (training steps), the forward's output (--config 1/4), the loss (--impl reference)")
     ap.add_argument("--stem", default="patch", choices=["patch", "hybrid"],
                     help="hybrid: merlot.yaml as shipped (ResNet-lite stem before the ViT); default = the north star's patch embedding")
     args = ap.parse_args()

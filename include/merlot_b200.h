@@ -1,5 +1,5 @@
 /*
- * merlot_b200 -- C-ABI of the B200-native (sm_100a) implementation of MERLOT's dense forward/backward hot path.
+ * merlot_b200 -- C-ABI of the H100-native (sm_90a) implementation of MERLOT's dense forward/backward hot path.
  *
  * The reference (rowanz/merlot) has no FFI/operator layer: its boundary is the Python class `MerlotModel`
  * (model/modeling.py:47-668) plus `optimization.build_optimizer_from_config` (utils/optimization.py:11-30), both of
@@ -41,7 +41,7 @@ long long merlot_launch_count(void);
 void merlot_reset_launch_count(void);
 
 /* ------------------------------------------------------------------------------------------------------------
- * K1: bf16 tensor-core GEMM (tcgen05.mma, TMA-fed, fp32 accumulation in TMEM) with fused epilogues.
+ * K1: bf16 tensor-core GEMM (wgmma, TMA-fed, fp32 accumulation in registers) with fused epilogues.
  *     C[M,N] = epilogue( alpha * sum_k A(m,k) * B(n,k) )
  * Replaces every tf.layers.dense / tf.matmul on the hot path and their tf.gradients:
  *   utils/transformer.py:21-25 (q/k/v), :130-135 (context_projection_layer), :149-155 (intermediate + gelu),
@@ -83,13 +83,13 @@ typedef struct merlot_gemm {
   uint32_t flags;
   float dropout_p; uint64_t dropout_seed; uint32_t dropout_site;
   int splits;                     /* 0 = auto; >1 requires MERLOT_GEMM_ATOMIC */
-  int block_n;                    /* 0 = auto; else 128, 192 or 256; -256 / -192 force the CTA-pair kernel (tuning / tests) */
+  int block_n;                    /* 0 = auto; else 128, 192 or 256 (tuning / tests) */
 } merlot_gemm_t;
 
 int merlot_gemm_bf16(const merlot_gemm_t* g, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
- * K2/K3/K4: masked softmax attention, FlashAttention-tiled on tcgen05 (probabilities never materialised in HBM).
+ * K2/K3/K4: masked softmax attention, FlashAttention-tiled on wgmma (probabilities never materialised in HBM).
  * Replaces utils/transformer.py:98-127 (scores = q k^T / sqrt(d); scores*m - 1e10*(1-m); softmax; probs @ v), its
  * tf.gradients, and the column sums of `self_attn_probs` consumed by model/modeling.py:428 (mask_inputs).
  *  qkv   : bf16 [B*S, ld_qkv], columns [0,H)=q, [H,2H)=k, [2H,3H)=v with head h at column h*64 (the fused QKV GEMM out).
@@ -129,12 +129,6 @@ typedef struct merlot_attn {
 
 int merlot_attention_fwd(const merlot_attn_t* a, void* stream);
 int merlot_attention_bwd(const merlot_attn_t* a, void* stream);
-/* diagnostics: 24 x u64 device buffer (or NULL = off; [16,24) = the K3 issuer lane); one softmax thread per CTA adds its per-phase cycle counts, [0,8) = K2
- * {wait S, load+max, rescale, exp+store P, fence+sync, final wait, key tiles, epilogue}, [8,16) = K3 {wait S^T/dP^T, softmax
- * arithmetic, fence+sync, wait dV/dK/dQ, dQ read-out, sync, query chunks, dK/dV epilogue} (tools/attn_phases.py) */
-void merlot_attention_debug_counters(void* buf_u64x24);
-/* timing experiments (results are WRONG when non-zero): K3 bit 0 = skip the arithmetic, bit 1 = skip MMA2, bit 2 = skip MMA1 */
-void merlot_attention_debug_mode(int mode);
 int merlot_attention_bwd_dq_parts(int S);                          /* slices used by bwd for this S; 0 = atomic single slice */
 size_t merlot_attention_bwd_workspace_bytes(int B, int S, int heads); /* bytes of dq_accum (ld_dq = heads*64) */
 int merlot_attention_colsum(const merlot_attn_t* a, void* stream);
@@ -353,8 +347,8 @@ int merlot_group_norm_fwd(const void* x_bf16, const float* gamma, const float* b
 /* tf.nn.avg_pool2d(ksize 2, strides 2, 'SAME') on NHWC bf16 (:81,93,159) */
 int merlot_avgpool2_same(const void* x_bf16, int N, int h, int w, int C, void* y_bf16, void* stream);
 
-/* K13 backward pieces (tf.gradients of the same graph).  Verified on the B200 through the whole training step (parameter
- * gradients on the bf16 noise floor of the graph, profiles/r01_hybrid_stem_backward.txt) and, once, op by op. */
+/* K13 backward pieces (tf.gradients of the same graph); tests/test_gpu_stem.py checks them op by op and through the whole
+ * training step. */
 /* GroupNorm(+ReLU, +shortcut) backward: g = dy * [y > 0]; dx, dshortcut (= g, optional), dgamma += , dbeta += ;
  * red: f32 scratch [N, groups, 2]; stats: what merlot_group_norm_fwd left for this site */
 int merlot_group_norm_bwd(const void* dy_bf16, const void* x_bf16, const void* y_bf16, const float* stats, const float* gamma,
@@ -383,10 +377,6 @@ int merlot_add_bf16(const void* a, const void* b, void* out, long long n, void* 
  * end() synchronises the device and returns the summed duration (ms), algorithmic FLOPs (2*M*N*K) and launch count. */
 void merlot_gemm_profile_begin(void);
 int merlot_gemm_profile_end(double* total_ms, double* total_flops, long long* launches);
-/* kernel-tuning diagnostics: when buf (device, 8 x u64 per CTA, >= 8*148 entries) is non-null every 1-CTA K1 launch writes
- * per-CTA stall cycles {total, mma:wait-smem-full, mma:wait-tmem-empty, tma:wait-smem-empty, epi:wait-tmem-full,
- * epi:wait-staging, epi:work, tiles}.  Pass NULL to switch off (the default). */
-void merlot_gemm_debug_counters(void* buf_u64);
 
 #ifdef __cplusplus
 }

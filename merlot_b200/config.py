@@ -1,6 +1,6 @@
 """NeatConfig mirror (utils/neat_config.py:19-119): same YAML files, same sections, same error behaviour.
 
-The TPU RunConfig part (utils/neat_config.py:122-151) has no meaning on B200 and is dropped; `device.*` TPU keys are
+The TPU RunConfig part (utils/neat_config.py:122-151) has no meaning on a GPU and is dropped; `device.*` TPU keys are
 accepted and ignored.  File globs in `data.*_file` are expanded with the stdlib instead of tf.io.gfile.
 """
 from __future__ import annotations

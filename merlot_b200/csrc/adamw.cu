@@ -126,7 +126,7 @@ extern "C" int merlot_clip_by_global_norm(float* g, long long n, float clip_norm
   MB_REQUIRE(clip_norm > 0.f && ((uintptr_t)g % 16) == 0, MERLOT_EINVAL, "clip_by_global_norm: clip_norm must be > 0 and g 16-byte aligned");
   if (n <= 0) return MERLOT_OK;
   MB_CHECK_CUDA(cudaMemsetAsync(scratch_f64, 0, sizeof(double), st));
-  const int grid = 148 * 8;
+  const int grid = device_sms() * 8;
   sumsq_kernel<<<grid, 256, 0, st>>>(g, n, scratch_f64);
   MB_CHECK_LAUNCH();
   clip_scale_kernel<<<grid, 256, 0, st>>>(g, n, scratch_f64, clip_norm, norm_out);

@@ -1,71 +1,89 @@
-// K1 1-CTA kernel template and its launch dispatch; instantiated per tile width in gemm_bn{128,192,256}.cu so the three
-// widths compile in parallel (12 operand/epilogue combinations x 7 epilogue feature sets each).
+// K1 kernel template and its launch dispatch; instantiated per tile width in gemm_bn{128,192,256}.cu so the three widths
+// compile in parallel (4 operand-major combinations each).
 #pragma once
 #include "gemm_common.cuh"
 
 namespace mb {
 
-// EPI 1 (bf16 outputs) and EPI 2 (fp32 split-K accumulation) leave through the warp-private staged epilogue of
-// gemm_common.cuh, compiled for the feature set FL; EPI 0 = direct register->global stores (other fp32 outputs).
-template <int BN, bool A_MN, bool B_MN, int EPI, int FL>
+// Fused epilogue of one warp's [16 rows][64 columns] fp32 slot (float4 units XOR-swizzled by row): lane l handles the 8-column
+// groups l, l + 32, l + 64, l + 96 (row = group / 8), so 8 lanes cover one row's 256 contiguous bytes.  Inlined: a call would
+// have to save every live accumulator register around it.
+static __device__ __forceinline__ void gemm_epilogue_slot(const GemmDev& p, const float* slot, int row0, int col0, int lane) {
+#pragma unroll 1
+  for (int it = 0; it < 4; ++it) {
+    const int item = it * 32 + lane;
+    const int rr = item >> 3, g = item & 7;
+    const int row = row0 + rr, col = col0 + g * 8;
+    if (row >= p.M || col >= p.N) continue;
+    const float4 lo = *reinterpret_cast<const float4*>(slot + rr * 64 + (((2 * g) ^ rr) << 2));
+    const float4 hi = *reinterpret_cast<const float4*>(slot + rr * 64 + (((2 * g + 1) ^ rr) << 2));
+    float v[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w}, pre[8];
+    epi_math8(p, row, col, true, v, pre);
+    epi_store_direct(p, row, col, v, pre);
+  }
+}
+
+template <int BN>
+__device__ __forceinline__ void wgmma_tile(float (&acc)[BN / 2], uint64_t da, uint64_t db, uint32_t scale_d, bool a_mn, bool b_mn);
+
+#define MB_WGMMA_TILE(N)                                                                                                      \
+  template <>                                                                                                                 \
+  __device__ __forceinline__ void wgmma_tile<N>(float (&acc)[N / 2], uint64_t da, uint64_t db, uint32_t sd, bool a_mn, bool b_mn) { \
+    if (a_mn) {                                                                                                               \
+      if (b_mn) wgmma_m64n##N##_ss<1, 1>(acc, da, db, sd); else wgmma_m64n##N##_ss<1, 0>(acc, da, db, sd);                    \
+    } else {                                                                                                                  \
+      if (b_mn) wgmma_m64n##N##_ss<0, 1>(acc, da, db, sd); else wgmma_m64n##N##_ss<0, 0>(acc, da, db, sd);                    \
+    }                                                                                                                         \
+  }
+MB_WGMMA_TILE(128)
+MB_WGMMA_TILE(192)
+MB_WGMMA_TILE(256)
+#undef MB_WGMMA_TILE
+
+// Persistent, warp-specialised bf16 GEMM (static tile schedule, split-K for the wgrad orientation):
+//   warp 0 (one elected lane): TMA producer -- A/B tiles -> 128B-swizzled smem ring of STAGES stages; it runs ahead across
+//                              tiles, so the loads of tile i+1 overlap the epilogue of tile i;
+//   warpgroups 1, 2:           rows [0, 64) / [64, 128) of the tile: m64 x BN x 16 wgmma with fp32 accumulators in registers,
+//                              one k-block in flight behind the one being issued, then the fused epilogue.
+template <int BN, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const GemmDev p) {
-  using Cfg = GemmCfg<BN, EPI>;
-  constexpr bool TS = EPI != 0;
+  using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   // 128B swizzle atoms need 1024-byte alignment
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * Cfg::A_BYTES;
-  uint8_t* staging = smem + STAGES * Cfg::STAGE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + (TS ? STAGING_BYTES : 0));
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + STAGES;
-  uint64_t* tmem_full = bars + 2 * STAGES;
-  uint64_t* tmem_empty = bars + 2 * STAGES + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-  float* bias_slots = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);
+  float* staging = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES + STAGING_BYTES);
+  uint64_t* empty_bar = full_bar + STAGES;
 
-  // warp index through a shuffle = provably warp-uniform, single issuing lane through elect.sync, TMEM base through a shuffle:
-  // with anything less ptxas wraps every tcgen05.mma / TMA instruction in a per-lane ELECT / BRA.U.ANY loop (measured with
-  // tools/micro/mma_bench*.cu: 119 -> 32..128 cycles per MMA, i.e. the 128 x 256 x 16 MMA ran at 167 instead of 128 cycles)
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);  // provably warp-uniform
   const int lane = threadIdx.x & 31;
-  const bool leader = elect_one();
   pdl_launch_dependents();
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tma_a);
     tma_prefetch_desc(&tma_b);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tmem_full[s], 1);
-      mbar_init(&tmem_empty[s], EPI_WARPS);  // one arrival per epilogue warp
+      mbar_init(&empty_bar[s], 2);  // one arrival per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_ptr_smem, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_ptr_smem, 0);
   pdl_wait();  // everything above overlapped the previous kernel's tail
 
   const int num_tiles = p.m_blocks * p.n_blocks * p.splits;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================== TMA producer =====================
-    if (leader) {
+    // the producer warpgroup hands registers to the consumers (40 + 2 x 232 per thread x 128 <= 64 K)
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+    if (warp == 0 && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
-      long long w_empty = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int split = tile % p.splits;
         const int mn = tile / p.splits;
@@ -74,9 +92,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
         const int kb0 = split * p.kb_per_split;
         const int kb1 = min(p.num_kb, kb0 + p.kb_per_split);
         for (int kb = kb0; kb < kb1; ++kb) {
-          const long long t0 = p.dbg ? clock64() : 0;
           mbar_wait(&empty_bar[stage], phase ^ 1);
-          if (p.dbg) w_empty += clock64() - t0;
           mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
           uint8_t* sa = smem_a + stage * Cfg::A_BYTES;
           uint8_t* sb = smem_b + stage * Cfg::B_BYTES;
@@ -97,131 +113,71 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
-      if (p.dbg) p.dbg[blockIdx.x * 8 + 3] = (unsigned long long)w_empty;
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (leader) {
-      constexpr uint32_t idesc = make_idesc_bf16(BLOCK_M, BN, A_MN ? 1 : 0, B_MN ? 1 : 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      long long w_full = 0, w_tempty = 0, ntiles = 0;
-      const long long t_begin = p.dbg ? clock64() : 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int split = tile % p.splits;
-        const int kb0 = split * p.kb_per_split;
-        const int kb1 = min(p.num_kb, kb0 + p.kb_per_split);
-        long long t0 = p.dbg ? clock64() : 0;
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);  // epilogue has drained this accumulator stage
-        if (p.dbg) { w_tempty += clock64() - t0; ++ntiles; }
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * BN;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          t0 = p.dbg ? clock64() : 0;
-          mbar_wait(&full_bar[stage], phase);
-          if (p.dbg) w_full += clock64() - t0;
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem_a + stage * Cfg::A_BYTES);
-          const uint32_t b_addr = smem_u32(smem_b + stage * Cfg::B_BYTES);
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / 16; ++k) {
-            const uint64_t da = A_MN ? desc_mnmajor(a_addr, k, BLOCK_K * 128) : desc_kmajor(a_addr, k);
-            const uint64_t db = B_MN ? desc_mnmajor(b_addr, k, BLOCK_K * 128) : desc_kmajor(b_addr, k);
-            umma_bf16_ss(tmem_d, da, db, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);  // frees the smem slot once these MMAs have read it
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tmem_full[acc]);  // accumulator complete -> epilogue
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-      if (p.dbg) {
-        unsigned long long* d = p.dbg + blockIdx.x * 8;
-        d[0] = (unsigned long long)(clock64() - t_begin); d[1] = (unsigned long long)w_full;
-        d[2] = (unsigned long long)w_tempty; d[7] = (unsigned long long)ntiles;
-      }
     }
   } else {
-    // ===================== epilogue warps (2 .. 2+EPI_WARPS) =====================
-    const int e = warp - 2;
-    const int quad = warp & 3;          // TMEM lane window this warp may touch: lanes [32*quad, 32*quad+32)
-    const int half = e >> 2;            // which half of the tile's columns this warp owns
-    const int row_in_tile = quad * 32 + lane;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    const int rtf = FL == F_GENERIC ? epi_features(p) : FL;
-    long long w_tfull = 0, w_stage = 0, w_work = 0;
-    const bool dbg = p.dbg != nullptr && e == 0 && lane == 0;
-    EpiCarry cy;
+    // ===================== consumer warpgroups =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+    const int wg = (warp - 4) >> 2;  // rows [64 wg, 64 wg + 64) of the tile
+    const int wq = warp & 3;         // 16-row slice of this warp inside the warpgroup's 64 rows
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    float* slot = staging + (warp - 4) * 1024;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int stage = 0;
+    uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int split = tile % p.splits;
       const int mn = tile / p.splits;
       const int n_blk = mn % p.n_blocks;
       const int m_blk = mn / p.n_blocks;
-      const int row = m_blk * BLOCK_M + row_in_tile;
-      const bool in_range = row < p.M;
-      long long t0 = dbg ? clock64() : 0;
-      if (EPI != 0) epilogue_prefetch<BN, EPI, FL>(p, rtf, m_blk * BLOCK_M + quad * 32, n_blk * BN, half, lane, cy);  // hidden by the wait
-      mbar_wait(&tmem_full[acc], acc_phase);
-      if (dbg) { const long long t1 = clock64(); w_tfull += t1 - t0; t0 = t1; }
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + acc * BN + ((uint32_t)(quad * 32) << 16);
-      if (!TS) {
-        constexpr int CH = BN / 64;  // 32-column chunks per warp
-#pragma unroll 1
-        for (int c = 0; c < CH; ++c) {
-          uint32_t r[32];
-          const int tcol = half * (BN / 2) + c * 32;
-          tmem_ld_32x32(taddr + tcol, r);
-          tmem_wait_ld();
-          const int col0 = n_blk * BN + tcol;
-          if (in_range && col0 < p.N) {
+      const int kb0 = split * p.kb_per_split;
+      const int kb1 = min(p.num_kb, kb0 + p.kb_per_split);
+      int prev = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t a_addr = smem_u32(smem_a + stage * Cfg::A_BYTES) + (uint32_t)wg * (A_MN ? BLOCK_K * 128 : 64 * 128);
+        const uint32_t b_addr = smem_u32(smem_b + stage * Cfg::B_BYTES);
+        wgmma_fence();
 #pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              const int col = col0 + g * 8;
-              if (col < p.N) {
-                float v[8], pre[8];
-#pragma unroll
-                for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[g * 8 + i]);
-                epi_math8(p, row, col, true, v, pre);
-                epi_store_direct(p, row, col, v, pre);
-              }
-            }
-          }
+        for (int k = 0; k < BLOCK_K / 16; ++k) {
+          const uint64_t da = A_MN ? desc_mnmajor(a_addr, k, BLOCK_K * 128) : desc_kmajor(a_addr, k);
+          const uint64_t db = B_MN ? desc_mnmajor(b_addr, k, BLOCK_K * 128) : desc_kmajor(b_addr, k);
+          wgmma_tile<BN>(acc, da, db, (kb > kb0 || k > 0) ? 1u : 0u, A_MN, B_MN);
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      } else {
-        epilogue_tile_loop<BN, EPI, FL>(p, rtf, staging + e * 4096, bias_slots + e * 32, taddr, m_blk * BLOCK_M + quad * 32, n_blk * BN, half,
-                                      lane, cy, [&] {
-                                        tc_fence_before();
-                                        __syncwarp();
-                                        if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-                                      });
+        wgmma_commit();
+        wgmma_wait<1>();  // the k-block before this one has been read: its stage goes back to the producer
+        if (prev >= 0 && wg_leader) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-      if (dbg) w_work += clock64() - t0;
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      wgmma_wait<0>();
+      reg_fence(acc);
+      if (prev >= 0 && wg_leader) mbar_arrive(&empty_bar[prev]);
+      // ---- epilogue: 64-column chunks through the warp's slot ----
+      const int row0 = m_blk * BLOCK_M + wg * 64 + wq * 16;
+      const int r = lane >> 2;
+#pragma unroll
+      for (int c = 0; c < BN / 64; ++c) {
+        __syncwarp();
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int j = c * 8 + jj;
+          const int unit = jj * 2 + ((lane & 3) >> 1), within = (lane & 1) * 2;
+          *reinterpret_cast<float2*>(slot + r * 64 + ((unit ^ r) << 2) + within) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(slot + (r + 8) * 64 + ((unit ^ (r + 8)) << 2) + within) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+        __syncwarp();
+        if (n_blk * BN + c * 64 < p.N) gemm_epilogue_slot(p, slot, row0, n_blk * BN + c * 64, lane);
+      }
     }
-    if (dbg) {
-      unsigned long long* d = p.dbg + blockIdx.x * 8;
-      d[4] = (unsigned long long)w_tfull; d[5] = (unsigned long long)w_stage; d[6] = (unsigned long long)w_work;
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
   }
 }
 
-template <int BN, bool A_MN, bool B_MN, int EPI, int FL>
+template <int BN, bool A_MN, bool B_MN>
 static int launch_gemm_inst(const CUtensorMap& ta, const CUtensorMap& tb, const GemmDev& p, int grid, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN, EPI>;
-  auto kern = gemm_bf16_kernel<BN, A_MN, B_MN, EPI, FL>;
+  using Cfg = GemmCfg<BN>;
+  auto kern = gemm_bf16_kernel<BN, A_MN, B_MN>;
   static bool attr_set = false;  // per instantiation
   if (!attr_set) {
     MB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_TOTAL));
@@ -234,40 +190,12 @@ static int launch_gemm_inst(const CUtensorMap& ta, const CUtensorMap& tb, const 
   return MERLOT_OK;
 }
 
-
-// Feature sets with a dedicated epilogue instance (everything else runs the generic, run-time-flag instance).
-__host__ inline int epi_specialised(int fl) {
-  switch (fl) {
-    case 0: case F_BIAS: case F_BIAS | F_GELU | F_DUAL: case F_BIAS | F_GELU | F_DUAL | F_GRADOUT: case F_MULAUX: case F_DGELU: case F_BIAS | F_RESID | F_DROP: case F_BIAS | F_RESID: case F_RESID: return fl;
-    default: return F_GENERIC;
-  }
-}
-
-template <int BN, bool A_MN, bool B_MN>
-static int launch_gemm_mn(int epi, int fl, const CUtensorMap& ta, const CUtensorMap& tb, const GemmDev& p, int grid, cudaStream_t stream) {
-  if (epi == 0) return launch_gemm_inst<BN, A_MN, B_MN, 0, F_GENERIC>(ta, tb, p, grid, stream);
-  if (epi == 2) return launch_gemm_inst<BN, A_MN, B_MN, 2, F_ALPHA>(ta, tb, p, grid, stream);
-  switch (epi_specialised(fl)) {
-    case 0: return launch_gemm_inst<BN, A_MN, B_MN, 1, 0>(ta, tb, p, grid, stream);
-    case F_BIAS: return launch_gemm_inst<BN, A_MN, B_MN, 1, F_BIAS>(ta, tb, p, grid, stream);
-    case F_BIAS | F_GELU | F_DUAL: return launch_gemm_inst<BN, A_MN, B_MN, 1, F_BIAS | F_GELU | F_DUAL>(ta, tb, p, grid, stream);
-    case F_DGELU: return launch_gemm_inst<BN, A_MN, B_MN, 1, F_DGELU>(ta, tb, p, grid, stream);
-    case F_BIAS | F_GELU | F_DUAL | F_GRADOUT: return launch_gemm_inst<BN, A_MN, B_MN, 1, F_BIAS | F_GELU | F_DUAL | F_GRADOUT>(ta, tb, p, grid, stream);
-    case F_MULAUX: return launch_gemm_inst<BN, A_MN, B_MN, 1, F_MULAUX>(ta, tb, p, grid, stream);
-    case F_BIAS | F_RESID: return launch_gemm_inst<BN, A_MN, B_MN, 1, F_BIAS | F_RESID>(ta, tb, p, grid, stream);
-    case F_BIAS | F_RESID | F_DROP: return launch_gemm_inst<BN, A_MN, B_MN, 1, F_BIAS | F_RESID | F_DROP>(ta, tb, p, grid, stream);
-    case F_RESID: return launch_gemm_inst<BN, A_MN, B_MN, 1, F_RESID>(ta, tb, p, grid, stream);
-    default: return launch_gemm_inst<BN, A_MN, B_MN, 1, F_GENERIC>(ta, tb, p, grid, stream);
-  }
-}
-
 template <int BN>
-int launch_gemm_bn(bool a_mn, bool b_mn, int epi, int fl, const CUtensorMap& ta, const CUtensorMap& tb, const GemmDev& p, int grid,
-                   cudaStream_t stream) {
-  if (a_mn && b_mn) return launch_gemm_mn<BN, true, true>(epi, fl, ta, tb, p, grid, stream);
-  if (!a_mn && b_mn) return launch_gemm_mn<BN, false, true>(epi, fl, ta, tb, p, grid, stream);
-  if (!a_mn && !b_mn) return launch_gemm_mn<BN, false, false>(epi, fl, ta, tb, p, grid, stream);
-  return launch_gemm_mn<BN, true, false>(epi, fl, ta, tb, p, grid, stream);
+int launch_gemm_bn(bool a_mn, bool b_mn, const CUtensorMap& ta, const CUtensorMap& tb, const GemmDev& p, int grid, cudaStream_t stream) {
+  if (a_mn && b_mn) return launch_gemm_inst<BN, true, true>(ta, tb, p, grid, stream);
+  if (!a_mn && b_mn) return launch_gemm_inst<BN, false, true>(ta, tb, p, grid, stream);
+  if (!a_mn && !b_mn) return launch_gemm_inst<BN, false, false>(ta, tb, p, grid, stream);
+  return launch_gemm_inst<BN, true, false>(ta, tb, p, grid, stream);
 }
 
 }  // namespace mb

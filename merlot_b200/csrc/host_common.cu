@@ -27,13 +27,19 @@ static std::atomic<int> g_sm_reserve{0};
 // SMs the persistent kernels (K1, K3) may fill.  With data parallelism NCCL's collective CTAs each occupy a whole SM for
 // milliseconds; a persistent kernel launched with one CTA per SM then has CTAs that cannot start until others have finished
 // and, with a static tile schedule, takes up to twice as long.  merlot_set_sm_reserve(n) leaves n SMs to the collective.
-int num_sms() {
+// SMs of the current device (132 on an H100 SXM), independent of the reserve below: for workspace sizes and fixed grids.
+int device_sms() {
   static int sms = 0;
   if (sms == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
   }
+  return sms;
+}
+
+int num_sms() {
+  const int sms = device_sms();
   const int r = g_sm_reserve.load(std::memory_order_relaxed);
   return (r > 0 && r < sms - 8) ? sms - r : sms;
 }

@@ -46,7 +46,8 @@ int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64
 int make_tmap_bf16_3d(CUtensorMap* out, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t ld1,
                       uint64_t ld2, uint32_t b0, uint32_t b1, uint32_t b2);
 
-int num_sms();
+int device_sms();  // SMs of the device
+int num_sms();     // SMs the persistent kernels may fill (device_sms() minus merlot_set_sm_reserve)
 
 // Launch with the programmatic-stream-serialization attribute (PDL). Kernels launched this way MUST call pdl_wait()
 // before their first global-memory access.

@@ -660,7 +660,7 @@ extern "C" int merlot_layernorm_fwd(const merlot_ln_t* d, void* stream_) {
   return MERLOT_OK;
 }
 
-extern "C" size_t merlot_layernorm_bwd_workspace_bytes(int H) { return (size_t)4 * 148 * 3 * (size_t)H * sizeof(float); }
+extern "C" size_t merlot_layernorm_bwd_workspace_bytes(int H) { return (size_t)4 * device_sms() * 3 * (size_t)H * sizeof(float); }
 
 extern "C" int merlot_layernorm_bwd(const merlot_ln_bwd_t* d, void* stream_) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
@@ -671,7 +671,8 @@ extern "C" int merlot_layernorm_bwd(const merlot_ln_bwd_t* d, void* stream_) {
   const uint32_t th = d->dropout_p > 0.f ? thresh16(d->dropout_p) : 0;
   const float sc = d->dropout_p > 0.f ? 1.f / (1.f - d->dropout_p) : 1.f;
   long long want = ceil_div_ll(d->rows, 8);
-  const int grid = (int)(want < 2 * 148 ? want : 2 * 148);
+  const int max_grid = 2 * device_sms();  // the workspace holds 2H partials per block for this many blocks (and more)
+  const int grid = (int)(want < max_grid ? want : max_grid);
   const size_t smem = (size_t)2 * d->H * sizeof(float);
   float* part = reinterpret_cast<float*>(d->workspace);
 #define LNB(TX, TDY, TDX)                                                                                                         \

@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's `MerlotModel` (model/modeling.py:47-668) over the sm_100a C-ABI.
+"""Host-side mirror of the reference's `MerlotModel` (model/modeling.py:47-668) over the sm_90a C-ABI.
 
 Same constructor arguments, attributes and methods as the reference class, so `model_fn`-style callers
 (model/modeling.py:691-713, downstream/sort_story/get_zero_shot_logits.py:58-79) read the same.  Construction *is* the

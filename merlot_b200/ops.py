@@ -31,7 +31,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn_major: bool = False, b_mn_maj
          alpha: float = 1.0, atomic: bool = False, dropout_p: float = 0.0, dropout_seed: int = 0,
          dropout_site: int = 0, splits: int = 0, block_n: int = 0,
          M: Optional[int] = None, N: Optional[int] = None, K: Optional[int] = None) -> torch.Tensor:
-    """C[M,N] = epilogue(alpha * A @ B^T) on tcgen05 tensor cores (see include/merlot_b200.h, K1).
+    """C[M,N] = epilogue(alpha * A @ B^T) on wgmma tensor cores (see include/merlot_b200.h, K1).
 
     a: [M,K] (or [K,M] when a_mn_major); b: [N,K] (or [K,N] when b_mn_major); both bf16, row-major, 2-D.
     With gelu=True and out_pre given: out_pre <- pre-activation, return value <- gelu(pre).

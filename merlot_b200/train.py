@@ -209,7 +209,7 @@ def model_fn_builder(config: NeatConfig, *, store: Optional[ParamStore] = None, 
 
 def main(argv=None):
     """`python -m merlot_b200.train configs/merlot.yaml` -- the role of model/train.py:9-26 on synthetic data."""
-    config = NeatConfig.from_args("Train MERLOT (B200-native)", argv=argv)
+    config = NeatConfig.from_args("Train MERLOT (H100-native)", argv=argv)
     dist = DataParallel() if int(os.environ.get("WORLD_SIZE", "1")) > 1 else None
     if torch.cuda.is_available():
         torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))

@@ -67,7 +67,7 @@ def test_bench_reference_arm_prints_the_contract_line():
 
 def test_pairwise_partner_words_equal_the_reference_mask():
     """disable_pairwise_lang_attn (model/modeling.py:160-168): the attention kernels never see an [S, S] mask -- every row
-    derives its partners as two bit ranges per 32-position word (csrc/attention_tcgen05.cu: span_word / pair_lo_of / pair_word).
+    derives its partners as two bit ranges per 32-position word (csrc/attention.cu: span_word / pair_lo_of / pair_word).
     The same integer arithmetic restated here must reproduce the reference's segment_idx construction bit for bit, for chunk
     lengths that are not word-aligned, P = 0, single-token chunks, and the 16-bit extraction K3 uses."""
     def span_word(x0, a, b):

@@ -50,7 +50,7 @@ t("FFN2-dgrad x gelu'(pre)", lambda: ops.gemm(x, w2, out=oi, dgelu_aux=oi2, M=M,
 t("FFN1-dgrad plain (N=768,K=3072)", lambda: ops.gemm(xi, w1, out=oh, M=M, N=H, K=I), 2.0 * M * I * H)
 t("QKV-dgrad plain (N=768,K=2304)", lambda: ops.gemm(oqkv, wqkv, out=oh, M=M, N=H, K=3 * H), 2.0 * M * 3 * H * H)
 
-# 256 x 192 CTA-pair tile vs the 1-CTA 192 tile on the N = 768 dgrads (K-major weights)
+# tile widths on the N = 768 dgrads (K-major weights)
 for name, A, W, K_ in (("FFN1-dgrad K=3072", xi, w1, I), ("QKV-dgrad K=2304", oqkv, wqkv, 3 * H), ("out-proj dgrad K=768", x, wo, H)):
-    for bn in (192, -192):
+    for bn in (128, 192, 256):
         t(f"{name} block_n={bn}", lambda: ops.gemm(A, W, out=oh, M=M, N=H, K=K_, block_n=bn), 2.0 * M * H * K_)
