@@ -250,11 +250,13 @@ def dropout_apply(x, y, p, seed, site):
     return y
 
 
-def bias_grad(dy, out, rows=None, N=None):
+def bias_grad(dy, out, rows=None, N=None, dropout=(0.0, 0, 0)):
+    """out[n] += sum_m dy[m, n]; with dropout=(p, seed, site), dy first goes through that forward dropout mask."""
     N = out.numel() if N is None else N
     rows = dy.numel() // dy.stride(-2) if rows is None else rows
+    p, seed, site = dropout
     L.check(L.lib().merlot_bias_grad(C.c_void_p(dy.data_ptr()), _f32(dy), dy.stride(-2), C.c_longlong(rows), N,
-                                     C.c_void_p(out.data_ptr()), C.c_float(0.0), C.c_uint64(0), C.c_uint32(0), _stream()))
+                                     C.c_void_p(out.data_ptr()), C.c_float(p), C.c_uint64(seed), C.c_uint32(site), _stream()))
 
 
 def gather_rows(src, idx, dst, n=None, H=None):

@@ -119,9 +119,18 @@ def mlp_block(x, p: Params, scope: str):
     return dense(dense(x, p, f"{scope}/intermediate", gelu), p, f"{scope}/output")
 
 
-def transformer(hidden, mask, p: Params, scope: str, num_layers: int, heads: int, return_attn_probs=False):
-    """utils/transformer.py:171-247, pre-LN, dropout 0.  hidden [B,S,H]; mask [B,S,S].
-    self_attn_probs (if requested) is the head-MEAN, stacked over layers: [B, layers, S, S] (:208-209,238)."""
+def _scoped(dropout, name):
+    """The dropout hook of one stack: the stack's keys (layer, kind) become (name, layer, kind)."""
+    if dropout is None:
+        return None
+    return lambda key, x: dropout((name,) + tuple(key), x)
+
+
+def transformer(hidden, mask, p: Params, scope: str, num_layers: int, heads: int, return_attn_probs=False, dropout=None):
+    """utils/transformer.py:171-247, pre-LN.  hidden [B,S,H]; mask [B,S,S].
+    self_attn_probs (if requested) is the head-MEAN, stacked over layers: [B, layers, S, S] (:208-209,238).
+    dropout: None (dropout 0) or a callable dropout(key, x [B*S, H]) applied to the projected context, bias included
+    (:136, key (layer, "attn")) and to the FFN output (:162, key (layer, "ffn")), each before its residual add."""
     B, S, H = hidden.shape
     h = hidden.reshape(B * S, H)
     probs_all = []
@@ -130,8 +139,13 @@ def transformer(hidden, mask, p: Params, scope: str, num_layers: int, heads: int
         a, probs = attention_layer(layer_norm(h, p, f"{ls}/LayerNorm_attn_ln0"), mask, B, S, heads, p, ls)
         if return_attn_probs:
             probs_all.append(probs.mean(1))
+        if dropout is not None:
+            a = dropout((l, "attn"), a)
         h = h + a
-        h = h + mlp_block(layer_norm(h, p, f"{ls}/LayerNorm_mlp_ln0"), p, ls)
+        f = mlp_block(layer_norm(h, p, f"{ls}/LayerNorm_mlp_ln0"), p, ls)
+        if dropout is not None:
+            f = dropout((l, "ffn"), f)
+        h = h + f
     h = layer_norm(h, p, f"{scope}/LayerNorm_ln_final")
     out = {"_hidden_state_flat": h, "hidden_state": h.reshape(B, S, H)}
     if return_attn_probs:
@@ -285,7 +299,9 @@ def resnet_param_shapes(scope: str, layers, width: int = 64, hidden_size: int = 
 # ------------------------------------------------------------------------------------------------------------
 # ViT backbone (utils/vision_transformer.py:173-274): patch-embed stem (resnet_layers == []) or the hybrid stem
 # ------------------------------------------------------------------------------------------------------------
-def vision_transformer_backbone(image: torch.Tensor, cfg: dict, p: Params):
+def vision_transformer_backbone(image: torch.Tensor, cfg: dict, p: Params, dropout=None):
+    """dropout: None or the model's dropout hook; the ViT stack calls it with keys ("vit", layer, "attn" | "ffn").  The hook
+    applies vit_hidden_dropout_prob there when the config sets it (:243-244)."""
     P = cfg["patch_size"]
     H = cfg["hidden_size"]
     num_cls = cfg.get("num_cls_emb", 2)
@@ -312,7 +328,7 @@ def vision_transformer_backbone(image: torch.Tensor, cfg: dict, p: Params):
     S = h1 * w1 + num_cls
     mask = torch.ones(n, S, S, dtype=x.dtype)  # :239
     info = transformer(x, mask, p, scope, cfg.get("num_vision_transformer_hidden_layers", cfg["num_hidden_layers"]),
-                       cfg["num_attention_heads"])
+                       cfg["num_attention_heads"], dropout=_scoped(dropout, "vit"))
     info["cls"] = info["hidden_state"][:, :num_cls]
     seq = info["hidden_state"][:, num_cls:]
     sp = cfg["spatial_pool_size"]
@@ -399,15 +415,18 @@ def mask_inputs(input_ids_2d: torch.Tensor, attention_summs: Optional[torch.Tens
 # MerlotModel (model/modeling.py:47-668)
 # ------------------------------------------------------------------------------------------------------------
 class MerlotOracle:
-    """Functional mirror of MerlotModel.__init__ + loss heads, dropout 0, single replica, fp32 (or fp64) throughout.
+    """Functional mirror of MerlotModel.__init__ + loss heads, single replica, fp32 (or fp64) throughout.
 
     image: [batch*num_chunks, h, w, 3] float in [0,1]; input_ids: int [batch, num_chunks, Lc] or [batch, Lc].
     mask_draws: dict from make_mask_draws (required when mask_input=True) or
     mask_override: {'masked_ids','masked_idx'} to bypass mask selection (used to feed the GPU-chosen mask).
+    dropout: None (dropout 0, the eval model) or a callable dropout(key, x [rows, H]) -> x, applied wherever the reference
+    applies hidden dropout: keys ("vit" | "langonly" | "joint", layer, "attn" | "ffn") inside the three stacks and
+    ("embed", "langonly" | "joint") after the two embedding LayerNorms (oracle/dropout_mask.py builds the training one).
     """
 
     def __init__(self, config: dict, params: Params, image, input_ids, mask_input=False, shuffled_idx_img=None,
-                 mask_draws=None, mask_override=None, log_attention_probs=True):
+                 mask_draws=None, mask_override=None, log_attention_probs=True, dropout=None):
         self.config = copy.deepcopy(config)
         self.p = params
         cfg = self.config
@@ -430,7 +449,7 @@ class MerlotOracle:
         dt = image.dtype
 
         # ---- vision backbone (:95-133) ----
-        self.vision_transformer_info = vit = vision_transformer_backbone(image, cfg, params)
+        self.vision_transformer_info = vit = vision_transformer_backbone(image, cfg, params, dropout)
         self.img_trg_h = vit["cls"][:, 1]  # :99
         feats = torch.cat([vit["cls"][:, 0, None], vit["seq"]], 1)  # :101-104
         self.viz_chunk_length = vit["num_h"] * vit["num_w"] + 1
@@ -445,7 +464,7 @@ class MerlotOracle:
 
         # ---- language side ----
         if mask_input:  # :135-139
-            self.lang_trg_h, self.lang_transformer_info = self.langonly_reps()
+            self.lang_trg_h, self.lang_transformer_info = self.langonly_reps(dropout)
             if mask_override is not None:
                 self.lang_mask_info = {k: torch.as_tensor(v) for k, v in mask_override.items()}
             else:
@@ -457,7 +476,7 @@ class MerlotOracle:
         else:
             ids_to_use = self.input_ids
         ids_to_use = ids_to_use.reshape(self.B, self.L)  # :143
-        pieces.append({"name": "lang", "x": self.embed_words(ids_to_use), "is_valid": ids_to_use != 0})  # :145-149
+        pieces.append({"name": "lang", "x": self.embed_words(ids_to_use, dropout=dropout), "is_valid": ids_to_use != 0})  # :145-149
 
         enc_in = torch.cat([x["x"] for x in pieces], 1)  # :151
         is_valid = torch.cat([x["is_valid"] for x in pieces], 1)  # :152
@@ -470,7 +489,8 @@ class MerlotOracle:
             attn_mask = attn_mask & can_attend[None]
         attn_mask = attn_mask.to(dt)  # :170
         self.encoder_info = transformer(enc_in, attn_mask, params, "encoder", cfg["num_hidden_layers"],
-                                        cfg["num_attention_heads"], return_attn_probs=log_attention_probs)  # :171-174
+                                        cfg["num_attention_heads"], return_attn_probs=log_attention_probs,
+                                        dropout=_scoped(dropout, "joint"))  # :171-174
         self.encoder_hidden_states = {}
         cur = 0
         for x in pieces:  # :176-184
@@ -504,15 +524,20 @@ class MerlotOracle:
     def P(self):
         return self.viz_chunk_length * self.num_chunks_in_group
 
-    def embed_words(self, ids_2d, norm_scope_name="position_embeddings"):
-        """:262-297 -- E[ids] + Pos[0:L] -> LN embed_norm (dropout 0)."""
+    def embed_words(self, ids_2d, norm_scope_name="position_embeddings", dropout=None):
+        """:262-297 -- E[ids] + Pos[0:L] -> LN embed_norm -> dropout (:294; key ("embed", "joint") for position_embeddings,
+        ("embed", "langonly") for langonly_embeddings, on the [B*L, H] rows)."""
         p = self.p
         L = ids_2d.shape[1]
         assert L <= self.config["max_position_embeddings"]  # model_utils.py:282
         assert int(ids_2d.min()) >= 0 and int(ids_2d.max()) <= self.vocab_size - 1  # model_utils.py:256-257
         emb = p["word_embeddings/word_embeddings"][ids_2d.long()]
         pos = p[f"{norm_scope_name}/position_embeddings"][:L][None]
-        return layer_norm(emb + pos, p, f"{norm_scope_name}/LayerNorm_embed_norm")
+        y = layer_norm(emb + pos, p, f"{norm_scope_name}/LayerNorm_embed_norm")
+        if dropout is not None:
+            name = {"position_embeddings": "joint", "langonly_embeddings": "langonly"}[norm_scope_name]
+            y = dropout(("embed", name), y.reshape(-1, y.shape[-1])).reshape(y.shape)
+        return y
 
     def vision_pos_emb(self, shuffled_idx_img=None):
         """:299-337."""
@@ -528,8 +553,8 @@ class MerlotOracle:
                                    self.vision_transformer_info["num_w"], 1)  # :327-335
         return my_pe + pe2d.repeat(n, 1)[None]  # :336
 
-    def langonly_reps(self):
-        """:339-379."""
+    def langonly_reps(self, dropout=None):
+        """:339-379.  dropout: None or the model's dropout hook (keys ("embed", "langonly") and ("langonly", layer, kind))."""
         cfg = self.config
         if "langonly_num_chunks_in_group" in cfg:
             g = cfg["langonly_num_chunks_in_group"]
@@ -538,11 +563,11 @@ class MerlotOracle:
             ids = self.input_ids.reshape(self.batch_size * ng, self.lang_chunk_length * g)
         else:
             ids = self.input_ids.reshape(self.batch_size, self.lang_chunk_length * self.num_chunks)
-        emb = self.embed_words(ids, "langonly_embeddings")
+        emb = self.embed_words(ids, "langonly_embeddings", dropout)
         valid = ids != 0
         mask = (valid[:, None] & valid[:, :, None]).to(emb.dtype)
         info = transformer(emb, mask, self.p, "encoder", cfg["num_lang_transformer_hidden_layers"],
-                           cfg["num_attention_heads"], return_attn_probs=True)
+                           cfg["num_attention_heads"], return_attn_probs=True, dropout=_scoped(dropout, "langonly"))
         pool = info["_hidden_state_flat"].reshape(self.batch_size * self.num_chunks, self.lang_chunk_length, -1)[:, 0]
         return pool, info
 

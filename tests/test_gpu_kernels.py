@@ -2,10 +2,13 @@
 seeded inputs, through the C-ABI.  Tolerances: bit-exact for integer/index work and the packed bf16 Adam moments;
 bf16 tensor-core outputs compared in relative Frobenius norm against the fp32 oracle evaluated on the SAME bf16-rounded
 inputs (GEMM fp32-out 1e-4; bf16-out / attention 1e-2 -- one bf16 rounding is 2^-9 = 2e-3 per element)."""
+import itertools
+
 import numpy as np
 import pytest
 import torch
 
+from oracle import dropout_mask as DM
 from oracle import merlot_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -16,6 +19,11 @@ DEV = "cuda"
 def rel(a, b):
     a, b = a.detach().float().cpu(), b.detach().float().cpu()
     return ((a - b).norm() / (b.norm() + 1e-30)).item()
+
+
+def keep_ref(seed, site, rows, N, p):
+    """float {0, 1} [rows, N]: the restated counter-based dropout mask (oracle/dropout_mask.py)."""
+    return torch.from_numpy(DM.counter_dropout_keep(seed, site, rows, N, p)).float()
 
 
 @pytest.fixture(scope="module")
@@ -248,11 +256,13 @@ def test_layernorm_fwd_bwd(ops, rows, H):
 
 
 @pytest.mark.parametrize("rows,H,with_dres,p", [(1, 768, True, 0.1), (13, 64, False, 0.0), (1777, 768, True, 0.1), (8512, 768, True, 0.1),
-                                                  (8512, 768, False, 0.0), (5000, 1024, True, 0.1), (20000, 256, True, 0.0), (3, 512, True, 0.1)])
+                                                  (8512, 768, False, 0.0), (5000, 1024, True, 0.1), (20000, 256, True, 0.0), (3, 512, True, 0.1),
+                                                  (1031, 256, True, 0.5), (640, 768, False, 0.2)])
 def test_layernorm_bwd_fused(ops, rows, H, with_dres, p):
     """The stacks' fused LayerNorm backward (rows arrive through per-warp bulk-copy rings): every output against the fp32 graph
-    of utils/model_utils.py:113-130, the dropout mask against merlot_dropout_apply, the bias gradient against the exact column
-    sums of what the kernel wrote; row counts that leave warps without rows, with one row, and with many ring refills."""
+    of utils/model_utils.py:113-130, the dropout mask against merlot_dropout_apply and against the restated mask bit for bit,
+    the bias gradient against the exact column sums of what the kernel wrote; row counts that leave warps without rows, with
+    one row, and with many ring refills."""
     g = torch.Generator().manual_seed(rows + H)
     x = (torch.randn(rows, H, generator=g) * 2 + 0.5).bfloat16()
     gam = torch.randn(H, generator=g)
@@ -266,17 +276,20 @@ def test_layernorm_bwd_fused(ops, rows, H, with_dres, p):
     dx = torch.full((rows, H), float("nan"), dtype=torch.bfloat16, device=DEV)
     dmask = torch.full((rows, H), float("nan"), dtype=torch.bfloat16, device=DEV)
     dg, db, dbias = torch.zeros(H, device=DEV), torch.zeros(H, device=DEV), torch.zeros(H, device=DEV)
+    seed, site = (2 ** 40 + 3, 223) if rows % 2 else (7, 3)  # odd row counts: a seed with a non-zero high key word
     for rep in range(2):  # twice: the accumulators add up, the ring barriers start fresh every launch
         ops.layernorm_bwd_fused(dy.to(DEV), x.to(DEV), mu.to(DEV), rs.to(DEV), gam.to(DEV), dx, dg, db,
-                                dres=None if dres is None else dres.to(DEV), dmask=dmask, dbias=dbias, dropout=(p, 7, 3))
+                                dres=None if dres is None else dres.to(DEV), dmask=dmask, dbias=dbias, dropout=(p, seed, site))
     want = xr.grad + (dres.float() if with_dres else 0.0)
     assert torch.isfinite(dx.float()).all()
     assert rel(dx, want) < 6e-3
     assert rel(dg, 2 * gr.grad) < 2e-3 and rel(db, 2 * br.grad) < 2e-3
     if p > 0:
         ref_mask = torch.empty_like(dx)
-        ops.dropout_apply(dx, ref_mask, p, 7, 3)
+        ops.dropout_apply(dx, ref_mask, p, seed, site)
         assert torch.equal(dmask, ref_mask)
+        keep = keep_ref(seed, site, rows, H, p)  # dmask = bf16(bf16(dx) * keep * scale)
+        assert torch.equal(dmask.cpu(), (dx.cpu().float() * keep * float(DM.dropout_scale(p))).bfloat16())
         assert rel(dbias, 2 * dmask.float().sum(0)) < 1e-5
         kept = float((dmask != 0).float().mean())
         assert abs(kept - (1 - p)) < (0.2 if rows * H < 4096 else 0.02)
@@ -423,3 +436,157 @@ def test_device_mask_draws_distributions_and_bit_exact_masking(ops):
     mx = torch.empty(B, k, dtype=torch.int32, device=DEV)
     o.mask_inputs(ids.to(DEV), summ.to(DEV), d, mi, mx, None, 25, k, True, 1, consts)
     assert torch.equal(mi.cpu(), ref["masked_ids"]) and torch.equal(mx.cpu(), ref["masked_idx"])
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Training-mode hidden dropout: every kernel that draws the counter-based mask (GEMM epilogue, LayerNorm forward, both
+# LayerNorm backwards, bias gradient, dropout_apply) against the NumPy restatement of its definition, bit for bit.
+# Inputs are chosen so that the kernel's output reads the mask back exactly (ones, gamma = 0 / beta = 1, A = 0 / bias = 1).
+# ---------------------------------------------------------------------------------------------------------------
+DROP_CASES = [(0, 0, 0.1), (7, 1, 0.2), (2 ** 40 + 3, 223, 0.5), (2 ** 40 + 3, 301, 0.1)]  # (seed, site, p)
+
+
+def _drop_cases(*axes):
+    """The product of `axes`, each combination paired with one of DROP_CASES in turn."""
+    return [(*combo, *DROP_CASES[i % len(DROP_CASES)]) for i, combo in enumerate(itertools.product(*axes))]
+
+
+@pytest.mark.parametrize("seed,site,p", DROP_CASES)
+@pytest.mark.parametrize("rows,N,ld_x,ld_y", [(1, 8, 8, 8), (37, 136, 136, 136), (515, 72, 96, 104), (8512, 768, 768, 768)])
+def test_dropout_apply_mask(ops, rows, N, ld_x, ld_y, seed, site, p):
+    """Ones in: every kept element is bf16(1/(1-p)), every dropped one 0.  Leading dimensions larger than N: the mask is
+    keyed by row * N + col, not by the leading dimension, and the columns past N are neither read into the mask nor written."""
+    x = torch.full((rows, ld_x), 5.0, dtype=torch.bfloat16, device=DEV)
+    x[:, :N] = 1.0
+    y = torch.full((rows, ld_y), float("nan"), dtype=torch.bfloat16, device=DEV)
+    ops.dropout_apply(x[:, :N], y[:, :N], p, seed, site)
+    keep = keep_ref(seed, site, rows, N, p)
+    assert torch.equal(y[:, :N].cpu(), (keep * float(DM.dropout_scale(p))).bfloat16())
+    assert torch.isnan(y[:, N:].float()).all()
+
+
+@pytest.mark.parametrize("bn,M,N,seed,site,p", [(bn, M, N, *c) for bn, (M, N), *c in _drop_cases((128, 192, 256), ((300, 264), (515, 72), (8512, 768)))])
+def test_gemm_dropout_epilogue_mask(ops, bn, M, N, seed, site, p):
+    """A = 0, bias = 1: the epilogue's output is exactly keep * scale, and bf16(keep * scale + R) with a residual.  Every tile
+    width, ragged M / N edges, and at 8512 x 768 more tiles than SMs (the persistent loop runs several tiles per CTA)."""
+    g = torch.Generator().manual_seed(M + N + bn)
+    K = 64
+    a = torch.zeros(M, K, dtype=torch.bfloat16, device=DEV)
+    w = (torch.randn(K, N, generator=g) * 0.1).bfloat16().to(DEV)
+    ones = torch.ones(N, device=DEV)
+    resid = torch.randn(M, N, generator=g).bfloat16()
+    kw = dict(b_mn_major=True, bias=ones, dropout_p=p, dropout_seed=seed, dropout_site=site, block_n=bn)
+    want = keep_ref(seed, site, M, N, p) * float(DM.dropout_scale(p))
+    assert torch.equal(ops.gemm(a, w, **kw).cpu(), want.bfloat16())
+    assert torch.equal(ops.gemm(a, w, resid=resid.to(DEV), **kw).cpu(), (want + resid.float()).bfloat16())
+
+
+def test_gemm_dropout_epilogue_values(ops):
+    """Non-zero A: (A @ B + bias) * keep / (1 - p) + resid -- the mask sits after the bias and before the residual."""
+    g = torch.Generator().manual_seed(3)
+    M, N, K = 520, 768, 768
+    seed, site, p = 2 ** 40 + 3, 223, 0.2
+    a = (torch.randn(M, K, generator=g) * 0.3).bfloat16()
+    w = (torch.randn(K, N, generator=g) * 0.05).bfloat16()
+    bias = torch.randn(N, generator=g)
+    resid = torch.randn(M, N, generator=g).bfloat16()
+    out = ops.gemm(a.to(DEV), w.to(DEV), b_mn_major=True, bias=bias.to(DEV), resid=resid.to(DEV), dropout_p=p,
+                   dropout_seed=seed, dropout_site=site)
+    keep = keep_ref(seed, site, M, N, p)
+    want = (a.float() @ w.float() + bias) * keep / (1 - p) + resid.float()
+    assert rel(out, want) < 6e-3
+    assert rel(out, (a.float() @ w.float()) * keep / (1 - p) + bias + resid.float()) > 6e-3  # mask before the bias: caught
+
+
+def _remap_rows(rows, remap):
+    per, stride, off = remap
+    r = torch.arange(rows)
+    return (r // per) * stride + off + r % per if per > 0 else r
+
+
+@pytest.mark.parametrize("x_f32,y_f32,remap,seed,site,p", _drop_cases((False, True), (False, True), ((0, 0, 0), (29, 40, 6))))
+def test_layernorm_fwd_dropout_mask(ops, x_f32, y_f32, remap, seed, site, p):
+    """gamma = 0, beta = 1: y = keep * scale exactly, in all four x / y dtypes, with and without the row remap of the joint
+    encoder's embedding rows.  The mask follows the LOGICAL row; rows the remap skips keep their NaN sentinel.  Then random
+    gamma / beta against the fp32 LayerNorm times the mask."""
+    rows, H = 203, 256
+    g = torch.Generator().manual_seed(rows + int(x_f32) + 2 * int(y_f32))
+    x = torch.randn(rows, H, generator=g) * 2 + 0.5
+    x = x if x_f32 else x.bfloat16()
+    ydt = torch.float32 if y_f32 else torch.bfloat16
+    orow = _remap_rows(rows, remap)
+    out_rows = int(orow.max()) + 1 + (11 if remap[0] else 0)
+    keep = keep_ref(seed, site, rows, H, p)
+    scale = float(DM.dropout_scale(p))
+    y = torch.full((out_rows, H), float("nan"), dtype=ydt, device=DEV)
+    ops.layernorm_fwd(x.to(DEV), y, torch.zeros(H, device=DEV), torch.ones(H, device=DEV), rows=rows, remap=remap,
+                      dropout=(p, seed, site))
+    yc = y.cpu()
+    assert torch.equal(yc[orow], (keep * scale).to(ydt))
+    skipped = torch.ones(out_rows, dtype=torch.bool)
+    skipped[orow] = False
+    assert torch.isnan(yc[skipped].float()).all() and (not remap[0] or bool(skipped.any()))
+    gam, bet = torch.randn(H, generator=g), torch.randn(H, generator=g)
+    y.fill_(float("nan"))
+    ops.layernorm_fwd(x.to(DEV), y, gam.to(DEV), bet.to(DEV), rows=rows, remap=remap, dropout=(p, seed, site))
+    want = O.layer_norm(x.float(), {"l/gamma": gam, "l/beta": bet}, "l") * keep * scale
+    assert rel(y.cpu()[orow], want) < (1e-5 if y_f32 else 4e-3)
+
+
+def _ln_bwd_reference(x, dy_logical, dres, gam, bet, keep, scale):
+    xr, gr, br = x.float().requires_grad_(True), gam.clone().requires_grad_(True), bet.clone().requires_grad_(True)
+    y = O.layer_norm(xr, {"l/gamma": gr, "l/beta": br}, "l") * keep * scale
+    y.backward(dy_logical.float())
+    return xr.grad + dres.float(), gr.grad, br.grad
+
+
+@pytest.mark.parametrize("x_f32,dy_f32,dx_f32,remap,seed,site,p",
+                         [(*d, *rest) for d, *rest in _drop_cases(((False, False, False), (True, False, True), (True, True, True),
+                                                                   (False, True, False)), ((0, 0, 0), (37, 50, 5)))])
+def test_layernorm_bwd_dropout(ops, x_f32, dy_f32, dx_f32, remap, seed, site, p):
+    """The unfused LayerNorm backward of the embedding LayerNorms: dy is the gradient of dropout(LN(x)) (read through the row
+    remap), dx / dgamma / dbeta against fp32 autograd under the restated mask; the mask of site + 1 must miss those bounds."""
+    rows, H = 333, 384
+    g = torch.Generator().manual_seed(rows + int(x_f32) + 2 * int(dy_f32))
+    xdt = torch.float32 if x_f32 else torch.bfloat16
+    dxdt = torch.float32 if dx_f32 else torch.bfloat16
+    x = (torch.randn(rows, H, generator=g) * 2 + 0.5).to(xdt)
+    gam, bet = torch.randn(H, generator=g), torch.randn(H, generator=g)
+    orow = _remap_rows(rows, remap)
+    dy_full = torch.randn(int(orow.max()) + 1, H, generator=g).to(torch.float32 if dy_f32 else torch.bfloat16)
+    dres = torch.randn(rows, H, generator=g).to(dxdt)
+    xf = x.float()
+    mu, rs = xf.mean(-1), torch.rsqrt(xf.var(-1, unbiased=False) + 1e-5)
+    dx = torch.full((rows, H), float("nan"), dtype=dxdt, device=DEV)
+    dg, db = torch.zeros(H, device=DEV), torch.zeros(H, device=DEV)
+    ops.layernorm_bwd(dy_full.to(DEV), x.to(DEV), mu.to(DEV), rs.to(DEV), gam.to(DEV), dx, dg, db, dres=dres.to(DEV), rows=rows,
+                      remap=remap, dropout=(p, seed, site))
+    scale = float(DM.dropout_scale(p))
+    tol = 1e-5 if dx_f32 else 6e-3
+
+    def within(keep):
+        want_dx, want_g, want_b = _ln_bwd_reference(x, dy_full[orow], dres, gam, bet, keep, scale)
+        return rel(dx, want_dx) < tol and rel(dg, want_g) < 2e-3 and rel(db, want_b) < 2e-3
+
+    assert within(keep_ref(seed, site, rows, H, p))
+    assert not within(keep_ref(seed, site + 1, rows, H, p))
+
+
+@pytest.mark.parametrize("dy_f32,rows,N,ld,seed,site,p", [(f, *shape, *c) for f, shape, *c in _drop_cases((False, True), ((8512, 768, 768), (300, 264, 280)))])
+def test_bias_grad_dropout(ops, dy_f32, rows, N, ld, seed, site, p):
+    """merlot_bias_grad through the forward dropout mask: dy = 1 gives scale x (kept rows of each column) to 1e-6; random dy
+    against fp64 to 1e-5.  A leading dimension larger than N leaves the mask keyed by row * N + col."""
+    g = torch.Generator().manual_seed(rows + N)
+    dt = torch.float32 if dy_f32 else torch.bfloat16
+    keep = keep_ref(seed, site, rows, N, p).double()
+    scale = float(DM.dropout_scale(p))
+    ones = torch.full((rows, ld), 3.0, dtype=dt, device=DEV)
+    ones[:, :N] = 1.0
+    out = torch.zeros(N, device=DEV)
+    ops.bias_grad(ones[:, :N], out, rows=rows, N=N, dropout=(p, seed, site))
+    want = keep.sum(0) * scale
+    assert ((out.cpu().double() - want).abs() <= 1e-6 * want).all()
+    dy = torch.randn(rows, ld, generator=g).to(dt)
+    out.zero_()
+    ops.bias_grad(dy.to(DEV)[:, :N], out, rows=rows, N=N, dropout=(p, seed, site))
+    assert rel(out, (dy[:, :N].double() * keep * scale).sum(0)) < 1e-5

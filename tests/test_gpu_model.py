@@ -1,6 +1,7 @@
 """GPU parity of the whole hot path through the MerlotModel mirror (pytest -m gpu): forward activations, the three
-losses, every parameter gradient, one optimizer step -- against the oracle on identical weights and inputs (dropout 0);
-plus size-independent properties at merlot.yaml's full sizes."""
+losses, every parameter gradient, one optimizer step -- against the oracle on identical weights and inputs, in eval mode
+(dropout 0) and in training mode (hidden dropout under the kernels' own masks); plus size-independent properties at
+merlot.yaml's full sizes."""
 import pytest
 import torch
 
@@ -46,23 +47,26 @@ def build(cfg, seed=1):
     return params, store, ocfg
 
 
-def test_pretrain_step_parity(tiny_cfg):
+def _step_parity(cfg, is_training=False, dropout_seed=0, oracle_dropout=None, wrong_dropout=None):
+    """One pretraining step (forward, the three losses, backward, AdamW) against the oracle on the same weights and inputs.
+    Training mode: the model runs with dropout_seed, the oracle applies `oracle_dropout` (its hook for the same seed) and an
+    oracle with `wrong_dropout` (another seed) must miss the hidden-state or loss bars."""
     from merlot_b200.modeling import MerlotModel
     from merlot_b200.optimization import build_optimizer_from_config
-    cfg = tiny_cfg
     batch, nc, Lc = 2, 4, 16
     image, ids, shuf, vid = synth(cfg, batch, nc, Lc, 64, 96, 0)
     params, store, ocfg = build(cfg)
     B, Lj = batch * nc // cfg["num_chunks_in_group"], Lc * cfg["num_chunks_in_group"]
     draws = O.make_mask_draws(B, Lj, int(Lj * 0.2), cfg["vocab_size"], seed=5)
-    m = MerlotModel(cfg, is_training=False, use_tpu=False, image=image.to(DEV), input_ids=ids.to(DEV), mask_input=True,
-                    shuffled_idx_img=shuf.to(DEV), params=store, mask_draws=draws, save_for_backward=True)
+    m = MerlotModel(cfg, is_training=is_training, use_tpu=False, image=image.to(DEV), input_ids=ids.to(DEV), mask_input=True,
+                    shuffled_idx_img=shuf.to(DEV), params=store, mask_draws=draws, save_for_backward=True, dropout_seed=dropout_seed)
     leaf = {k: v.clone().requires_grad_(True) for k, v in params.items()}
-    om = O.MerlotOracle(cfg, leaf, image, ids, mask_input=True, shuffled_idx_img=shuf, mask_draws=draws)
+    om = O.MerlotOracle(cfg, leaf, image, ids, mask_input=True, shuffled_idx_img=shuf, mask_draws=draws, dropout=oracle_dropout)
     assert rel(m.lang_transformer_info["attention_summs"], om.attention_summs) < 2e-3
     gm = {"masked_ids": m.lang_mask_info["masked_ids"].cpu().reshape(B, Lj), "masked_idx": m.lang_mask_info["masked_idx"].cpu()}
     if not (torch.equal(gm["masked_ids"], om.lang_mask_info["masked_ids"]) and torch.equal(gm["masked_idx"], om.lang_mask_info["masked_idx"])):
-        om = O.MerlotOracle(cfg, leaf, image, ids, mask_input=True, shuffled_idx_img=shuf, mask_override=gm)  # near-tie in attn sums
+        om = O.MerlotOracle(cfg, leaf, image, ids, mask_input=True, shuffled_idx_img=shuf, mask_override=gm,
+                            dropout=oracle_dropout)  # near-tie in attn sums
     for name in ("viz", "lang"):
         assert rel(m.encoder_hidden_states[name], om.encoder_hidden_states[name]) < 1e-2  # rel-Frobenius, bf16 stacks
     for k, v in om.attention_log.items():  # attention_log metrics (model/modeling.py:186-203)
@@ -78,6 +82,11 @@ def test_pretrain_step_parity(tiny_cfg):
         assert abs(float(a) - float(b)) <= 2e-3 * abs(float(b)), (float(a), float(b))
     total = float(ll) + float(cl) + float(tl)
     assert abs(total - float(total_ref)) <= 1e-3 * abs(float(total_ref))  # north-star bar: losses within 1e-3 rel
+    if wrong_dropout is not None:  # the comparison notices a mask that is not the one the step used
+        bad = O.MerlotOracle(cfg, params, image, ids, mask_input=True, shuffled_idx_img=shuf, mask_override=gm, dropout=wrong_dropout)
+        bad_total, _ = O.pretrain_losses(bad, shuf, vid)
+        assert (max(rel(m.encoder_hidden_states[n], bad.encoder_hidden_states[n]) for n in ("viz", "lang")) >= 1e-2
+                or abs(total - float(bad_total)) > 1e-3 * abs(float(bad_total)))
     assert float(tinfo["lang_viz_acc"]) == pytest.approx(float(oinfo["temporal"]["lang_viz_acc"]), abs=1e-6)
     store.g.zero_()
     m.backward()
@@ -97,6 +106,21 @@ def test_pretrain_step_parity(tiny_cfg):
     for k in after:
         assert (after[k] - p_before[k]).abs().max().item() < 2e-6, k
     assert float(store.g.abs().max()) == 0.0 and store.global_step == 1
+
+
+def test_pretrain_step_parity(tiny_cfg):
+    _step_parity(tiny_cfg)
+
+
+def test_pretrain_step_parity_training_mode(tiny_cfg):
+    """The training step with hidden dropout on (the headline configuration), against the oracle under the very masks the
+    kernels draw (oracle/dropout_mask.py).  ViT and text stacks use different probabilities, so swapped ones are caught; the
+    seed has a non-zero high word."""
+    from oracle import dropout_mask as DM
+    cfg = dict(tiny_cfg, hidden_dropout_prob=0.1, vit_hidden_dropout_prob=0.2)
+    seed = 2 ** 32 + 77
+    _step_parity(cfg, is_training=True, dropout_seed=seed, oracle_dropout=DM.dropout_hook(seed, 0.1, 0.2),
+                 wrong_dropout=DM.dropout_hook(seed + 1, 0.1, 0.2))
 
 
 def test_disable_pairwise_lang_attn(tiny_cfg):
@@ -225,18 +249,17 @@ def test_full_size_properties():
     assert fn(feats).loss < l0  # the step trains
 
 
-def test_partial_stack_backward_equals_full(tiny_cfg):
-    """merlot_stack_backward walked in layer groups (bwd_lo/bwd_hi; data-parallel bucket overlap) gives the gradients of one
-    full call (the only difference allowed is the order of fp32 atomic adds in split-K wgrads / LN column sums)."""
+def _partial_backward_equals_full(tiny_cfg, training):
     from merlot_b200.modeling import MerlotModel
-    cfg = dict(tiny_cfg, num_vision_transformer_hidden_layers=4)
+    cfg = dict(tiny_cfg, num_vision_transformer_hidden_layers=4, vit_hidden_dropout_prob=0.2)
     image, ids, shuf, vid = synth(cfg, 2, 4, 16, 64, 96, 0)
     params, store, _ = build(cfg)
     draws = O.make_mask_draws(4, 32, 6, cfg["vocab_size"], seed=5)
     gs = []
     for groups in (None, [(2, 4), (1, 2), (0, 1)]):
-        m = MerlotModel(cfg, is_training=False, use_tpu=False, image=image.to(DEV), input_ids=ids.to(DEV), mask_input=True,
-                        shuffled_idx_img=shuf.to(DEV), params=store, mask_draws=draws, save_for_backward=True)
+        m = MerlotModel(cfg, is_training=training, use_tpu=False, image=image.to(DEV), input_ids=ids.to(DEV), mask_input=True,
+                        shuffled_idx_img=shuf.to(DEV), params=store, mask_draws=draws, save_for_backward=True,
+                        dropout_seed=2 ** 32 + 5)
         m.mask_loss(), m.contrastive_loss(), m.temporal_loss(shuf.to(DEV), vid.to(DEV))
         store.g.zero_()
         seen = []
@@ -245,6 +268,18 @@ def test_partial_stack_backward_equals_full(tiny_cfg):
         assert seen == ([] if groups is None else [0, 1, 2])
     assert rel(gs[1], gs[0]) < 1e-3
     store.g.zero_()
+
+
+def test_partial_stack_backward_equals_full(tiny_cfg):
+    """merlot_stack_backward walked in layer groups (bwd_lo/bwd_hi; data-parallel bucket overlap) gives the gradients of one
+    full call (the only difference allowed is the order of fp32 atomic adds in split-K wgrads / LN column sums)."""
+    _partial_backward_equals_full(tiny_cfg, training=False)
+
+
+def test_partial_stack_backward_equals_full_training_mode(tiny_cfg):
+    """The same with hidden dropout on: each layer-group call hands the next one the dropout-masked stream gradient of the
+    layer below it (`dmask` in the stack's scratch)."""
+    _partial_backward_equals_full(tiny_cfg, training=True)
 
 
 def test_exported_attention_probabilities(tiny_cfg):

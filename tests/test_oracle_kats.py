@@ -287,3 +287,158 @@ def test_hybrid_stem_two_restatements_agree():  # torch fp64 (merlot_oracle) vs 
         y = relu(z + sc)
     assert ref.shape == y.shape == (1, 4, 6, 512)
     assert np.allclose(ref, y, rtol=1e-7, atol=1e-8)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Training-mode dropout: the CUDA path's counter-based mask restated from its definition (oracle/dropout_mask.py), and the
+# hook through which the oracle applies it at the reference's dropout call sites
+# ---------------------------------------------------------------------------------------------------------------
+def test_philox4x32_known_answers():
+    """The round function and key schedule against the Philox4x32-10 known-answer vectors published with Random123
+    (kat_vectors); the dropout mask runs the same rounds, 7 of them."""
+    from oracle import dropout_mask as DM
+    kats = [((0, 0, 0, 0), (0, 0), [0x6627E8D5, 0xE169C58D, 0xBC57AC4C, 0x9B00DBD8]),
+            ((0xFFFFFFFF,) * 4, (0xFFFFFFFF,) * 2, [0x408F276D, 0x41C83B0E, 0xA20BC7C6, 0x6D5451FD]),
+            ((0x243F6A88, 0x85A308D3, 0x13198A2E, 0x03707344), (0xA4093822, 0x299F31D0),
+             [0xD16CFE09, 0x94FDCCEB, 0x5001E420, 0x24126EA1])]
+    for ctr, key, want in kats:
+        assert [int(w) for w in DM.philox4x32(ctr, key, 10)] == want
+    assert DM.DROPOUT_ROUNDS == 7
+
+
+def test_dropout_threshold_and_scale():  # float32 host arithmetic: 0.1f * 65536 = 6553.6001, + 0.5, truncated
+    from oracle import dropout_mask as DM
+    assert (DM.thresh16(0.1), DM.thresh16(0.2), DM.thresh16(0.5)) == (6554, 13107, 32768)
+    assert DM.dropout_scale(0.5) == np.float32(2.0) and DM.dropout_scale(0.1) == np.float32(1.1111112)
+
+
+@pytest.mark.parametrize("p", [0.1, 0.2, 0.5])
+def test_counter_dropout_keep_rate(p):
+    from oracle import dropout_mask as DM
+    keep = DM.counter_dropout_keep(2 ** 40 + 3, 223, 2048, 512, p)
+    q = 1.0 - DM.thresh16(p) / 65536.0
+    assert abs(keep.mean() - q) < 5.0 * math.sqrt(q * (1.0 - q) / keep.size)
+
+
+@pytest.mark.parametrize("p", [0.1, 0.5])
+def test_counter_dropout_keep_pairwise_uncorrelated(p):
+    """Adjacent 16-bit lanes of one Philox word, adjacent counters (idx8), adjacent sites, and seeds s / s + 2^32 (the key's
+    high word): every pair's correlation within 5 / sqrt(n)."""
+    from oracle import dropout_mask as DM
+    s, site, rows, N = 7, 1, 1024, 512
+    k = DM.counter_dropout_keep(s, site, rows, N, p).reshape(-1, 8).astype(np.float64)
+
+    def check(a, b):
+        a, b = a.ravel(), b.ravel()
+        assert abs(np.corrcoef(a, b)[0, 1]) < 5.0 / math.sqrt(a.size)
+
+    check(k[:, 0::2], k[:, 1::2])  # low / high half of each word
+    check(k[:-1], k[1:])  # idx8 and idx8 + 1
+    check(k, DM.counter_dropout_keep(s, site + 1, rows, N, p).reshape(-1, 8))
+    check(k, DM.counter_dropout_keep(s + 2 ** 32, site, rows, N, p).reshape(-1, 8))
+
+
+def test_counter_dropout_keep_depends_on_linear_index_only():
+    from oracle import dropout_mask as DM
+    a = DM.counter_dropout_keep(2 ** 40 + 3, 301, 96, 768, 0.2)
+    assert np.array_equal(a.ravel(), DM.counter_dropout_keep(2 ** 40 + 3, 301, 96 * 768 // 8, 8, 0.2).ravel())
+    assert np.array_equal(a.ravel(), DM.counter_dropout_keep(2 ** 40 + 3, 301, 96 * 6, 128, 0.2).ravel())
+    with pytest.raises(ValueError):
+        DM.counter_dropout_keep(0, 0, 2, 12, 0.1)
+
+
+def test_dropout_kernel_sites():  # merlot_b200/modeling.py _SITE_*, merlot_stack_forward: base + 2l (out-proj), + 2l + 1 (FFN2)
+    from oracle import dropout_mask as DM
+    assert [DM.kernel_site(k) for k in (("vit", 0, "attn"), ("vit", 0, "ffn"), ("vit", 3, "ffn"), ("langonly", 1, "attn"),
+                                        ("joint", 11, "ffn"), ("embed", "langonly"), ("embed", "joint"))] == \
+        [0, 1, 7, 102, 223, 300, 301]
+
+
+def _oracle_case(tiny_cfg):
+    g = torch.Generator().manual_seed(0)
+    image = torch.rand(4, 64, 96, 3, generator=g)
+    ids = torch.randint(100, 1000, (2, 2, 16), generator=g, dtype=torch.int32)
+    ids[:, :, 0] = O.START
+    ids[:, :, 12:] = 0
+    params = O.init_params(tiny_cfg, 1, perturb=0.05)
+    shuf = torch.tensor([0, 1, 17, 16], dtype=torch.int32)
+    vid = torch.zeros(2, 2, dtype=torch.int32)
+    draws = O.make_mask_draws(2, 32, 6, 1000, seed=2)
+    return image, ids, params, shuf, vid, draws
+
+
+def _oracle_outputs(m, shuf, vid):
+    tot, info = O.pretrain_losses(m, shuf, vid)
+    out = {"total": tot, "lang_trg_h": m.lang_trg_h, "img_trg_h": m.img_trg_h, "attention_summs": m.attention_summs,
+           "masked_ids": m.lang_mask_info["masked_ids"], "masked_idx": m.lang_mask_info["masked_idx"],
+           "vit": m.vision_transformer_info["hidden_state"], "lo": m.lang_transformer_info["hidden_state"],
+           "joint": m.encoder_info["hidden_state"], "joint_probs": m.encoder_info["self_attn_probs"]}
+    out.update({f"log/{k}": v for k, v in m.attention_log.items()})
+    out.update({f"{h}/{k}": v for h, d in info.items() for k, v in d.items()})
+    return out
+
+
+def test_dropout_hook_off_leaves_the_oracle_unchanged(tiny_cfg):
+    """No hook, dropout=None, an identity hook and a p = 0 training hook: every output bit for bit the same."""
+    from oracle import dropout_mask as DM
+    image, ids, params, shuf, vid, draws = _oracle_case(tiny_cfg)
+    kw = dict(mask_input=True, shuffled_idx_img=shuf, mask_draws=draws)
+    ref = _oracle_outputs(O.MerlotOracle(tiny_cfg, params, image, ids, **kw), shuf, vid)
+    for hook in (None, lambda key, x: x, DM.dropout_hook(5, 0.0, 0.0)):
+        got = _oracle_outputs(O.MerlotOracle(tiny_cfg, params, image, ids, dropout=hook, **kw), shuf, vid)
+        assert got.keys() == ref.keys()
+        for k in ref:
+            assert torch.equal(torch.as_tensor(got[k]), torch.as_tensor(ref[k])), k
+
+
+def test_dropout_hook_call_sites(tiny_cfg):
+    """The hook runs exactly where the reference applies hidden dropout: 2 per layer in each of the three stacks (after the
+    context projection, after the FFN output) and once after each embedding LayerNorm, on [rows, H] in logical row order."""
+    image, ids, params, shuf, vid, draws = _oracle_case(tiny_cfg)
+    calls = []
+
+    def spy(key, x):
+        calls.append((key, tuple(x.shape)))
+        return x
+
+    m = O.MerlotOracle(tiny_cfg, params, image, ids, mask_input=True, shuffled_idx_img=shuf, mask_draws=draws, dropout=spy)
+    H = tiny_cfg["hidden_size"]
+    n_vit, n_lo, n_j = (tiny_cfg["num_vision_transformer_hidden_layers"], tiny_cfg["num_lang_transformer_hidden_layers"],
+                        tiny_cfg["num_hidden_layers"])
+    rows_vit = image.shape[0] * ((64 // 16) * (96 // 16) + 2)
+    rows_lo = ids.shape[0] * ids.shape[1] * ids.shape[2]
+    rows_j = m.B * (m.P + m.L)
+
+    def stack(name, n, rows):
+        return [((name, l, kind), (rows, H)) for l in range(n) for kind in ("attn", "ffn")]
+
+    want = (stack("vit", n_vit, rows_vit) + [(("embed", "langonly"), (rows_lo, H))] + stack("langonly", n_lo, rows_lo)
+            + [(("embed", "joint"), (m.B * m.L, H))] + stack("joint", n_j, rows_j))
+    assert calls == want
+    assert len(calls) == 2 * (n_vit + n_lo + n_j) + 2
+
+
+def test_dropout_hook_mask_scale_and_gradient(tiny_cfg):
+    """The training hook multiplies by keep * 1/(1-p) of the restated mask (vit_hidden_dropout_prob in the ViT), autograd
+    carries the same factor back, and a whole oracle step with it is finite and differs from the eval step."""
+    from oracle import dropout_mask as DM
+    seed = 2 ** 32 + 9
+    hook = DM.dropout_hook(seed, 0.2, 0.5)
+    for key, p in ((("joint", 1, "ffn"), 0.2), (("vit", 0, "attn"), 0.5), (("embed", "langonly"), 0.2)):
+        x = torch.randn(64, 128, generator=torch.Generator().manual_seed(1), requires_grad=True)
+        y = hook(key, x)
+        keep = torch.from_numpy(DM.counter_dropout_keep(seed, DM.kernel_site(key), 64, 128, p))
+        factor = keep.float() * float(DM.dropout_scale(p))
+        assert torch.equal(y, x * factor)
+        y.sum().backward()
+        assert torch.equal(x.grad, factor)
+    image, ids, params, shuf, vid, draws = _oracle_case(tiny_cfg)
+    leaf = {k: v.clone().requires_grad_(True) for k, v in params.items()}
+    kw = dict(mask_input=True, shuffled_idx_img=shuf, mask_draws=draws)
+    m = O.MerlotOracle(tiny_cfg, leaf, image, ids, dropout=hook, **kw)
+    tot, _ = O.pretrain_losses(m, shuf, vid)
+    ev, _ = O.pretrain_losses(O.MerlotOracle(tiny_cfg, params, image, ids, **kw), shuf, vid)
+    assert math.isfinite(float(tot.detach())) and float(tot.detach()) != float(ev)
+    tot.backward()
+    g = leaf["encoder/layer00/output/bias"].grad
+    assert g is not None and torch.isfinite(g).all() and float(g.norm()) > 0
