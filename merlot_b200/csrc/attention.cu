@@ -749,6 +749,8 @@ extern "C" int merlot_attention_bwd(const merlot_attn_t* a, void* stream_) {
              "attention_bwd: ctx, d_ctx, lse, dsum, dq_accum and dqkv are all required");
   MB_REQUIRE((a->ld_ctx % 8) == 0 && (a->ld_dqkv % 8) == 0 && (a->ld_dq % 4) == 0, MERLOT_ESHAPE,
              "attention_bwd: leading dimensions must keep 16-byte alignment");
+  // before the first launch: a rejected call must leave dsum (and everything else) untouched
+  MB_REQUIRE(a->S <= MAX_MASK_WORDS * 32 - AT_M, MERLOT_ESHAPE, "attention_bwd: sequence longer than %d keys", MAX_MASK_WORDS * 32 - AT_M);
   AttnDev p; fill_dev(a, &p);
   const int H = p.H;
   const long long tokens = (long long)a->B * a->S;
@@ -768,7 +770,6 @@ extern "C" int merlot_attention_bwd(const merlot_attn_t* a, void* stream_) {
   if (rc) return rc;
   rc = make_tmap_bf16_2d(&tdo, a->d_ctx, (uint64_t)a->ld_ctx, (uint64_t)tokens, (uint64_t)a->ld_ctx, 64, BQ);
   if (rc) return rc;
-  MB_REQUIRE(a->S <= MAX_MASK_WORDS * 32 - AT_M, MERLOT_ESHAPE, "attention_bwd: sequence longer than %d keys", MAX_MASK_WORDS * 32 - AT_M);
   static bool attr = false;
   if (!attr) {
     MB_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));

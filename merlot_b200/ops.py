@@ -129,9 +129,11 @@ def attention_bwd_workspace(B: int, S: int, heads: int, device) -> torch.Tensor:
     return torch.zeros((n // H, H), dtype=torch.float32, device=device)
 
 
-def attention_bwd(qkv, ctx, d_ctx, lse, B, S, heads, valid=None, dqkv=None, dq_accum=None, dsum=None, pair=(0, 0)):
+def attention_bwd(qkv, ctx, d_ctx, lse, B, S, heads, valid=None, dqkv=None, dq_accum=None, dsum=None, pair=(0, 0),
+                  d_bias_qkv=None):
     """K3: dqkv[B*S,3H] from d_ctx.  dq_accum: fp32 workspace of merlot_attention_bwd_workspace_bytes (see the header);
-    in atomic mode (long sequences) it must be zero on entry and is returned zeroed."""
+    in atomic mode (long sequences) it must be zero on entry and is returned zeroed.  d_bias_qkv: optional fp32 [3H] that
+    the column sums of dqkv (the gradient of the fused q/k/v bias) are added to."""
     a = _attn_desc(qkv, B, S, heads, valid, pair)
     H = heads * a.head_dim
     dev = qkv.device
@@ -148,6 +150,10 @@ def attention_bwd(qkv, ctx, d_ctx, lse, B, S, heads, valid=None, dqkv=None, dq_a
     a.d_ctx, a.dsum = d_ctx.data_ptr(), dsum.data_ptr()
     a.dq_accum, a.ld_dq = dq_accum.data_ptr(), H
     a.dqkv, a.ld_dqkv = dqkv.data_ptr(), dqkv.stride(0)
+    if d_bias_qkv is not None:
+        _require_cuda(d_bias_qkv)
+        assert d_bias_qkv.dtype == torch.float32 and d_bias_qkv.numel() == 3 * H and d_bias_qkv.is_contiguous()
+        a.d_bias_qkv = d_bias_qkv.data_ptr()
     L.check(L.lib().merlot_attention_bwd(C.byref(a), _stream()))
     return dqkv
 

@@ -148,10 +148,12 @@ def test_gemm_shape_errors(ops):
 # ---------------------------------------------------------------------------------------------------------------
 # K2/K3/K4 attention
 # ---------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("B,S,heads,masked", [(1, 128, 1, False), (2, 64, 2, True), (2, 266, 12, False), (2, 396, 12, True),
-                                              (3, 93, 4, True), (1, 885, 2, True), (1, 1, 1, False)])
-def test_attention_fwd_bwd_colsum(ops, B, S, heads, masked):
-    g = torch.Generator().manual_seed(S)
+def _attn_case(B, S, heads, masked, seed):
+    """Seeded bf16 qkv [B*S, 3H] -- masked: ragged valid lengths and a hole in the last sequence -- and the fp32 reference of
+    utils/transformer.py:98-120 on the same rounded values.  Returns the generator (for further draws), qkv, the uint8
+    validity [B*S] or None, the reference probabilities [B, heads, S, S] and context [B*S, H], and grad(d_ctx), the
+    reference dqkv [B*S, 3H] for an upstream gradient d_ctx [B*S, H]."""
+    g = torch.Generator().manual_seed(seed)
     H = heads * 64
     qkv = torch.randn(B * S, 3 * H, generator=g).bfloat16()
     valid = None
@@ -168,6 +170,23 @@ def test_attention_fwd_bwd_colsum(ops, B, S, heads, masked):
     q, k, v = (x[i].clone().requires_grad_(True) for i in range(3))
     probs, ctx4 = O.attention_core(q, k, v, mask)
     ctx_ref = ctx4.permute(0, 2, 1, 3).reshape(B * S, H)
+
+    def grad(d_ctx):
+        gq, gk, gv = torch.autograd.grad(ctx_ref, (q, k, v), d_ctx.float(), retain_graph=True)
+        return torch.stack([gq, gk, gv], 0).permute(1, 3, 0, 2, 4).reshape(B * S, 3 * H)
+    return g, qkv, valid, probs.detach(), ctx_ref.detach(), grad
+
+
+def _assert_dqkv(dqkv, ref, H):
+    for i in range(3):
+        assert rel(dqkv[:, i * H:(i + 1) * H], ref[:, i * H:(i + 1) * H]) < 1.5e-2, "qkv"[i]
+
+
+@pytest.mark.parametrize("B,S,heads,masked", [(1, 128, 1, False), (2, 64, 2, True), (2, 266, 12, False), (2, 396, 12, True),
+                                              (3, 93, 4, True), (1, 885, 2, True), (1, 1, 1, False)])
+def test_attention_fwd_bwd_colsum(ops, B, S, heads, masked):
+    g, qkv, valid, probs, ctx_ref, ref_grad = _attn_case(B, S, heads, masked, seed=S)
+    H = heads * 64
     vd = valid.to(DEV) if valid is not None else None
     ctx, lse = ops.attention_fwd(qkv.to(DEV), B, S, heads, vd)
     assert rel(ctx, ctx_ref) < 1e-2
@@ -175,21 +194,119 @@ def test_attention_fwd_bwd_colsum(ops, B, S, heads, masked):
     # padding QUERY rows get a gradient too (they never do in the model): the reference's scores*m - 1e10*(1-m) keeps their
     # uniform probabilities in dV and sends nothing into q / k (utils/transformer.py:109-112)
     dqkv = ops.attention_bwd(qkv.to(DEV), ctx, d_ctx.to(DEV), lse, B, S, heads, vd)
-    ctx_ref.backward(d_ctx.float())
-    ref = torch.stack([q.grad, k.grad, v.grad], 0).permute(1, 3, 0, 2, 4).reshape(B * S, 3 * H)
-    for i in range(3):
-        assert rel(dqkv[:, i * H:(i + 1) * H], ref[:, i * H:(i + 1) * H]) < 1.5e-2
+    _assert_dqkv(dqkv, ref_grad(d_ctx), H)
     colsum = torch.zeros(B, S, device=DEV)
     ops.attention_colsum(qkv.to(DEV), lse, colsum, B, S, heads, vd)
-    assert rel(colsum, probs.detach().mean(1).sum(1)) < 2e-3  # head-mean, summed over queries (transformer.py:208-209)
+    assert rel(colsum, probs.mean(1).sum(1)) < 2e-3  # head-mean, summed over queries (transformer.py:208-209)
 
 
-@pytest.mark.parametrize("B,P,chunk,nch,heads", [(2, 13, 8, 4, 2), (2, 100, 32, 5, 4), (1, 266, 32, 4, 12), (2, 0, 16, 6, 1), (1, 70, 33, 3, 2)])
+# merlot_attention_bwd reduces dQ in one of two ways, chosen by merlot_attention_bwd_dq_parts(S): up to 4 key tiles of 128
+# (S <= 512) every tile stores its own fp32 slice and the finish pass adds the slices in a fixed order; longer sequences
+# red.add into ONE slice that the finish pass sets back to zero for the next layer (0 = atomic mode).
+DQ_MODE_CASES = [(128, 1), (129, 2), (512, 4), (513, 0), (640, 0), (1100, 0), (3968, 0)]  # (S, parts); 3968: the longest S
+# Bias gradient against the fp32 reference's column sums.  The q and v column sums do not cancel and keep about the element
+# error of the bf16 gradient (one bf16 rounding: 2^-9 = 2e-3); the k block, zero in exact arithmetic, is measured against
+# the column sums of |dK|.  Observed on an H100 SXM 80 GB (400 W limit) over all DQ_MODE_CASES: q 3.0e-3, v 1.4e-3, k 3.2e-4.
+BIAS_GRAD_BAR = 1e-2
+
+
+@pytest.mark.parametrize("masked", [False, True])
+@pytest.mark.parametrize("S,parts", DQ_MODE_CASES)
+def test_attention_bwd_dq_modes(ops, S, parts, masked):
+    """Both dQ modes and their boundary (S = 512 / 513) up to the longest accepted sequence: dq / dk / dv against the fp32
+    reference, and the fused q/k/v bias gradient, added to a non-zero buffer, against (a) the exact column sums of the bf16
+    dqkv the finish pass wrote (only the fp32 summation order differs) and (b) the column sums of the fp32 reference
+    gradient.  (b) cannot use the element bar: the k block of the bias gradient is zero in exact arithmetic (softmax is
+    shift invariant), so the kernel's k block is pure rounding noise of the cancelling dK rows."""
+    from merlot_b200._lib import lib
+    assert lib().merlot_attention_bwd_dq_parts(S) == parts  # a changed MAX_DQ_PARTS must not move cases between modes silently
+    B, heads = (1, 2) if S > 2048 else (2, 2)
+    g, qkv, valid, _, ctx_ref, ref_grad = _attn_case(B, S, heads, masked, seed=2 * S + masked)
+    H = heads * 64
+    vd = valid.to(DEV) if valid is not None else None
+    ctx, lse = ops.attention_fwd(qkv.to(DEV), B, S, heads, vd)
+    assert rel(ctx, ctx_ref) < 1e-2
+    d_ctx = (torch.randn(B * S, H, generator=g) * 0.1).bfloat16()
+    start = torch.randn(3 * H, generator=g) * 0.1
+    d_bias = start.to(DEV)
+    dqkv = ops.attention_bwd(qkv.to(DEV), ctx, d_ctx.to(DEV), lse, B, S, heads, vd, d_bias_qkv=d_bias)
+    ref = ref_grad(d_ctx)
+    _assert_dqkv(dqkv, ref, H)
+    d_bias = d_bias.cpu().double()
+    assert rel(d_bias, start.double() + dqkv.cpu().double().sum(0)) < 1e-5
+    got, ref = d_bias - start.double(), ref.double()
+    for i, name in enumerate("qkv"):
+        blk = slice(i * H, (i + 1) * H)
+        if name == "k":  # zero up to fp32 rounding: the error against the size of the terms that cancel
+            err = float((got[blk] - ref[:, blk].sum(0)).norm() / ref[:, blk].abs().sum(0).norm())
+        else:
+            err = rel(got[blk], ref[:, blk].sum(0))
+        assert err < BIAS_GRAD_BAR, (name, err)
+
+
+@pytest.mark.parametrize("S,masked", [(640, True), (1100, False), (129, True), (512, False)])
+def test_attention_bwd_workspace_contract(ops, S, masked):
+    """The dQ workspace as consecutive layers of a stack use it: one buffer, several backwards.  Atomic mode (S > 512): the
+    workspace starts zeroed, every call's result matches its own reference and the call hands the workspace back exactly
+    zero -- a slice left dirty would pollute the dQ of every later layer.  Slices mode: NaN in the workspace before each call
+    must not reach the result, so every slice is fully overwritten."""
+    from merlot_b200._lib import lib
+    parts = lib().merlot_attention_bwd_dq_parts(S)
+    assert (parts == 0) == (S > 512)
+    B, heads = 2, 2
+    g, qkv, valid, _, _, ref_grad = _attn_case(B, S, heads, masked, seed=3 * S + masked)
+    H = heads * 64
+    vd = valid.to(DEV) if valid is not None else None
+    qd = qkv.to(DEV)
+    ctx, lse = ops.attention_fwd(qd, B, S, heads, vd)
+    ws = ops.attention_bwd_workspace(B, S, heads, DEV)
+    for rep in range(2):
+        if parts:
+            ws.fill_(float("nan"))
+        d_ctx = (torch.randn(B * S, H, generator=g) * (0.1 if rep == 0 else 0.3)).bfloat16()
+        dqkv = ops.attention_bwd(qd, ctx, d_ctx.to(DEV), lse, B, S, heads, vd, dq_accum=ws)
+        assert torch.isfinite(dqkv.float()).all()
+        _assert_dqkv(dqkv, ref_grad(d_ctx), H)
+        if not parts:
+            assert torch.equal(ws, torch.zeros_like(ws)), rep
+
+
+def test_attention_rejects_sequences_past_the_validity_mask(ops):
+    """The kernels keep token validity as a bitmask of 4096 positions and the host accepts sequences up to one 128-row tile
+    shorter: S = 3968 is the longest (test_attention_bwd_dq_modes runs it).  S = 3969 raises MerlotShapeError in the host-side
+    check of forward, backward and column sums before anything is launched: every output keeps its sentinel."""
+    from merlot_b200._lib import MerlotShapeError, lib
+    B, S, heads, H = 1, 3969, 1, 64
+    qkv = torch.zeros(B * S, 3 * H, dtype=torch.bfloat16, device=DEV)
+    zeros = torch.zeros(B * S, H, dtype=torch.bfloat16, device=DEV)
+    lse = torch.zeros(B, heads, S, device=DEV)
+    ctx_out = torch.full((B * S, H), 7.0, dtype=torch.bfloat16, device=DEV)
+    lse_out = torch.full((B, heads, S), 7.0, device=DEV)
+    dqkv = torch.full((B * S, 3 * H), 7.0, dtype=torch.bfloat16, device=DEV)
+    dsum = torch.full((B, heads, S), 7.0, device=DEV)  # a launched dsum pass would write rowsum(0 * 0) = 0 here
+    colsum = torch.full((B, S), 7.0, device=DEV)
+    torch.cuda.synchronize()
+    lib().merlot_reset_launch_count()
+    with pytest.raises(MerlotShapeError):
+        ops.attention_fwd(qkv, B, S, heads, ctx=ctx_out, lse=lse_out)
+    with pytest.raises(MerlotShapeError):
+        ops.attention_bwd(qkv, zeros, zeros, lse, B, S, heads, dqkv=dqkv, dsum=dsum)
+    with pytest.raises(MerlotShapeError):
+        ops.attention_colsum(qkv, lse, colsum, B, S, heads)
+    assert lib().merlot_launch_count() == 0
+    torch.cuda.synchronize()
+    for t in (ctx_out, lse_out, dqkv, dsum, colsum):
+        assert bool((t.float() == 7.0).all())
+
+
+@pytest.mark.parametrize("B,P,chunk,nch,heads", [(2, 13, 8, 4, 2), (2, 100, 32, 5, 4), (1, 266, 32, 4, 12), (2, 0, 16, 6, 1), (1, 70, 33, 3, 2),
+                                                 (1, 56, 80, 8, 2), (1, 60, 100, 6, 2)])
 def test_attention_disable_pairwise_lang_attn(ops, B, P, chunk, nch, heads):
     """model/modeling.py:160-168: segment 0 = P vision tokens, segment 1 + c = language chunk c; a pair attends iff it shares a
     segment or either side is a vision token.  K2 / K3 / K4 and the export kernel take (P, chunk) and derive the partner set of
     every row arithmetically; the oracle gets the explicit [B, S, S] mask the reference builds.  Chunk boundaries fall inside
-    32-position words, inside and across the 64 / 128-wide tiles, and some tokens are padding."""
+    32-position words, inside and across the 64 / 128-wide tiles, and some tokens are padding.  S = 696 and 660 (more than 4
+    key tiles) run the backward's atomic dQ mode."""
     S = P + chunk * nch
     g = torch.Generator().manual_seed(S + chunk)
     H = heads * 64
@@ -330,8 +447,10 @@ def test_softmax_ce_and_l2norm(ops):
 # ---------------------------------------------------------------------------------------------------------------
 # K12 masking: bit-exact given injected draws (integer path)
 # ---------------------------------------------------------------------------------------------------------------
+# L > 1024: the block's 1024 threads stride over the positions; L = 3072 is the language length of configs[4]
 @pytest.mark.parametrize("B,L,spanbert,use_attn", [(8, 128, True, True), (3, 32, True, True), (4, 128, False, True),
-                                                   (2, 64, True, False), (2, 1024, True, True)])
+                                                   (2, 64, True, False), (2, 1024, True, True), (2, 1500, True, True),
+                                                   (2, 1500, False, True), (1, 3072, True, True), (1, 3072, False, True)])
 def test_mask_inputs_bit_exact(ops, tiny_cfg, B, L, spanbert, use_attn):
     cfg = dict(tiny_cfg, masking_do_spanbert=spanbert, masking_use_attn=use_attn)
     g = torch.Generator().manual_seed(L + B)

@@ -47,14 +47,14 @@ def build(cfg, seed=1):
     return params, store, ocfg
 
 
-def _step_parity(cfg, is_training=False, dropout_seed=0, oracle_dropout=None, wrong_dropout=None):
-    """One pretraining step (forward, the three losses, backward, AdamW) against the oracle on the same weights and inputs.
-    Training mode: the model runs with dropout_seed, the oracle applies `oracle_dropout` (its hook for the same seed) and an
-    oracle with `wrong_dropout` (another seed) must miss the hidden-state or loss bars."""
+def _step_parity(cfg, is_training=False, dropout_seed=0, oracle_dropout=None, wrong_dropout=None, batch=2, nc=4, Lc=16, hw=(64, 96)):
+    """One pretraining step (forward, the three losses, backward, AdamW) against the oracle on the same weights and inputs:
+    `batch` videos of `nc` segments, captions of `Lc` tokens, frames of hw.  Training mode: the model runs with dropout_seed,
+    the oracle applies `oracle_dropout` (its hook for the same seed) and an oracle with `wrong_dropout` (another seed) must
+    miss the hidden-state or loss bars.  Returns the model."""
     from merlot_b200.modeling import MerlotModel
     from merlot_b200.optimization import build_optimizer_from_config
-    batch, nc, Lc = 2, 4, 16
-    image, ids, shuf, vid = synth(cfg, batch, nc, Lc, 64, 96, 0)
+    image, ids, shuf, vid = synth(cfg, batch, nc, Lc, *hw, 0)
     params, store, ocfg = build(cfg)
     B, Lj = batch * nc // cfg["num_chunks_in_group"], Lc * cfg["num_chunks_in_group"]
     draws = O.make_mask_draws(B, Lj, int(Lj * 0.2), cfg["vocab_size"], seed=5)
@@ -106,6 +106,7 @@ def _step_parity(cfg, is_training=False, dropout_seed=0, oracle_dropout=None, wr
     for k in after:
         assert (after[k] - p_before[k]).abs().max().item() < 2e-6, k
     assert float(store.g.abs().max()) == 0.0 and store.global_step == 1
+    return m
 
 
 def test_pretrain_step_parity(tiny_cfg):
@@ -121,6 +122,36 @@ def test_pretrain_step_parity_training_mode(tiny_cfg):
     seed = 2 ** 32 + 77
     _step_parity(cfg, is_training=True, dropout_seed=seed, oracle_dropout=DM.dropout_hook(seed, 0.1, 0.2),
                  wrong_dropout=DM.dropout_hook(seed + 1, 0.1, 0.2))
+
+
+def _long_sequence_step_parity(tiny_cfg, Lc, max_pos):
+    """The training-mode step of test_pretrain_step_parity_training_mode at tiny width but long sequences: one video of 8
+    segments with Lc-token captions and 64x96 frames (7 vision tokens per segment), so the language-only stack runs over
+    L = 8 Lc tokens and the joint encoder over Sj = 8 Lc + 56.  Both are longer than 4 key tiles, so every attention backward
+    reduces dQ atomically into the one workspace slice that the stack clears once and each layer hands back zeroed to the
+    layer below it; with two layers per stack, the lower layer consumes a workspace the upper one used."""
+    from merlot_b200._lib import lib
+    from oracle import dropout_mask as DM
+    cfg = dict(tiny_cfg, num_chunks_in_group=8, max_position_embeddings=max_pos, hidden_dropout_prob=0.1, vit_hidden_dropout_prob=0.2)
+    L, Sj = 8 * Lc, 8 * Lc + 56
+    assert lib().merlot_attention_bwd_dq_parts(L) == 0 and lib().merlot_attention_bwd_dq_parts(Sj) == 0
+    assert cfg["num_hidden_layers"] >= 2 and cfg["num_lang_transformer_hidden_layers"] >= 2
+    seed = 2 ** 32 + 78
+    m = _step_parity(cfg, is_training=True, dropout_seed=seed, oracle_dropout=DM.dropout_hook(seed, 0.1, 0.2),
+                     wrong_dropout=DM.dropout_hook(seed + 1, 0.1, 0.2), batch=1, nc=8, Lc=Lc)
+    assert m.lang_transformer_info["hidden_state"].shape[1] == L and m._dims["Sj"] == Sj
+
+
+def test_pretrain_step_parity_long_sequence(tiny_cfg):
+    """80-token captions: L = 640, Sj = 696."""
+    _long_sequence_step_parity(tiny_cfg, Lc=80, max_pos=1024)
+
+
+def test_pretrain_step_parity_config5_lengths(tiny_cfg):
+    """configs[4]'s sequence lengths (8 segments x 384-token captions, max_position_embeddings 3072) at tiny width:
+    L = 3072, Sj = 3128.  The full-width step is out of reach of the CPU oracle (its attention probabilities alone would
+    take 12 x 3608^2 x 4 B = 625 MB per layer before autograd)."""
+    _long_sequence_step_parity(tiny_cfg, Lc=384, max_pos=3072)
 
 
 def test_disable_pairwise_lang_attn(tiny_cfg):

@@ -22,6 +22,17 @@ def test_library_exports_every_header_symbol():
     assert lib.merlot_abi_version() == 1
 
 
+def test_attention_bwd_dq_mode_boundary():
+    """merlot_attention_bwd reduces dQ through per-key-tile fp32 slices while the sequence has at most 4 tiles of 128 keys
+    (S <= 512) and atomically into one slice beyond (0 = atomic mode); the workspace a caller allocates follows the mode:
+    parts x B x S x H floats, or one slice."""
+    lib = _lib.lib()
+    for S, parts in [(1, 1), (128, 1), (129, 2), (512, 4), (513, 0), (3608, 0)]:
+        assert lib.merlot_attention_bwd_dq_parts(S) == parts, S
+        for B, heads in [(1, 1), (3, 12)]:
+            assert lib.merlot_attention_bwd_workspace_bytes(B, S, heads) == max(parts, 1) * B * S * heads * 64 * 4, (S, B, heads)
+
+
 def test_ctypes_structs_match_the_header_layout(tmp_path):
     """The descriptor structs of include/merlot_b200.h compiled by gcc (sizeof and the offset of the last member) against their
     ctypes mirrors in merlot_b200/_lib.py: a field added on one side only would shift every later argument silently."""
