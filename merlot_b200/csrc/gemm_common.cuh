@@ -61,17 +61,33 @@ __device__ __forceinline__ void epi_math8(const GemmDev& p, int row, int col, bo
     }
   }
   if (p.flags & MERLOT_GEMM_GELU) {
+    if (p.flags & MERLOT_GEMM_GELU_GRAD_OUT) {
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      pre[i] = (p.flags & MERLOT_GEMM_GELU_GRAD_OUT) ? gelu_erf_grad_fast(v[i]) : v[i];
-      v[i] = gelu_erf_fast(v[i]);
+      for (int i = 0; i < 8; ++i) {  // gelu_erf_grad_fast and gelu_erf_fast from one Phi / exp evaluation
+        float e;
+        const float cdf = normal_cdf_fast(v[i], &e);
+        pre[i] = fmaf(v[i] * 0.39894228040143267794f, e, cdf);
+        v[i] = v[i] * cdf;
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        pre[i] = v[i];
+        v[i] = gelu_erf_fast(v[i]);
+      }
     }
   }
   if ((p.flags & MERLOT_GEMM_MUL_AUX) && in_range) {
-    const bf16* a = p.aux + (size_t)row * p.ld_aux + col;
+    const bf16* a = p.aux + (size_t)row * p.ld_aux + col;  // 16-byte aligned: aux base and ld_aux checked on the host
+    if (full) {
+      uint4 u = __ldg(reinterpret_cast<const uint4*>(a));
+      float2 f0 = unpack_bf16x2(u.x), f1 = unpack_bf16x2(u.y), f2 = unpack_bf16x2(u.z), f3 = unpack_bf16x2(u.w);
+      v[0] *= f0.x; v[1] *= f0.y; v[2] *= f1.x; v[3] *= f1.y; v[4] *= f2.x; v[5] *= f2.y; v[6] *= f3.x; v[7] *= f3.y;
+    } else {
 #pragma unroll
-    for (int i = 0; i < 8; ++i)
-      if (col + i < p.N) v[i] *= __bfloat162float(a[i]);
+      for (int i = 0; i < 8; ++i)
+        if (col + i < p.N) v[i] *= __bfloat162float(a[i]);
+    }
   }
   if ((p.flags & MERLOT_GEMM_MUL_DGELU) && in_range) {
     const bf16* a = p.aux + (size_t)row * p.ld_aux + col;

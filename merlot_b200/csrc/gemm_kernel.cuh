@@ -155,17 +155,24 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
       reg_fence(acc);
       if (prev >= 0 && wg_leader) mbar_arrive(&empty_bar[prev]);
       // ---- epilogue: 64-column chunks through the warp's slot ----
+      // A run-time loop over the chunks, so the fused epilogue (every flag's path) is in the kernel once rather than once
+      // per chunk: unrolled, it made the kernel too large for the instruction cache and the fetch misses slowed the whole
+      // tile loop.  Only the register -> slot copy is unrolled per chunk (accumulator indices must be compile-time).
       const int row0 = m_blk * BLOCK_M + wg * 64 + wq * 16;
       const int r = lane >> 2;
-#pragma unroll
+#pragma unroll 1
       for (int c = 0; c < BN / 64; ++c) {
         __syncwarp();
 #pragma unroll
-        for (int jj = 0; jj < 8; ++jj) {
-          const int j = c * 8 + jj;
-          const int unit = jj * 2 + ((lane & 3) >> 1), within = (lane & 1) * 2;
-          *reinterpret_cast<float2*>(slot + r * 64 + ((unit ^ r) << 2) + within) = make_float2(acc[4 * j], acc[4 * j + 1]);
-          *reinterpret_cast<float2*>(slot + (r + 8) * 64 + ((unit ^ (r + 8)) << 2) + within) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        for (int cc = 0; cc < BN / 64; ++cc) {
+          if (cc != c) continue;
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = cc * 8 + jj;
+            const int unit = jj * 2 + ((lane & 3) >> 1), within = (lane & 1) * 2;
+            *reinterpret_cast<float2*>(slot + r * 64 + ((unit ^ r) << 2) + within) = make_float2(acc[4 * j], acc[4 * j + 1]);
+            *reinterpret_cast<float2*>(slot + (r + 8) * 64 + ((unit ^ (r + 8)) << 2) + within) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+          }
         }
         __syncwarp();
         if (n_blk * BN + c * 64 < p.N) gemm_epilogue_slot(p, slot, row0, n_blk * BN + c * 64, lane);

@@ -47,6 +47,9 @@ t("FFN2 plain", lambda: ops.gemm(xi, w2, b_mn_major=True, out=oh), 2.0 * M * I *
 t("FFN2 +bias+resid+dropout", lambda: ops.gemm(xi, w2, b_mn_major=True, bias=bh, resid=x, out=oh, dropout_p=0.1, dropout_seed=1), 2.0 * M * I * H)
 t("FFN2-dgrad plain (N=3072,K=768)", lambda: ops.gemm(x, w2, out=oi, M=M, N=I, K=H), 2.0 * M * I * H)
 t("FFN2-dgrad x gelu'(pre)", lambda: ops.gemm(x, w2, out=oi, dgelu_aux=oi2, M=M, N=I, K=H), 2.0 * M * I * H)
+# the pair the training step launches: the forward saves gelu'(pre), the dgrad multiplies by it
+t("FFN1 +bias+gelu (gelu'+act)", lambda: ops.gemm(x, w1, b_mn_major=True, bias=b1, gelu=True, out_pre=oi2, gelu_grad_out=True, out=oi), 2.0 * M * I * H)
+t("FFN2-dgrad x saved gelu'", lambda: ops.gemm(x, w2, out=oi, mul_aux=oi2, M=M, N=I, K=H), 2.0 * M * I * H)
 t("FFN1-dgrad plain (N=768,K=3072)", lambda: ops.gemm(xi, w1, out=oh, M=M, N=H, K=I), 2.0 * M * I * H)
 t("QKV-dgrad plain (N=768,K=2304)", lambda: ops.gemm(oqkv, wqkv, out=oh, M=M, N=H, K=3 * H), 2.0 * M * 3 * H * H)
 
