@@ -104,6 +104,7 @@ int merlot_gemm_bf16(const merlot_gemm_t* g, void* stream);
  *          ONE slice that MUST be zero on entry and is re-zeroed on exit;
  *          with d_bias_qkv != NULL the same pass adds colsum(dqkv) to it (bias gradient of the q/k/v tf.layers.dense).
  *  colsum: colsum[b,k] += (1/heads) * sum_q P[b,h,q,k]   (f32 [B,S]; caller zeroes it once per stack).
+ *  With dropout_p > 0, P above is the dropped P o Z / (1 - p) wherever it multiplies v or is summed (see the fields below).
  * ------------------------------------------------------------------------------------------------------------ */
 typedef struct merlot_attn {
   int B, S, heads, head_dim;
@@ -125,6 +126,12 @@ typedef struct merlot_attn {
    * is a vision token (segment 0) and position t >= pair_viz_len belongs to language chunk (t - pair_viz_len) / pair_chunk_len;
    * query and key exchange attention iff they share a segment or either one is a vision token.  0 = every valid pair. */
   int pair_viz_len, pair_chunk_len;
+  /* attention_probs_dropout_prob (utils/transformer.py:114-115): probs = dropout(softmax(.), p) before probs @ v, with the
+   * counter-based mask keep(seed, site, b, h, q, k) of ptx.cuh `attn_dropout_words` (restated in tests/attn_dropout_oracle.py).
+   * fwd, bwd, colsum and probs must get the same triple for one layer; lse stays that of the undropped softmax; colsum and
+   * probs sum the DROPPED probabilities (self_attn_probs is built from them, transformer.py:138).  p must lie in [0, 1)
+   * (else MERLOT_EINVAL before any launch); p = 0 runs exactly the dropout-free kernels. */
+  float dropout_p; uint64_t dropout_seed; uint32_t dropout_site;
 } merlot_attn_t;
 
 int merlot_attention_fwd(const merlot_attn_t* a, void* stream);
@@ -236,6 +243,8 @@ typedef struct merlot_stack {
   void* y;                                     /* bf16 [B*S, H] = LN_final(h_last) */
   void* act_arena;                             /* merlot_stack_activation_bytes() */
   int save_for_backward;                       /* 0: forward only (arena holds one layer) */
+  /* hidden dropout of layer l draws sites base + 2l (out-projection) and base + 2l + 1 (FFN2); attention-probability dropout
+   * draws site base + l in its own counter stream.  attention_dropout_p must lie in [0, 1) (else MERLOT_EINVAL). */
   float hidden_dropout_p; float attention_dropout_p; uint64_t dropout_seed; uint32_t dropout_site_base;
   float* attn_colsum;                          /* optional f32 [B,S]: += sum over layers,queries of head-mean probs */
   float* attn_colsum2; int attn_colsum_split; int attn_colsum_valid_q;  /* optional split by query piece (attention_log) */

@@ -113,6 +113,7 @@ class AttnDesc(C.Structure):
         ("d_bias_qkv", C.c_void_p),
         ("colsum2", C.c_void_p), ("colsum_split", C.c_int), ("colsum_valid_q", C.c_int),
         ("pair_viz_len", C.c_int), ("pair_chunk_len", C.c_int),
+        ("dropout_p", C.c_float), ("dropout_seed", C.c_uint64), ("dropout_site", C.c_uint32),
     ]
 
 

@@ -41,6 +41,11 @@ struct AttnDev {
   int colsum_split;              // 0 = no split
   int colsum_valid_q;            // 1 = only valid (non-padding) queries contribute (attention_log, modeling.py:192-193)
   int pair_P, pair_chunk;        // disable_pairwise_lang_attn (model/modeling.py:160-168); pair_chunk == 0: off
+  // attention-probability dropout (DROP instances only; utils/transformer.py:114-115): keep <=> lane16 >= drop_thresh16
+  uint32_t drop_thresh16;
+  float drop_scale;              // 1 / (1 - p)
+  uint64_t drop_seed;
+  uint32_t drop_site;
 };
 
 constexpr int MAX_MASK_WORDS = 128;  // validity bitmask for up to 4096 positions
@@ -107,7 +112,7 @@ constexpr int FK = 64;  // keys per tile
 constexpr int FWD_THREADS = 256;
 constexpr int FWD_SMEM = 16384 + 2 * 16384 + 512 + 64 + 1024;  // Q, 2 x {K, V}, masks, barriers, alignment
 
-template <bool HAS_MASK>
+template <bool HAS_MASK, bool DROP>
 __global__ void __launch_bounds__(FWD_THREADS, 2) attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_kv,
                                                                   const AttnDev p) {
   extern __shared__ uint8_t smem_raw[];
@@ -168,10 +173,34 @@ __global__ void __launch_bounds__(FWD_THREADS, 2) attn_fwd_kernel(const __grid_c
   float o[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  // dropout block index of this thread's queries {q, q + 8} (ptx.cuh attn_dropout_words) up to the key terms
+  uint64_t drop_row = 0;
+  if (DROP) {
+    const uint64_t n16 = (uint64_t)((S + 15) >> 4);
+    drop_row = ((((uint64_t)b * p.heads + h) * n16 + (uint64_t)((q0 + wg * 64 + wq * 16) >> 4)) * 8 + (lane >> 2)) * n16 * 8;
+  }
 
   mbar_wait(bar_q, 0);
   const uint32_t qa = smem_u32(sQ) + wg * 8192;
   for (int j = 0; j < n_kv; ++j) {
+    // keep bits of this key tile, bit x for accumulator element s[x] (x = 4 jj + 2 i + e), drawn while only O is live: with
+    // S live as well the no-mask instance would spill at 128 registers
+    uint32_t zq = 0;
+    if (DROP) {
+#pragma unroll
+      for (int jp = 0; jp < FK / 16; ++jp) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const uint4 r = attn_dropout_words(p.drop_seed, p.drop_site, drop_row + (uint64_t)((j * FK >> 4) + jp) * 8 + 2 * (lane & 3) + e);
+          const uint32_t w[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+          for (int i = 0; i < 2; ++i)
+#pragma unroll
+            for (int kh = 0; kh < 2; ++kh)  // word 2 (q/8 & 1) + (k/8 & 1); accumulator column group jj = 2 jp + kh
+              zq |= ((w[2 * i + kh] >> 16) >= p.drop_thresh16 ? 1u : 0u) << (4 * (2 * jp + kh) + 2 * i + e);
+        }
+      }
+    }
     mbar_wait(&bar_kv[j & 1], (uint32_t)((j >> 1) & 1));
     const uint32_t ka = smem_u32(sKV + (j & 1) * 16384), va = ka + 8192;
     float s[32];
@@ -222,6 +251,11 @@ __global__ void __launch_bounds__(FWD_THREADS, 2) attn_fwd_kernel(const __grid_c
       }
       l_run[i] = l_run[i] * f + rs;
     }
+    if (DROP) {  // P o Z after l_run took the undropped sum; the 1/(1-p) rides on the final 1/l
+#pragma unroll
+      for (int x = 0; x < 32; ++x)
+        if (!((zq >> x) & 1u)) s[x] = 0.f;
+    }
     // ---- O += P V (P from registers, V MN-major: rows are keys) ----
     wgmma_fence();
 #pragma unroll
@@ -242,7 +276,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 2) attn_fwd_kernel(const __grid_c
     quad_sum(l_run[i]);
     const int q = q0 + wg * 64 + wq * 16 + (lane >> 2) + 8 * i;
     if (!q_in[i]) continue;
-    const float inv = 1.0f / l_run[i];
+    const float inv = (DROP ? p.drop_scale : 1.0f) / l_run[i];
     bf16* dst = p.ctx + (size_t)(tok0 + q) * p.ld_ctx + h * AT_D + 2 * (lane & 3);
 #pragma unroll
     for (int jj = 0; jj < 8; ++jj)
@@ -270,7 +304,30 @@ constexpr int BWD_THREADS = 256;
 // K, V (16 KB each), 2 x {Q, dO} chunk (8 KB each), dS^T 16 KB, statistics 2 x 2 x 256 B, query mask, barriers, alignment
 constexpr int BWD_SMEM = 32768 + 32768 + 16384 + 1024 + 512 + 64 + 1024;
 
-template <bool HAS_MASK, bool DQ_ATOMIC>
+// Attention-probability dropout with keys on the accumulator rows (K3, K4): bit 4 jj + 2 i + e of the result is the keep bit of
+// accumulator element s[4 jj + 2 i + e] of this thread in the query chunk starting at q0 (ptx.cuh attn_dropout_words: word
+// 2 (q/8 & 1) + (k/8 & 1), with q/8 & 1 = jj & 1 and k/8 & 1 = i here).  drop_bh = (b heads + h) n16; drop_key = the key terms.
+__device__ __forceinline__ uint32_t attn_keep_bits_keyrows(const AttnDev& p, uint64_t drop_bh, uint64_t drop_key, uint64_t n16, int q0,
+                                                           int lane) {
+  uint32_t z = 0;
+#pragma unroll
+  for (int jp = 0; jp < BQ / 16; ++jp) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const uint64_t blk = ((drop_bh + (uint64_t)((q0 >> 4) + jp)) * 8 + 2 * (lane & 3) + e) * n16 * 8 + drop_key;
+      const uint4 r = attn_dropout_words(p.drop_seed, p.drop_site, blk);
+      const uint32_t w[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+      for (int qh = 0; qh < 2; ++qh)
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+          z |= ((w[2 * qh + i] >> 16) >= p.drop_thresh16 ? 1u : 0u) << (4 * (2 * jp + qh) + 2 * i + e);
+    }
+  }
+  return z;
+}
+
+template <bool HAS_MASK, bool DQ_ATOMIC, bool DROP>
 __global__ void __launch_bounds__(BWD_THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_kv, const __grid_constant__ CUtensorMap tm_q,
                 const __grid_constant__ CUtensorMap tm_do, const AttnDev p) {
@@ -340,6 +397,12 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_kv, const __grid_constant
 #pragma unroll
   for (int i = 0; i < 32; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
   float* dq_base = p.dq_accum + (DQ_ATOMIC ? (size_t)0 : (size_t)kt * p.dq_part_stride);
+  uint64_t drop_n16 = 0, drop_bh = 0, drop_key = 0;
+  if (DROP) {
+    drop_n16 = (uint64_t)((S + 15) >> 4);
+    drop_bh = ((uint64_t)b * p.heads + h) * drop_n16;
+    drop_key = (uint64_t)((k0 + wg * 64 + wq * 16) >> 4) * 8 + (lane >> 2);
+  }
 
   mbar_wait(bar_kv, 0);
   const uint32_t ka = smem_u32(sK) + wg * 8192, va = smem_u32(sV) + wg * 8192;
@@ -366,6 +429,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_kv, const __grid_constant
       iw[w] = range_word(q0 + 32 * w, S);                                  // query in range
       qw[w] = HAS_MASK ? s_mask[(q0 >> 5) + w] : 0xffffffffu;              // query validity
     }
+    const uint32_t zk = DROP ? attn_keep_bits_keyrows(p, drop_bh, drop_key, drop_n16, q0, lane) : 0u;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       uint32_t aw[2];
@@ -387,8 +451,14 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_kv, const __grid_constant
           // d(score)/d(q k^T) = m * scale (utils/transformer.py:109-110: scores*m - 1e10*(1-m)): a padding QUERY row keeps
           // its uniform probabilities for dV but sends nothing back into q and k.  (scale itself: dK epilogue / dQ finish)
           const float gq = ((qw[w] >> bit) & 1u) ? pr : 0.f;
-          pv[e] = pr;
-          dsv[e] = (dp[4 * jj + 2 * i + e] - dsm[col]) * gq;
+          if (DROP) {  // dV += (P o Z s) dO;  dS' = P o (Z s dP - D)
+            const float zs = ((zk >> (4 * jj + 2 * i + e)) & 1u) ? p.drop_scale : 0.f;
+            pv[e] = pr * zs;
+            dsv[e] = (dp[4 * jj + 2 * i + e] * zs - dsm[col]) * gq;
+          } else {
+            pv[e] = pr;
+            dsv[e] = (dp[4 * jj + 2 * i + e] - dsm[col]) * gq;
+          }
         }
         s[4 * jj + 2 * i] = pv[0]; s[4 * jj + 2 * i + 1] = pv[1];
         dp[4 * jj + 2 * i] = dsv[0]; dp[4 * jj + 2 * i + 1] = dsv[1];
@@ -559,7 +629,7 @@ __global__ void __launch_bounds__(256) attn_dqkv_finish_kernel(float* __restrict
 constexpr int CS_THREADS = 256;
 constexpr int CS_SMEM = 16384 + 2 * 8192 + 512 + 512 + 64 + 1024;  // K, 2 x Q chunk, statistics, query mask, barriers, alignment
 
-template <bool HAS_MASK>
+template <bool HAS_MASK, bool DROP>
 __global__ void __launch_bounds__(CS_THREADS, 2) attn_colsum_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_q,
                                                                     const AttnDev p) {
   extern __shared__ uint8_t smem_raw[];
@@ -614,6 +684,12 @@ __global__ void __launch_bounds__(CS_THREADS, 2) attn_colsum_kernel(const __grid
   const float sc2 = p.scale * LOG2E;
   const int split = p.colsum2 ? p.colsum_split : 0x7fffffff;
   float acc[2] = {0.f, 0.f}, acc2[2] = {0.f, 0.f};
+  uint64_t drop_n16 = 0, drop_bh = 0, drop_key = 0;
+  if (DROP) {
+    drop_n16 = (uint64_t)((S + 15) >> 4);
+    drop_bh = ((uint64_t)b * p.heads + h) * drop_n16;
+    drop_key = (uint64_t)((k0 + wg * 64 + wq * 16) >> 4) * 8 + (lane >> 2);
+  }
   mbar_wait(bar_k, 0);
   const uint32_t ka = smem_u32(sK) + wg * 8192;
   for (int c = 0; c < n_q; ++c) {
@@ -635,6 +711,7 @@ __global__ void __launch_bounds__(CS_THREADS, 2) attn_colsum_kernel(const __grid
       qw[w] = HAS_MASK ? s_mask[(q0 >> 5) + w] : 0xffffffffu;          // query validity
       sw[w] = range_word(q0 + 32 * w, split);                          // query < split -> colsum, else colsum2
     }
+    const uint32_t zk = DROP ? attn_keep_bits_keyrows(p, drop_bh, drop_key, drop_n16, q0, lane) : 0u;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       uint32_t aw[2], keep[2];
@@ -653,6 +730,7 @@ __global__ void __launch_bounds__(CS_THREADS, 2) attn_colsum_kernel(const __grid
           x = ((qw[w] >> bit) & 1u) ? x : 0.f;  // padding query: uniform row (zero scores)
           float pr = ex2_approx(x + nl[col]);
           pr = ((keep[w] >> bit) & 1u) ? pr : 0.f;
+          if (DROP && !((zk >> (4 * jj + 2 * i + e)) & 1u)) pr = 0.f;  // P o Z; the scale s is applied once per sum below
           if ((sw[w] >> bit) & 1u) acc[i] += pr; else acc2[i] += pr;
         }
       }
@@ -665,6 +743,7 @@ __global__ void __launch_bounds__(CS_THREADS, 2) attn_colsum_kernel(const __grid
   for (int i = 0; i < 2; ++i) {
     quad_sum(acc[i]);
     quad_sum(acc2[i]);
+    if (DROP) { acc[i] *= p.drop_scale; acc2[i] *= p.drop_scale; }
     const int kk = k0 + wg * 64 + wq * 16 + (lane >> 2) + 8 * i;
     if ((lane & 3) == 0 && k_in[i]) {
       atomicAdd(p.colsum + (size_t)b * S + kk, acc[i] / (float)p.heads);
@@ -682,6 +761,8 @@ static int check_common(const merlot_attn_t* a) {
              "attention: qkv must be [tokens, >=3H] with ld %% 8 == 0");
   MB_REQUIRE(a->pair_chunk_len >= 0 && a->pair_viz_len >= 0 && (a->pair_chunk_len == 0 || a->valid != nullptr), MERLOT_EINVAL,
              "attention: pair_chunk_len > 0 (disable_pairwise_lang_attn) needs the token-validity mask and non-negative lengths");
+  MB_REQUIRE(a->dropout_p >= 0.f && a->dropout_p < 1.f, MERLOT_EINVAL, "attention: dropout_p must lie in [0, 1) (got %g)",
+             (double)a->dropout_p);
   return MERLOT_OK;
 }
 
@@ -700,6 +781,10 @@ static void fill_dev(const merlot_attn_t* a, AttnDev* p) {
   p->colsum_split = a->colsum_split;
   p->colsum_valid_q = a->colsum_valid_q;
   p->pair_P = a->pair_viz_len; p->pair_chunk = a->pair_chunk_len;
+  // the same float32 quantisation as the hidden-dropout kernels (gemm.cu, rowwise.cu)
+  p->drop_thresh16 = (uint32_t)(a->dropout_p * 65536.0f + 0.5f);
+  p->drop_scale = 1.0f / (1.0f - a->dropout_p);
+  p->drop_seed = a->dropout_seed; p->drop_site = a->dropout_site;
 }
 
 }  // namespace mb
@@ -720,13 +805,17 @@ extern "C" int merlot_attention_fwd(const merlot_attn_t* a, void* stream_) {
   MB_REQUIRE(a->S <= MAX_MASK_WORDS * 32 - AT_N, MERLOT_ESHAPE, "attention_fwd: sequence longer than %d keys", MAX_MASK_WORDS * 32 - AT_N);
   static bool attr = false;
   if (!attr) {
-    MB_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM));
-    MB_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM));
+    MB_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM));
+    MB_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM));
+    MB_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM));
+    MB_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM));
     attr = true;
   }
   dim3 grid(ceil_div(a->S, AT_M), a->heads, a->B);
-  if (a->valid) MB_CHECK_CUDA(launch_pdl(attn_fwd_kernel<true>, grid, dim3(FWD_THREADS), FWD_SMEM, stream, tq, tkv, p));
-  else MB_CHECK_CUDA(launch_pdl(attn_fwd_kernel<false>, grid, dim3(FWD_THREADS), FWD_SMEM, stream, tq, tkv, p));
+  const bool drop = a->dropout_p > 0.f;
+  auto kern = a->valid ? (drop ? attn_fwd_kernel<true, true> : attn_fwd_kernel<true, false>)
+                       : (drop ? attn_fwd_kernel<false, true> : attn_fwd_kernel<false, false>);
+  MB_CHECK_CUDA(launch_pdl(kern, grid, dim3(FWD_THREADS), FWD_SMEM, stream, tq, tkv, p));
   MB_CHECK_LAUNCH();
   return MERLOT_OK;
 }
@@ -770,22 +859,21 @@ extern "C" int merlot_attention_bwd(const merlot_attn_t* a, void* stream_) {
   if (rc) return rc;
   rc = make_tmap_bf16_2d(&tdo, a->d_ctx, (uint64_t)a->ld_ctx, (uint64_t)tokens, (uint64_t)a->ld_ctx, 64, BQ);
   if (rc) return rc;
+  // [HAS_MASK][DQ_ATOMIC][DROP]
+  static void (*const kerns[2][2][2])(CUtensorMap, CUtensorMap, CUtensorMap, AttnDev) = {
+      {{attn_bwd_kernel<false, false, false>, attn_bwd_kernel<false, false, true>},
+       {attn_bwd_kernel<false, true, false>, attn_bwd_kernel<false, true, true>}},
+      {{attn_bwd_kernel<true, false, false>, attn_bwd_kernel<true, false, true>},
+       {attn_bwd_kernel<true, true, false>, attn_bwd_kernel<true, true, true>}}};
   static bool attr = false;
   if (!attr) {
-    MB_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
-    MB_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
-    MB_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
-    MB_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
+    for (int i = 0; i < 8; ++i)
+      MB_CHECK_CUDA(cudaFuncSetAttribute(kerns[i >> 2][(i >> 1) & 1][i & 1], cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
     attr = true;
   }
   dim3 grid(ceil_div(a->S, AT_N), a->heads, a->B);
-  if (parts > 0) {
-    if (a->valid) MB_CHECK_CUDA(launch_pdl(attn_bwd_kernel<true, false>, grid, dim3(BWD_THREADS), BWD_SMEM, stream, tkv, tq, tdo, p));
-    else MB_CHECK_CUDA(launch_pdl(attn_bwd_kernel<false, false>, grid, dim3(BWD_THREADS), BWD_SMEM, stream, tkv, tq, tdo, p));
-  } else {
-    if (a->valid) MB_CHECK_CUDA(launch_pdl(attn_bwd_kernel<true, true>, grid, dim3(BWD_THREADS), BWD_SMEM, stream, tkv, tq, tdo, p));
-    else MB_CHECK_CUDA(launch_pdl(attn_bwd_kernel<false, true>, grid, dim3(BWD_THREADS), BWD_SMEM, stream, tkv, tq, tdo, p));
-  }
+  MB_CHECK_CUDA(launch_pdl(kerns[a->valid != nullptr][parts == 0][a->dropout_p > 0.f], grid, dim3(BWD_THREADS), BWD_SMEM, stream, tkv,
+                           tq, tdo, p));
   MB_CHECK_LAUNCH();
   {
     long long slabs = ceil_div_ll(tokens, 64);
@@ -850,13 +938,17 @@ extern "C" int merlot_attention_colsum(const merlot_attn_t* a, void* stream_) {
   MB_REQUIRE(a->S <= MAX_MASK_WORDS * 32 - AT_M, MERLOT_ESHAPE, "attention_colsum: sequence longer than %d keys", MAX_MASK_WORDS * 32 - AT_M);
   static bool attr = false;
   if (!attr) {
-    MB_CHECK_CUDA(cudaFuncSetAttribute(attn_colsum_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, CS_SMEM));
-    MB_CHECK_CUDA(cudaFuncSetAttribute(attn_colsum_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, CS_SMEM));
+    MB_CHECK_CUDA(cudaFuncSetAttribute(attn_colsum_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, CS_SMEM));
+    MB_CHECK_CUDA(cudaFuncSetAttribute(attn_colsum_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, CS_SMEM));
+    MB_CHECK_CUDA(cudaFuncSetAttribute(attn_colsum_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, CS_SMEM));
+    MB_CHECK_CUDA(cudaFuncSetAttribute(attn_colsum_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, CS_SMEM));
     attr = true;
   }
   dim3 grid(ceil_div(a->S, AT_N), a->heads, a->B);
-  if (a->valid) MB_CHECK_CUDA(launch_pdl(attn_colsum_kernel<true>, grid, dim3(CS_THREADS), CS_SMEM, stream, tk, tq, p));
-  else MB_CHECK_CUDA(launch_pdl(attn_colsum_kernel<false>, grid, dim3(CS_THREADS), CS_SMEM, stream, tk, tq, p));
+  const bool drop = a->dropout_p > 0.f;
+  auto kern = a->valid ? (drop ? attn_colsum_kernel<true, true> : attn_colsum_kernel<true, false>)
+                       : (drop ? attn_colsum_kernel<false, true> : attn_colsum_kernel<false, false>);
+  MB_CHECK_CUDA(launch_pdl(kern, grid, dim3(CS_THREADS), CS_SMEM, stream, tk, tq, p));
   MB_CHECK_LAUNCH();
   return MERLOT_OK;
 }

@@ -10,10 +10,23 @@ namespace mb {
 
 constexpr int EXQ = 8;  // query rows per CTA
 
+// keep bit of probability (q, k) of head h under attention-probability dropout, one element at a time (ptx.cuh
+// attn_dropout_words; K2/K3/K4 draw the same bits four per call)
+__device__ __forceinline__ bool attn_keep_one(uint64_t seed, uint32_t site, uint32_t thresh16, int b, int heads, int h, int S, int q, int k) {
+  const uint64_t n16 = (uint64_t)((S + 15) >> 4);
+  const uint64_t blk = (((((uint64_t)b * heads + h) * n16 + (uint64_t)(q >> 4)) * 8 + (q & 7)) * n16 + (uint64_t)(k >> 4)) * 8 + (k & 7);
+  const uint4 r = attn_dropout_words(seed, site, blk);
+  const uint32_t w = ((q >> 3) & 1) ? (((k >> 3) & 1) ? r.w : r.z) : (((k >> 3) & 1) ? r.y : r.x);
+  return (w >> 16) >= thresh16;
+}
+
 // grid (ceil(S / EXQ), B); 256 threads, thread t walks keys t, t + 256, ...
+// DROP: the head mean of the dropped probabilities P o Z / (1 - p) (self_attn_probs is built from them, transformer.py:138)
+template <bool DROP>
 __global__ void __launch_bounds__(256) attn_probs_export_kernel(const bf16* __restrict__ qkv, int ld_qkv, const uint8_t* __restrict__ valid,
                                                                 const float* __restrict__ lse, float* __restrict__ out, int B, int S,
-                                                                int heads, float scale, int pair_P, int pair_chunk) {
+                                                                int heads, float scale, int pair_P, int pair_chunk, uint32_t drop_thresh16,
+                                                                float drop_scale, uint64_t drop_seed, uint32_t drop_site) {
   extern __shared__ float sm[];
   const int H = heads * 64;
   float* sq = sm;                 // [EXQ][H]   queries of this CTA (fp32), pre-scaled
@@ -37,7 +50,7 @@ __global__ void __launch_bounds__(256) attn_probs_export_kernel(const bf16* __re
   int sq_seg[EXQ];
 #pragma unroll
   for (int r = 0; r < EXQ; ++r) sq_seg[r] = seg_of(q0 + r);
-  const float inv_heads = 1.0f / (float)heads;
+  const float inv_heads = (DROP ? drop_scale : 1.0f) / (float)heads;
   for (int k = threadIdx.x; k < S; k += 256) {
     const bool vk = valid == nullptr || valid[tok0 + k] != 0;
     const int k_seg = seg_of(k);
@@ -66,7 +79,9 @@ __global__ void __launch_bounds__(256) attn_probs_export_kernel(const bf16* __re
         // utils/transformer.py:109-112: scores*m - 1e10*(1-m); a padding query row has every score equal => uniform
         const bool pair_ok = k_seg == 0 || sq_seg[r] == 0 || k_seg == sq_seg[r];
         const float s = !vq[r] ? 0.f : ((vk && pair_ok) ? dot[r] : -1e10f);
-        acc[r] += __expf(s - sl[r * heads + hh]);
+        const float pr = __expf(s - sl[r * heads + hh]);
+        if (DROP) acc[r] += attn_keep_one(drop_seed, drop_site, drop_thresh16, b, heads, hh, S, q0 + r, k) ? pr : 0.f;
+        else acc[r] += pr;
       }
     }
 #pragma unroll
@@ -86,18 +101,25 @@ extern "C" int merlot_attention_probs(const merlot_attn_t* a, float* probs_bss, 
              "attention_probs: head size 64, ld_qkv %% 8 == 0");
   MB_REQUIRE(a->pair_chunk_len >= 0 && a->pair_viz_len >= 0 && (a->pair_chunk_len == 0 || a->valid != nullptr), MERLOT_EINVAL,
              "attention_probs: pair_chunk_len > 0 (disable_pairwise_lang_attn) needs the token-validity mask");
+  MB_REQUIRE(a->dropout_p >= 0.f && a->dropout_p < 1.f, MERLOT_EINVAL, "attention_probs: dropout_p must lie in [0, 1) (got %g)",
+             (double)a->dropout_p);
   const int H = a->heads * 64;
   const size_t smem = (size_t)(EXQ * H + EXQ * a->heads) * sizeof(float);
   MB_REQUIRE(smem <= 200 * 1024, MERLOT_ESHAPE, "attention_probs: hidden size too large");
   static size_t attr = 0;
   if (smem > attr) {
-    MB_CHECK_CUDA(cudaFuncSetAttribute(attn_probs_export_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    MB_CHECK_CUDA(cudaFuncSetAttribute(attn_probs_export_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    MB_CHECK_CUDA(cudaFuncSetAttribute(attn_probs_export_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr = smem;
   }
   dim3 grid(ceil_div(a->S, EXQ), a->B);
-  attn_probs_export_kernel<<<grid, 256, smem, stream>>>(reinterpret_cast<const bf16*>(a->qkv), a->ld_qkv,
-                                                        reinterpret_cast<const uint8_t*>(a->valid), a->lse, probs_bss, a->B, a->S,
-                                                        a->heads, a->scale, a->pair_viz_len, a->pair_chunk_len);
+  // the same float32 quantisation as K2/K3/K4 (attention.cu fill_dev)
+  const uint32_t th = (uint32_t)(a->dropout_p * 65536.0f + 0.5f);
+  const float ds = 1.0f / (1.0f - a->dropout_p);
+  auto kern = a->dropout_p > 0.f ? attn_probs_export_kernel<true> : attn_probs_export_kernel<false>;
+  kern<<<grid, 256, smem, stream>>>(reinterpret_cast<const bf16*>(a->qkv), a->ld_qkv, reinterpret_cast<const uint8_t*>(a->valid), a->lse,
+                                    probs_bss, a->B, a->S, a->heads, a->scale, a->pair_viz_len, a->pair_chunk_len, th, ds,
+                                    a->dropout_seed, a->dropout_site);
   MB_CHECK_LAUNCH();
   return MERLOT_OK;
 }

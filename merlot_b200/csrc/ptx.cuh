@@ -303,4 +303,15 @@ __device__ __forceinline__ uint32_t dropout_keep8(uint64_t seed, uint32_t site, 
   return m;
 }
 
+// Attention-probability dropout: one Philox4x32-7 call per 2x2 block {q, q+8} x {k, k+8} (q % 16 < 8, k % 16 < 8), which is
+// exactly what one thread holds of an m64 wgmma accumulator with either queries or keys on the rows.
+//   blk = ((((b heads + h) n16 + q/16) 8 + q%8) n16 + k/16) 8 + k%8,  n16 = ceil(S / 16)
+//   counter = (blk lo, blk hi, site, "ATTN"), key = seed; word 2 ((q/8)&1) + ((k/8)&1) decides (q, k):
+//   keep <=> (word >> 16) >= thresh16.
+// The fourth counter word keeps this stream disjoint from dropout_keep8's ("MERL").  tests/attn_dropout_oracle.py restates it.
+__device__ __forceinline__ uint4 attn_dropout_words(uint64_t seed, uint32_t site, uint64_t blk) {
+  return philox4x32_7(make_uint4((uint32_t)blk, (uint32_t)(blk >> 32), site, 0x4154544eu),
+                      make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
+}
+
 }  // namespace mb

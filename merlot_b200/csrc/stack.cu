@@ -76,8 +76,8 @@ static int check_stack(const merlot_stack_t* s) {
              s->H, s->heads);
   MB_REQUIRE(s->H % 8 == 0 && s->I % 8 == 0 && s->H <= 1024, MERLOT_ESHAPE, "stack: H, I must be multiples of 8 and H <= 1024");
   MB_REQUIRE(s->layer_params && s->h_in && s->act_arena && s->final_gamma && s->final_beta, MERLOT_EINVAL, "stack: null pointer");
-  MB_REQUIRE(s->attention_dropout_p == 0.f, MERLOT_ENOTIMPL,
-             "stack: attention_probs_dropout_prob > 0 is not provided (0.0 in every shipped config; utils/transformer.py:114-115)");
+  MB_REQUIRE(s->attention_dropout_p >= 0.f && s->attention_dropout_p < 1.f, MERLOT_EINVAL,
+             "stack: attention_probs_dropout_prob must lie in [0, 1) (got %g)", (double)s->attention_dropout_p);
   return MERLOT_OK;
 }
 
@@ -178,6 +178,8 @@ extern "C" int merlot_stack_forward(const merlot_stack_t* s, void* stream_) {
       a.B = s->B; a.S = s->S; a.heads = s->heads; a.head_dim = 64; a.qkv = A.qkv; a.ld_qkv = 3 * H; a.valid = s->valid;
       a.pair_viz_len = s->pair_viz_len; a.pair_chunk_len = s->pair_chunk_len;
       a.scale = 0.125f; a.ctx = A.ctx; a.ld_ctx = H; a.lse = A.lse;
+      // utils/transformer.py:114-115; the colsum / probs calls below see the same mask (self_attn_probs is post-dropout)
+      a.dropout_p = s->attention_dropout_p; a.dropout_seed = s->dropout_seed; a.dropout_site = s->dropout_site_base + l;
       RC(merlot_attention_fwd(&a, st));
       if (s->attn_colsum) {
         a.colsum = s->attn_colsum;
@@ -324,6 +326,7 @@ extern "C" int merlot_stack_backward(const merlot_stack_t* s, void* stream_) {
       a.pair_viz_len = s->pair_viz_len; a.pair_chunk_len = s->pair_chunk_len;
       a.scale = 0.125f; a.ctx = A.ctx; a.ld_ctx = H; a.lse = A.lse; a.d_ctx = dtmp; a.dsum = dsum; a.dq_accum = dq_acc;
       a.ld_dq = H; a.dqkv = dqkv; a.ld_dqkv = 3 * H; a.d_bias_qkv = P.g_b_qkv;  // bias gradient fused into the finish pass
+      a.dropout_p = s->attention_dropout_p; a.dropout_seed = s->dropout_seed; a.dropout_site = s->dropout_site_base + l;
       RC(merlot_attention_bwd(&a, st));
     }
     // ---- QKV projection ----

@@ -94,7 +94,8 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn_major: bool = False, b_mn_maj
     return out
 
 
-def _attn_desc(qkv: torch.Tensor, B: int, S: int, heads: int, valid: Optional[torch.Tensor], pair=(0, 0)) -> L.AttnDesc:
+def _attn_desc(qkv: torch.Tensor, B: int, S: int, heads: int, valid: Optional[torch.Tensor], pair=(0, 0),
+               dropout=(0.0, 0, 0)) -> L.AttnDesc:
     _require_cuda(qkv, valid)
     assert qkv.dtype == torch.bfloat16 and qkv.dim() == 2 and qkv.stride(1) == 1 and qkv.shape[0] == B * S
     a = L.AttnDesc()
@@ -105,13 +106,16 @@ def _attn_desc(qkv: torch.Tensor, B: int, S: int, heads: int, valid: Optional[to
         a.valid = valid.data_ptr()
     a.scale = 1.0 / (a.head_dim ** 0.5)
     a.pair_viz_len, a.pair_chunk_len = int(pair[0]), int(pair[1])  # disable_pairwise_lang_attn (0, 0 = off)
+    # attention-probability dropout (p, seed, site); one layer's forward, backward, colsum and probs take the same triple
+    a.dropout_p, a.dropout_seed, a.dropout_site = float(dropout[0]), int(dropout[1]), int(dropout[2])
     return a
 
 
 def attention_fwd(qkv: torch.Tensor, B: int, S: int, heads: int, valid: Optional[torch.Tensor] = None,
-                  ctx: Optional[torch.Tensor] = None, lse: Optional[torch.Tensor] = None, pair=(0, 0)):
-    """K2: ctx[B*S,H] = softmax(mask(q k^T / sqrt(d))) v, reading q/k/v in place from the fused qkv buffer."""
-    a = _attn_desc(qkv, B, S, heads, valid, pair)
+                  ctx: Optional[torch.Tensor] = None, lse: Optional[torch.Tensor] = None, pair=(0, 0), dropout=(0.0, 0, 0)):
+    """K2: ctx[B*S,H] = softmax(mask(q k^T / sqrt(d))) v, reading q/k/v in place from the fused qkv buffer.
+    dropout=(p, seed, site): the probabilities are dropped with p before the product with v (lse stays undropped)."""
+    a = _attn_desc(qkv, B, S, heads, valid, pair, dropout)
     H = heads * a.head_dim
     if ctx is None:
         ctx = torch.empty((B * S, H), dtype=torch.bfloat16, device=qkv.device)
@@ -130,11 +134,11 @@ def attention_bwd_workspace(B: int, S: int, heads: int, device) -> torch.Tensor:
 
 
 def attention_bwd(qkv, ctx, d_ctx, lse, B, S, heads, valid=None, dqkv=None, dq_accum=None, dsum=None, pair=(0, 0),
-                  d_bias_qkv=None):
+                  d_bias_qkv=None, dropout=(0.0, 0, 0)):
     """K3: dqkv[B*S,3H] from d_ctx.  dq_accum: fp32 workspace of merlot_attention_bwd_workspace_bytes (see the header);
     in atomic mode (long sequences) it must be zero on entry and is returned zeroed.  d_bias_qkv: optional fp32 [3H] that
-    the column sums of dqkv (the gradient of the fused q/k/v bias) are added to."""
-    a = _attn_desc(qkv, B, S, heads, valid, pair)
+    the column sums of dqkv (the gradient of the fused q/k/v bias) are added to.  dropout: the forward's (p, seed, site)."""
+    a = _attn_desc(qkv, B, S, heads, valid, pair, dropout)
     H = heads * a.head_dim
     dev = qkv.device
     if dqkv is None:
@@ -158,9 +162,10 @@ def attention_bwd(qkv, ctx, d_ctx, lse, B, S, heads, valid=None, dqkv=None, dq_a
     return dqkv
 
 
-def attention_probs(qkv, lse, B, S, heads, valid=None, out=None, pair=(0, 0)):
-    """Export path: head-mean probabilities [B,S,S] fp32 of one layer (one layer of `self_attn_probs`)."""
-    a = _attn_desc(qkv, B, S, heads, valid, pair)
+def attention_probs(qkv, lse, B, S, heads, valid=None, out=None, pair=(0, 0), dropout=(0.0, 0, 0)):
+    """Export path: head-mean probabilities [B,S,S] fp32 of one layer (one layer of `self_attn_probs`), after the
+    forward's dropout=(p, seed, site)."""
+    a = _attn_desc(qkv, B, S, heads, valid, pair, dropout)
     if out is None:
         out = torch.empty((B, S, S), dtype=torch.float32, device=qkv.device)
     a.lse = lse.data_ptr()
@@ -168,11 +173,17 @@ def attention_probs(qkv, lse, B, S, heads, valid=None, out=None, pair=(0, 0)):
     return out
 
 
-def attention_colsum(qkv, lse, colsum, B, S, heads, valid=None, pair=(0, 0)):
-    """K4: colsum[B,S] += mean_h sum_q P[b,h,q,k] (recomputed from q,k,lse)."""
-    a = _attn_desc(qkv, B, S, heads, valid, pair)
+def attention_colsum(qkv, lse, colsum, B, S, heads, valid=None, pair=(0, 0), dropout=(0.0, 0, 0), colsum2=None, split=0,
+                     valid_q=False):
+    """K4: colsum[B,S] += mean_h sum_q P[b,h,q,k] (recomputed from q,k,lse), P after the forward's dropout=(p, seed, site).
+    With colsum2, queries >= split add into colsum2 instead; valid_q: padding queries add nothing (attention_log)."""
+    a = _attn_desc(qkv, B, S, heads, valid, pair, dropout)
     assert colsum.dtype == torch.float32 and colsum.numel() == B * S
     a.lse, a.colsum = lse.data_ptr(), colsum.data_ptr()
+    if colsum2 is not None:
+        assert colsum2.dtype == torch.float32 and colsum2.numel() == B * S
+        a.colsum2, a.colsum_split = colsum2.data_ptr(), int(split)
+    a.colsum_valid_q = int(valid_q)
     L.check(L.lib().merlot_attention_colsum(C.byref(a), _stream()))
     return colsum
 
