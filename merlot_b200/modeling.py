@@ -30,6 +30,8 @@ PADDING = 0
 START = 2
 
 _SITE_VIT, _SITE_LANGONLY, _SITE_JOINT, _SITE_EMB_LO, _SITE_EMB_J = 0, 100, 200, 300, 301
+# VCR classifier towers (merlot_b200/vcr.py cls_head): dropout of each tower's input and of its hidden layer
+_SITE_VCR_ANS_IN, _SITE_VCR_ANS_HID, _SITE_VCR_RAT_IN, _SITE_VCR_RAT_HID = 400, 401, 402, 403
 
 
 def get_shape_list_rank(t: torch.Tensor, expected_rank, name="tensor"):

@@ -6,8 +6,12 @@ elements so every slice is 256-byte (fp32) / 128-byte (bf16) aligned and usable 
 
 Storage differs from the TF variables in three places (converted by load_tf_dict / to_tf_dict):
   * query/key/value kernels [H,H] x3 are fused into `.../qkv/kernel` [H,3H] (and biases into [3H]);
-  * the temporal `logits` layer [H,4] is zero-padded to [H,8] so its rows are 16-byte aligned for TMA;
+  * dense layers with fewer than 8 outputs (the temporal `logits` [H,4], VCR's `classifier_mlp1` [H/2,1]) are zero-padded
+    to 8 columns so their rows are 16-byte aligned for TMA; `Entry.ref_cols` records how many columns the reference has;
   * the patch conv kernel [P,P,3,H] is stored as the im2col matrix [P*P*3, H] (same memory order).
+
+`task` selects the variable set of one reference graph: "pretrain" (model/modeling.py model_fn, every head) or "vcr"
+(downstream/vcr/modeling.py model_fn: MerlotModel(mask_input=False) + the answer / rationale classifier towers).
 """
 from __future__ import annotations
 
@@ -22,6 +26,9 @@ from . import ops
 
 PAD = 64
 TEMPORAL_PAD_N = 8
+TASKS = ("pretrain", "vcr")
+VCR_TOWERS = ("answer_cls", "rationale_cls")
+VCR_BIAS_PI = 0.25  # cls_head(hidden_state, bias_pi=0.25), downstream/vcr/modeling.py:77
 
 
 @dataclass
@@ -33,15 +40,16 @@ class Entry:
     numel: int = 0
     padded: int = 0
     hyper: Tuple = ()
+    ref_cols: int = 0           # > 0: the last dim is zero-padded; the reference variable has this many columns
 
 
-def _entries(cfg: dict) -> List[Entry]:
+def _entries(cfg: dict, task: str = "pretrain") -> List[Entry]:
     H, I, V = cfg["hidden_size"], cfg["intermediate_size"], cfg["vocab_size"]
     P = cfg["patch_size"]
     out: List[Entry] = []
 
-    def add(name, shape, tf_names=None):
-        out.append(Entry(name, tuple(shape), tuple(tf_names) if tf_names else (name,)))
+    def add(name, shape, tf_names=None, ref_cols=0):
+        out.append(Entry(name, tuple(shape), tuple(tf_names) if tf_names else (name,), ref_cols=ref_cols))
 
     def ln(scope):
         add(f"{scope}/gamma", (H,))
@@ -80,6 +88,15 @@ def _entries(cfg: dict) -> List[Entry]:
     add("vision_backbone/final_pe/cls_emb", (1, H))
     ln("vision_backbone/LayerNorm_final_ln")
     add("word_embeddings/word_embeddings", (V, H))
+    if task == "vcr":  # mask_input=False: no language-only encoder, no masking, no pretraining heads
+        add("position_embeddings/position_embeddings", (cfg["max_position_embeddings"], H))
+        ln("position_embeddings/LayerNorm_embed_norm")
+        stack("encoder", cfg["num_hidden_layers"])
+        for tower in VCR_TOWERS:  # downstream/vcr/modeling.py:86-121, in creation order
+            lin(f"{tower}/classifier_mlp0", H, H // 2)
+            add(f"{tower}/classifier_mlp1/kernel", (H // 2, TEMPORAL_PAD_N), ref_cols=1)
+            add(f"{tower}/classifier_mlp1/bias", (TEMPORAL_PAD_N,), ref_cols=1)
+        return out
     for sc in ("position_embeddings", "langonly_embeddings"):
         add(f"{sc}/position_embeddings", (cfg["max_position_embeddings"], H))
         ln(f"{sc}/LayerNorm_embed_norm")
@@ -99,8 +116,8 @@ def _entries(cfg: dict) -> List[Entry]:
     for t in ("lang_viz", "viz_viz"):
         lin(f"{t}_temporal/intermediate", 2 * H, H)
         ln(f"{t}_temporal/LayerNorm_ln0")
-        add(f"{t}_temporal/logits/kernel", (H, TEMPORAL_PAD_N))
-        add(f"{t}_temporal/logits/bias", (TEMPORAL_PAD_N,))
+        add(f"{t}_temporal/logits/kernel", (H, TEMPORAL_PAD_N), ref_cols=4)
+        add(f"{t}_temporal/logits/bias", (TEMPORAL_PAD_N,), ref_cols=4)
     return out
 
 
@@ -179,12 +196,16 @@ def hyper_for(tf_name: str, optimizer_cfg: dict) -> Tuple[float, float, float, f
 class ParamStore:
     """Flat arenas + named views.  `optimizer_cfg` fixes the hyper-parameter grouping (needed only for training)."""
 
-    def __init__(self, model_cfg: dict, device="cuda", optimizer_cfg: Optional[dict] = None, with_optimizer_state=True):
+    def __init__(self, model_cfg: dict, device="cuda", optimizer_cfg: Optional[dict] = None, with_optimizer_state=True,
+                 task: str = "pretrain"):
         # resnet_layers != [] selects the hybrid ResNet-lite stem (utils/vision_transformer.py:206-223); forward and backward
         # are provided (K13), its variables follow the reference's creation order (stem_variables).
+        if task not in TASKS:
+            raise ValueError(f"ParamStore task must be one of {TASKS}, got {task!r}")
         self.cfg = model_cfg
+        self.task = task
         self.device = torch.device(device)
-        ents = _entries(model_cfg)
+        ents = _entries(model_cfg, task)
         ocfg = optimizer_cfg or {"learning_rate": 0.0, "param_overrides": [
             [["LayerNorm", "layer_norm", "GroupNorm", "bias"], {"weight_decay_rate": 0}]]}
         for e in ents:
@@ -274,10 +295,10 @@ class ParamStore:
         return self._view(self.pb, name)
 
     def num_params(self) -> int:
-        """Trainable scalars as the reference counts them (padding and the 4 dead logits columns excluded)."""
+        """Trainable scalars as the reference counts them (padding and the zero-padded columns excluded)."""
         n = 0
         for e in self.entries.values():
-            n += e.numel if "temporal/logits" not in e.name else e.numel // 2
+            n += e.numel if not e.ref_cols else e.numel // e.shape[-1] * e.ref_cols
         return n
 
     def sync_bf16(self):
@@ -301,9 +322,9 @@ class ParamStore:
                 dst = self.P(e.name)
                 if len(e.tf_names) == 3:
                     src = torch.cat([d[t] for t in e.tf_names], dim=-1)
-                elif "temporal/logits" in e.name:
+                elif e.ref_cols:
                     src = torch.zeros(e.shape, dtype=torch.float32)
-                    src[..., :4] = d[e.tf_names[0]]
+                    src[..., :e.ref_cols] = d[e.tf_names[0]]
                 else:
                     src = d[e.tf_names[0]].reshape(e.shape)
                 dst.copy_(src.to(torch.float32))
@@ -323,8 +344,8 @@ class ParamStore:
             if len(e.tf_names) == 3:
                 for nm, part in zip(e.tf_names, t.chunk(3, dim=-1)):
                     out[nm] = part.contiguous()
-            elif "temporal/logits" in e.name:
-                out[e.tf_names[0]] = t[..., :4].contiguous()
+            elif e.ref_cols:
+                out[e.tf_names[0]] = t[..., :e.ref_cols].contiguous()
             elif e.name.endswith("vision_transformer/conv2d/kernel"):
                 Pp = self.cfg["patch_size"]
                 out[e.tf_names[0]] = t.reshape(Pp, Pp, 3, -1)
@@ -341,7 +362,8 @@ class ParamStore:
         return out
 
     def init_reference(self, seed: int = 0):
-        """Reference initialisers (truncated normal 0.02 / variance-scaling patch kernel / LN 1,0 / zero biases)."""
+        """Reference initialisers (truncated normal 0.02 / variance-scaling patch kernel / LN 1,0 / zero biases; the VCR
+        towers' output bias is -log((1 - pi) / pi), downstream/vcr/modeling.py:71)."""
         g = torch.Generator().manual_seed(seed)
         std = self.cfg.get("initializer_range", 0.02)
         with torch.no_grad():
@@ -351,13 +373,15 @@ class ParamStore:
                     t = torch.ones(e.shape)
                 elif leaf in ("beta", "bias", "output_bias"):
                     t = torch.zeros(e.shape)
+                    if e.name.endswith("_cls/classifier_mlp1/bias"):
+                        t[0] = -math.log((1 - VCR_BIAS_PI) / VCR_BIAS_PI)
                 else:
                     s_ = std
                     if _CONV_KERNEL.search(e.name):  # tf.variance_scaling_initializer(): fan_in = kh*kw*cin = rows of the 2-D view
                         s_ = math.sqrt(1.0 / e.shape[0]) / 0.87962566103423978
                     t = torch.empty(e.shape)
                     torch.nn.init.trunc_normal_(t, 0.0, s_, -2 * s_, 2 * s_, generator=g)
-                    if "temporal/logits/kernel" in e.name:
-                        t[:, 4:] = 0
+                    if e.ref_cols:
+                        t[:, e.ref_cols:] = 0
                 self.P(e.name).copy_(t)
         self.sync_bf16()

@@ -3,6 +3,7 @@
   * `synthetic_batch`  -- features with the dataloader's output contract (model/dataloader.py:56-126,210-272):
                           images [b*n,H,W,3] bf16, input_ids [b,n,Lc] int32 (START first, zero padded),
                           shuffled_idx_img [B*g] int32, video_src_ids [b,n] int32.
+  * `synthetic_vcr_batch` -- the same for VCR fine-tuning (downstream/vcr/dataloader_joint.py:135-189,257-271).
   * `model_fn_builder` -- same name and call shape as the reference; returns a model_fn(features, labels, mode, params)
                           that builds MerlotModel(is_training=True, mask_input=True), sums lang + contr + temp losses
                           (modeling.py:700-713) and exposes `train_op()` = backward + gradient all-reduce + AdamW.
@@ -112,6 +113,28 @@ def synthetic_batch(config: NeatConfig, batch_size: int, seed: int = 0, device="
     return {k: v.to(device) for k, v in feats.items()}
 
 
+VCR_MAX_NUM_TOKENS = 184  # downstream/vcr/dataloader_joint.py:135
+
+
+def synthetic_vcr_batch(config: NeatConfig, questions: int, seed: int = 0, device="cuda") -> Dict[str, torch.Tensor]:
+    """Training features of `questions` VCR questions with the joint dataloader's shapes: images [2q, H, W, 3] bf16 uniform
+    [0,1) ordered [q0 answer, q0 rationale, q1 answer, ...]; lm_input [2q*4, 184] int32, every text START followed by ids in
+    [100, vocab) and a zero-padded tail; lm_targets [2q] int32 in [0, 4).  Synthetic ids stand in for the prompts, contexts
+    and answer choices (dataloader_joint.py:167-181)."""
+    m = config.model
+    Hh, Ww = m["image_size"]
+    L = VCR_MAX_NUM_TOKENS
+    g = torch.Generator().manual_seed(seed)
+    images = torch.rand(2 * questions, Hh, Ww, 3, generator=g).to(torch.bfloat16)
+    ids = torch.randint(100, m["vocab_size"], (2 * questions * 4, L), generator=g, dtype=torch.int32)
+    ids[:, 0] = START
+    lens = torch.randint(16, L + 1, (2 * questions * 4,), generator=g)
+    ids = ids * (torch.arange(L)[None] < lens[:, None]).int()
+    targets = torch.randint(0, 4, (2 * questions,), generator=g, dtype=torch.int32)
+    feats = {"images": images, "lm_input": ids, "lm_targets": targets}
+    return {k: v.to(device) for k, v in feats.items()}
+
+
 class StepSpec:
     """What TPUEstimatorSpec carries in the reference: loss, metrics and the train op."""
 
@@ -121,6 +144,51 @@ class StepSpec:
     @property
     def loss(self):
         return sum(float(x) for x in self.loss_parts)
+
+
+def backward_and_apply(model, optimizer, dist: Optional[DataParallel], *, metrics: dict, skip=(), vit_grad_buckets: int = 4,
+                       d_hidden_state=None):
+    """The train op of every training step: model.backward (with an external head's gradient `d_hidden_state`, if any, whose
+    parameter gradients are already in store.g), the gradient mean over replicas and AdamW.  With clip_norm > 0 the pre-clip
+    global norm goes into metrics['gradnorms/_overall']."""
+    store = optimizer.store
+    world = dist.world if dist is not None else 1
+    pending = []
+    if optimizer.clip_norm > 0.0:  # local clip needs the complete local gradient first: no bucket overlap
+        model.backward(d_hidden_state=d_hidden_state)
+        metrics["gradnorms/_overall"] = optimizer.clip_gradients()
+        if world > 1:
+            dist.all_reduce_grads(store.g)
+        optimizer.apply_gradients(grad_scale=1.0 / world, skip=skip, zero_grad=True)
+    elif world > 1:
+        # Bucketed, overlapped gradient all-reduce (CrossShardOptimizer's mean, utils/optimization.py:241-245; the 1/world
+        # is folded into AdamW).  Bucket 0 = everything outside the ViT, reduced while the ViT backward runs; the ViT is
+        # walked in layer groups top-down and each group's kernels are reduced as soon as that group has run, so only
+        # the last group's bucket is exposed.  AdamW updates every bucket as its reduction lands.
+        groups, vit_ranges = store.vit_buckets(vit_grad_buckets)
+        vit_pending = []
+
+        def on_group(k):
+            if k + 1 < len(groups):
+                vit_pending.append(dist.all_reduce_ranges_async(store.g, vit_ranges[k]))
+
+        def on_rest():
+            pending.extend(dist.all_reduce_ranges_async(store.g, store.rest_ranges))
+            dist.reserve_sms(True)  # the ViT backward is enqueued (and runs) under the collectives
+
+        model.backward(on_non_vit_grads_ready=on_rest, vit_layer_groups=groups, on_vit_group_done=on_group,
+                       d_hidden_state=d_hidden_state)
+        dist.reserve_sms(False)
+        vit_pending.append(dist.all_reduce_ranges_async(store.g, vit_ranges[-1]))
+        dist.wait_all(pending)
+        optimizer.apply_gradients(grad_scale=1.0 / world, skip=skip, zero_grad=True, only=store.rest_ranges, advance=False)
+        for k, hs in enumerate(vit_pending):
+            dist.wait_all(hs)
+            optimizer.apply_gradients(grad_scale=1.0 / world, skip=skip, zero_grad=True, only=vit_ranges[k],
+                                      advance=(k + 1 == len(vit_pending)))
+    else:
+        model.backward(d_hidden_state=d_hidden_state)
+        optimizer.apply_gradients(grad_scale=1.0 / world, skip=skip, zero_grad=True)
 
 
 def model_fn_builder(config: NeatConfig, *, store: Optional[ParamStore] = None, dist: Optional[DataParallel] = None,
@@ -163,42 +231,7 @@ def model_fn_builder(config: NeatConfig, *, store: Optional[ParamStore] = None, 
             losses.update({f"attn/{k}": v for k, v in model.attention_log.items()})
 
         def train_op():
-            world = dist.world if dist is not None else 1
-            pending = []
-            if optimizer.clip_norm > 0.0:  # local clip needs the complete local gradient first: no bucket overlap
-                model.backward()
-                losses["gradnorms/_overall"] = optimizer.clip_gradients()
-                if world > 1:
-                    dist.all_reduce_grads(store.g)
-                optimizer.apply_gradients(grad_scale=1.0 / world, skip=skip, zero_grad=True)
-            elif world > 1:
-                # Bucketed, overlapped gradient all-reduce (CrossShardOptimizer's mean, utils/optimization.py:241-245; the 1/world
-                # is folded into AdamW).  Bucket 0 = everything outside the ViT, reduced while the ViT backward runs; the ViT is
-                # walked in layer groups top-down and each group's kernels are reduced as soon as that group has run, so only
-                # the last group's bucket is exposed.  AdamW updates every bucket as its reduction lands.
-                groups, vit_ranges = store.vit_buckets(vit_grad_buckets)
-                vit_pending = []
-
-                def on_group(k):
-                    if k + 1 < len(groups):
-                        vit_pending.append(dist.all_reduce_ranges_async(store.g, vit_ranges[k]))
-
-                def on_rest():
-                    pending.extend(dist.all_reduce_ranges_async(store.g, store.rest_ranges))
-                    dist.reserve_sms(True)  # the ViT backward is enqueued (and runs) under the collectives
-
-                model.backward(on_non_vit_grads_ready=on_rest, vit_layer_groups=groups, on_vit_group_done=on_group)
-                dist.reserve_sms(False)
-                vit_pending.append(dist.all_reduce_ranges_async(store.g, vit_ranges[-1]))
-                dist.wait_all(pending)
-                optimizer.apply_gradients(grad_scale=1.0 / world, skip=skip, zero_grad=True, only=store.rest_ranges, advance=False)
-                for k, hs in enumerate(vit_pending):
-                    dist.wait_all(hs)
-                    optimizer.apply_gradients(grad_scale=1.0 / world, skip=skip, zero_grad=True, only=vit_ranges[k],
-                                              advance=(k + 1 == len(vit_pending)))
-            else:
-                model.backward()
-                optimizer.apply_gradients(grad_scale=1.0 / world, skip=skip, zero_grad=True)
+            backward_and_apply(model, optimizer, dist, metrics=losses, skip=skip, vit_grad_buckets=vit_grad_buckets)
 
         return StepSpec(model, (lang_loss, contr_loss, temp_loss), losses, train_op)
 
@@ -207,16 +240,27 @@ def model_fn_builder(config: NeatConfig, *, store: Optional[ParamStore] = None, 
     return model_fn
 
 
+def _step_for(config: NeatConfig):
+    """(model_fn_builder, synthetic batch) of the configured task: downstream.task 'vcr' fine-tunes on VCR
+    (downstream/vcr/train.py), anything else pretrains (model/train.py)."""
+    if config.downstream.get("task") == "vcr":
+        from .vcr import vcr_model_fn_builder
+        return vcr_model_fn_builder, synthetic_vcr_batch
+    return model_fn_builder, synthetic_batch
+
+
 def main(argv=None):
-    """`python -m merlot_b200.train configs/merlot.yaml` -- the role of model/train.py:9-26 on synthetic data."""
+    """`python -m merlot_b200.train configs/merlot.yaml` (or merlot_vcr.yaml) -- the role of model/train.py:9-26 and
+    downstream/vcr/train.py on synthetic data."""
     config = NeatConfig.from_args("Train MERLOT (H100-native)", argv=argv)
     dist = DataParallel() if int(os.environ.get("WORLD_SIZE", "1")) > 1 else None
     if torch.cuda.is_available():
         torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
-    model_fn = model_fn_builder(config, dist=dist)
+    builder, make_batch = _step_for(config)
+    model_fn = builder(config, dist=dist)
     per_rank = max(1, config.device.get("train_batch_size", 8) // (dist.world if dist else 1))
     for step in range(config.optimizer.get("num_train_steps", 10)):
-        feats = synthetic_batch(config, per_rank, seed=step + (dist.rank if dist else 0) * 100003)
+        feats = make_batch(config, per_rank, seed=step + (dist.rank if dist else 0) * 100003)
         spec = model_fn(feats, None, "train", None)
         spec.train_op()
         if step % 10 == 0 and (dist is None or dist.rank == 0):
