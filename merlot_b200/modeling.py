@@ -67,7 +67,7 @@ def _layer_params(store: ParamStore, scope: str, layers: int):
     key = ("_lp", scope, layers)
     if key in store._bufs:
         return store._bufs[key]
-    arr = (L.LayerParams * layers)()
+    arr = (L.merlot_layer_params_t * layers)()
     for l in range(layers):
         ls = f"{scope}/layer{l:02d}"
         lp = arr[l]
@@ -93,10 +93,10 @@ class _Stack:
         if H % heads != 0 or H // heads != 64:
             raise ValueError("passed in a tensor of shape {} when size_per_head={} and num_attention_heads={}".format(
                 (B * S, H), H // max(heads, 1), heads) + " (this build provides size_per_head=64 only)")
-        d = L.StackDesc()
+        d = L.merlot_stack_t()
         d.B, d.S, d.H, d.I, d.heads, d.layers = B, S, H, I, heads, layers
         self._lp = _layer_params(store, scope, layers)
-        d.layer_params = self._lp
+        d.layer_params = C.addressof(self._lp)
         fg, fb = f"{scope}/LayerNorm_ln_final/gamma", f"{scope}/LayerNorm_ln_final/beta"
         d.final_gamma, d.final_beta = store.P(fg).data_ptr(), store.P(fb).data_ptr()
         d.d_final_gamma, d.d_final_beta = store.G(fg).data_ptr(), store.G(fb).data_ptr()
@@ -118,7 +118,7 @@ class _Stack:
         self.d, self.bufs, self.tag, self.keep = d, bufs, tag, (valid, h_in, colsum, probs)
 
     def forward(self):
-        L.check(L.lib().merlot_stack_forward(C.byref(self.d), ops._stream()))
+        L.lib().merlot_stack_forward(C.byref(self.d), ops._stream())
         return self.y
 
     def backward(self, dy, dh_in, layer_groups=None, on_group_done=None):
@@ -129,12 +129,12 @@ class _Stack:
         d.dy, d.dh_in, d.scratch = dy.data_ptr(), dh_in.data_ptr(), scratch.data_ptr()
         if not layer_groups:
             d.bwd_lo, d.bwd_hi = 0, 0
-            L.check(L.lib().merlot_stack_backward(C.byref(d), ops._stream()))
+            L.lib().merlot_stack_backward(C.byref(d), ops._stream())
             return dh_in
         assert layer_groups[0][1] == d.layers and layer_groups[-1][0] == 0
         for k, (lo, hi) in enumerate(layer_groups):
             d.bwd_lo, d.bwd_hi = lo, hi
-            L.check(L.lib().merlot_stack_backward(C.byref(d), ops._stream()))
+            L.lib().merlot_stack_backward(C.byref(d), ops._stream())
             if on_group_done is not None:
                 on_group_done(k)
         d.bwd_lo, d.bwd_hi = 0, 0
@@ -356,9 +356,8 @@ class MerlotModel(object):
         self._attn_log = None
         if self._log_attention_probs:
             out4 = bf.get("joint.attn_log", (4,), torch.float32)
-            L.check(L.lib().merlot_attention_log_blocks(C.c_void_p(c_viz.data_ptr()), C.c_void_p(c_lang.data_ptr()),
-                                                        C.c_void_p(valid_j.data_ptr()), B, Sj, Pz, C.c_void_p(out4.data_ptr()),
-                                                        ops._stream()))
+            L.lib().merlot_attention_log_blocks(c_viz.data_ptr(), c_lang.data_ptr(), valid_j.data_ptr(), B, Sj, Pz,
+                                                out4.data_ptr(), ops._stream())
             self._attn_log = out4
         self.encoder_info = {"hidden_state": self._y_j.view(B, Sj, H)}
         if probs_j is not None:  # [layers,B,S,S] -> the reference's [B, layers, S, S] (utils/transformer.py:238), a view

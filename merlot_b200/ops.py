@@ -9,8 +9,8 @@ import torch
 from . import _lib as L
 
 
-def _stream() -> C.c_void_p:
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+def _stream() -> int:
+    return torch.cuda.current_stream().cuda_stream
 
 
 def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
@@ -48,7 +48,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn_major: bool = False, b_mn_maj
     if out is None:
         out = torch.empty((M, N), dtype=out_dtype, device=a.device)
     assert out.stride(1) == 1
-    g = L.GemmDesc()
+    g = L.merlot_gemm_t()
     g.M, g.N, g.K = M, N, K
     g.a, g.lda, g.a_mn_major = a.data_ptr(), a.stride(0), int(a_mn_major)
     g.b, g.ldb, g.b_mn_major = b.data_ptr(), b.stride(0), int(b_mn_major)
@@ -90,15 +90,15 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn_major: bool = False, b_mn_maj
     g.flags = flags
     g.dropout_p, g.dropout_seed, g.dropout_site = dropout_p, dropout_seed, dropout_site
     g.splits, g.block_n = splits, block_n
-    L.check(L.lib().merlot_gemm_bf16(C.byref(g), _stream()))
+    L.lib().merlot_gemm_bf16(C.byref(g), _stream())
     return out
 
 
 def _attn_desc(qkv: torch.Tensor, B: int, S: int, heads: int, valid: Optional[torch.Tensor], pair=(0, 0),
-               dropout=(0.0, 0, 0)) -> L.AttnDesc:
+               dropout=(0.0, 0, 0)) -> L.merlot_attn_t:
     _require_cuda(qkv, valid)
     assert qkv.dtype == torch.bfloat16 and qkv.dim() == 2 and qkv.stride(1) == 1 and qkv.shape[0] == B * S
-    a = L.AttnDesc()
+    a = L.merlot_attn_t()
     a.B, a.S, a.heads, a.head_dim = B, S, heads, qkv.shape[1] // (3 * heads)
     a.qkv, a.ld_qkv = qkv.data_ptr(), qkv.stride(0)
     if valid is not None:
@@ -122,7 +122,7 @@ def attention_fwd(qkv: torch.Tensor, B: int, S: int, heads: int, valid: Optional
     if lse is None:
         lse = torch.empty((B, heads, S), dtype=torch.float32, device=qkv.device)
     a.ctx, a.ld_ctx, a.lse = ctx.data_ptr(), ctx.stride(0), lse.data_ptr()
-    L.check(L.lib().merlot_attention_fwd(C.byref(a), _stream()))
+    L.lib().merlot_attention_fwd(C.byref(a), _stream())
     return ctx, lse
 
 
@@ -158,7 +158,7 @@ def attention_bwd(qkv, ctx, d_ctx, lse, B, S, heads, valid=None, dqkv=None, dq_a
         _require_cuda(d_bias_qkv)
         assert d_bias_qkv.dtype == torch.float32 and d_bias_qkv.numel() == 3 * H and d_bias_qkv.is_contiguous()
         a.d_bias_qkv = d_bias_qkv.data_ptr()
-    L.check(L.lib().merlot_attention_bwd(C.byref(a), _stream()))
+    L.lib().merlot_attention_bwd(C.byref(a), _stream())
     return dqkv
 
 
@@ -169,7 +169,7 @@ def attention_probs(qkv, lse, B, S, heads, valid=None, out=None, pair=(0, 0), dr
     if out is None:
         out = torch.empty((B, S, S), dtype=torch.float32, device=qkv.device)
     a.lse = lse.data_ptr()
-    L.check(L.lib().merlot_attention_probs(C.byref(a), C.c_void_p(out.data_ptr()), _stream()))
+    L.lib().merlot_attention_probs(C.byref(a), out.data_ptr(), _stream())
     return out
 
 
@@ -184,7 +184,7 @@ def attention_colsum(qkv, lse, colsum, B, S, heads, valid=None, pair=(0, 0), dro
         assert colsum2.dtype == torch.float32 and colsum2.numel() == B * S
         a.colsum2, a.colsum_split = colsum2.data_ptr(), int(split)
     a.colsum_valid_q = int(valid_q)
-    L.check(L.lib().merlot_attention_colsum(C.byref(a), _stream()))
+    L.lib().merlot_attention_colsum(C.byref(a), _stream())
     return colsum
 
 
@@ -200,7 +200,7 @@ def _f32(t: torch.Tensor) -> int:
 
 def layernorm_fwd(x, y, gamma, beta, mean=None, rstd=None, rows=None, remap=(0, 0, 0), dropout=(0.0, 0, 0), eps=1e-5):
     _require_cuda(x, y, gamma, beta, mean, rstd)
-    d = L.LnDesc()
+    d = L.merlot_ln_t()
     H = gamma.numel()
     d.x, d.x_f32, d.ld_x = x.data_ptr(), _f32(x), x.stride(-2)
     d.y, d.y_f32, d.ld_y = y.data_ptr(), _f32(y), y.stride(-2)
@@ -210,7 +210,7 @@ def layernorm_fwd(x, y, gamma, beta, mean=None, rstd=None, rows=None, remap=(0, 
     d.H, d.eps = H, eps
     d.map_per, d.map_stride, d.map_off = remap
     d.dropout_p, d.dropout_seed, d.dropout_site = dropout
-    L.check(L.lib().merlot_layernorm_fwd(C.byref(d), _stream()))
+    L.lib().merlot_layernorm_fwd(C.byref(d), _stream())
     return y
 
 
@@ -228,7 +228,7 @@ def _ln_workspace(H: int, device) -> torch.Tensor:
 
 def layernorm_bwd(dy, x, mean, rstd, gamma, dx, dgamma, dbeta, dres=None, rows=None, remap=(0, 0, 0), dropout=(0.0, 0, 0)):
     _require_cuda(dy, x, mean, rstd, gamma, dx, dgamma, dbeta, dres)
-    d = L.LnBwdDesc()
+    d = L.merlot_ln_bwd_t()
     H = gamma.numel()
     d.dy, d.dy_f32, d.ld_dy = dy.data_ptr(), _f32(dy), dy.stride(-2)
     d.x, d.x_f32, d.ld_x = x.data_ptr(), _f32(x), x.stride(-2)
@@ -242,7 +242,7 @@ def layernorm_bwd(dy, x, mean, rstd, gamma, dx, dgamma, dbeta, dres=None, rows=N
     d.H = H
     d.map_per, d.map_stride, d.map_off = remap
     d.dropout_p, d.dropout_seed, d.dropout_site = dropout
-    L.check(L.lib().merlot_layernorm_bwd(C.byref(d), _stream()))
+    L.lib().merlot_layernorm_bwd(C.byref(d), _stream())
     return dx
 
 
@@ -252,18 +252,15 @@ def layernorm_bwd_fused(dy, x, mean, rstd, gamma, dx, dgamma, dbeta, dres=None, 
     _require_cuda(dy, x, mean, rstd, gamma, dx, dgamma, dbeta, dres, dmask, dbias)
     H = gamma.numel()
     p, seed, site = dropout
-    L.check(L.lib().merlot_layernorm_bwd_fused(
-        C.c_void_p(dy.data_ptr()), C.c_void_p(x.data_ptr()), C.c_void_p(mean.data_ptr()), C.c_void_p(rstd.data_ptr()),
-        C.c_void_p(gamma.data_ptr()), C.c_void_p(_ptr(dres)), C.c_void_p(dx.data_ptr()), C.c_void_p(_ptr(dmask)),
-        C.c_void_p(dgamma.data_ptr()), C.c_void_p(dbeta.data_ptr()), C.c_void_p(_ptr(dbias)), C.c_void_p(None),
-        C.c_longlong(x.numel() // H), H, C.c_float(p), C.c_uint64(seed), C.c_uint32(site), _stream()))
+    L.lib().merlot_layernorm_bwd_fused(dy.data_ptr(), x.data_ptr(), mean.data_ptr(), rstd.data_ptr(), gamma.data_ptr(),
+                                       _ptr(dres), dx.data_ptr(), _ptr(dmask), dgamma.data_ptr(), dbeta.data_ptr(), _ptr(dbias),
+                                       None, x.numel() // H, H, p, seed, site, _stream())
     return dx
 
 
 def dropout_apply(x, y, p, seed, site):
     rows, N = x.numel() // x.shape[-1], x.shape[-1]
-    L.check(L.lib().merlot_dropout_apply(C.c_void_p(x.data_ptr()), x.stride(-2), C.c_void_p(y.data_ptr()), y.stride(-2),
-                                         C.c_longlong(rows), N, C.c_float(p), C.c_uint64(seed), C.c_uint32(site), _stream()))
+    L.lib().merlot_dropout_apply(x.data_ptr(), x.stride(-2), y.data_ptr(), y.stride(-2), rows, N, p, seed, site, _stream())
     return y
 
 
@@ -272,16 +269,15 @@ def bias_grad(dy, out, rows=None, N=None, dropout=(0.0, 0, 0)):
     N = out.numel() if N is None else N
     rows = dy.numel() // dy.stride(-2) if rows is None else rows
     p, seed, site = dropout
-    L.check(L.lib().merlot_bias_grad(C.c_void_p(dy.data_ptr()), _f32(dy), dy.stride(-2), C.c_longlong(rows), N,
-                                     C.c_void_p(out.data_ptr()), C.c_float(p), C.c_uint64(seed), C.c_uint32(site), _stream()))
+    L.lib().merlot_bias_grad(dy.data_ptr(), _f32(dy), dy.stride(-2), rows, N, out.data_ptr(), p, seed, site, _stream())
 
 
 def gather_rows(src, idx, dst, n=None, H=None):
     H = src.shape[-1] if H is None else H
     n = idx.numel() if n is None else n
     assert idx.dtype == torch.int32
-    L.check(L.lib().merlot_gather_rows(C.c_void_p(src.data_ptr()), _f32(src), src.stride(-2), C.c_void_p(idx.data_ptr()),
-                                       C.c_void_p(dst.data_ptr()), _f32(dst), dst.stride(-2), n, H, _stream()))
+    L.lib().merlot_gather_rows(src.data_ptr(), _f32(src), src.stride(-2), idx.data_ptr(), dst.data_ptr(), _f32(dst),
+                               dst.stride(-2), n, H, _stream())
     return dst
 
 
@@ -289,105 +285,95 @@ def scatter_add_rows(src, idx, dst, n=None, H=None, scale=1.0):
     H = dst.shape[-1] if H is None else H
     n = idx.numel() if n is None else n
     assert idx.dtype == torch.int32
-    L.check(L.lib().merlot_scatter_add_rows(C.c_void_p(src.data_ptr()), _f32(src), src.stride(-2), C.c_void_p(idx.data_ptr()),
-                                            C.c_void_p(dst.data_ptr()), _f32(dst), dst.stride(-2), n, H, C.c_float(scale),
-                                            _stream()))
+    L.lib().merlot_scatter_add_rows(src.data_ptr(), _f32(src), src.stride(-2), idx.data_ptr(), dst.data_ptr(), _f32(dst),
+                                    dst.stride(-2), n, H, scale, _stream())
     return dst
 
 
 def gelu_f32(x, y):
-    L.check(L.lib().merlot_gelu_f32(C.c_void_p(x.data_ptr()), C.c_void_p(y.data_ptr()), C.c_longlong(x.numel()), _stream()))
+    L.lib().merlot_gelu_f32(x.data_ptr(), y.data_ptr(), x.numel(), _stream())
     return y
 
 
 def gelu_bwd_f32(dy, pre, dx):
-    L.check(L.lib().merlot_gelu_bwd_f32(C.c_void_p(dy.data_ptr()), C.c_void_p(pre.data_ptr()), C.c_void_p(dx.data_ptr()),
-                                        C.c_longlong(dy.numel()), _stream()))
+    L.lib().merlot_gelu_bwd_f32(dy.data_ptr(), pre.data_ptr(), dx.data_ptr(), dy.numel(), _stream())
     return dx
 
 
 def cast_f32_to_bf16(x, y):
     assert x.dtype == torch.float32 and y.dtype == torch.bfloat16 and x.numel() == y.numel()
-    L.check(L.lib().merlot_cast_f32_to_bf16(C.c_void_p(x.data_ptr()), C.c_void_p(y.data_ptr()), C.c_longlong(x.numel()), _stream()))
+    L.lib().merlot_cast_f32_to_bf16(x.data_ptr(), y.data_ptr(), x.numel(), _stream())
     return y
 
 
 def cast_bf16_to_f32(x, y):
     assert x.dtype == torch.bfloat16 and y.dtype == torch.float32 and x.numel() == y.numel() and x.is_contiguous()
-    L.check(L.lib().merlot_cast_bf16_to_f32(C.c_void_p(x.data_ptr()), C.c_void_p(y.data_ptr()), C.c_longlong(x.numel()), _stream()))
+    L.lib().merlot_cast_bf16_to_f32(x.data_ptr(), y.data_ptr(), x.numel(), _stream())
     return y
 
 
 def l2norm_fwd(x, y, inv):
-    L.check(L.lib().merlot_l2norm_fwd(C.c_void_p(x.data_ptr()), C.c_void_p(y.data_ptr()), C.c_void_p(inv.data_ptr()),
-                                      x.shape[0], x.shape[1], _stream()))
+    L.lib().merlot_l2norm_fwd(x.data_ptr(), y.data_ptr(), inv.data_ptr(), x.shape[0], x.shape[1], _stream())
 
 
 def l2norm_bwd(dy, y, inv, dx):
-    L.check(L.lib().merlot_l2norm_bwd(C.c_void_p(dy.data_ptr()), C.c_void_p(y.data_ptr()), C.c_void_p(inv.data_ptr()),
-                                      C.c_void_p(dx.data_ptr()), y.shape[0], y.shape[1], _stream()))
+    L.lib().merlot_l2norm_bwd(dy.data_ptr(), y.data_ptr(), inv.data_ptr(), dx.data_ptr(), y.shape[0], y.shape[1], _stream())
 
 
 def softmax_ce_fwd(logits, labels, Cn, loss, lse, correct=None):
-    L.check(L.lib().merlot_softmax_ce_fwd(C.c_void_p(logits.data_ptr()), logits.stride(0), C.c_void_p(labels.data_ptr()),
-                                          logits.shape[0], Cn, C.c_void_p(loss.data_ptr()), C.c_void_p(lse.data_ptr()),
-                                          C.c_void_p(_ptr(correct)), _stream()))
+    L.lib().merlot_softmax_ce_fwd(logits.data_ptr(), logits.stride(0), labels.data_ptr(), logits.shape[0], Cn, loss.data_ptr(),
+                                  lse.data_ptr(), _ptr(correct), _stream())
 
 
 def softmax_ce_bwd(logits, labels, Cn, lse, coeff, dlogits):
-    L.check(L.lib().merlot_softmax_ce_bwd(C.c_void_p(logits.data_ptr()), logits.stride(0), C.c_void_p(labels.data_ptr()),
-                                          logits.shape[0], Cn, C.c_void_p(lse.data_ptr()), C.c_void_p(coeff.data_ptr()),
-                                          C.c_void_p(dlogits.data_ptr()), _f32(dlogits), dlogits.stride(0), _stream()))
+    L.lib().merlot_softmax_ce_bwd(logits.data_ptr(), logits.stride(0), labels.data_ptr(), logits.shape[0], Cn, lse.data_ptr(),
+                                  coeff.data_ptr(), dlogits.data_ptr(), _f32(dlogits), dlogits.stride(0), _stream())
 
 
 def patch_im2col(image, a, P):
     N, H0, W0, _ = image.shape
     assert image.dtype == torch.bfloat16 and image.is_contiguous()
-    L.check(L.lib().merlot_patch_im2col(C.c_void_p(image.data_ptr()), C.c_void_p(a.data_ptr()), N, H0, W0, P, _stream()))
+    L.lib().merlot_patch_im2col(image.data_ptr(), a.data_ptr(), N, H0, W0, P, _stream())
 
 
 def ws_weights(w2d: torch.Tensor, rows_pad: int) -> torch.Tensor:
     """K13: weight-standardised bf16 GEMM operand [rows_pad, cout] of a conv kernel stored as fp32 [kh*kw*cin, cout]."""
     rows, cout = w2d.shape
     out = torch.empty((rows_pad, cout), dtype=torch.bfloat16, device=w2d.device)
-    L.check(L.lib().merlot_ws_weights(C.c_void_p(w2d.data_ptr()), rows, rows_pad, cout, C.c_void_p(out.data_ptr()), _stream()))
+    L.lib().merlot_ws_weights(w2d.data_ptr(), rows, rows_pad, cout, out.data_ptr(), _stream())
     return out
 
 
 def im2col3x3(x: torch.Tensor, N, h, w, Cin, stride, out: torch.Tensor, sub_half=False):
-    L.check(L.lib().merlot_im2col3x3(C.c_void_p(x.data_ptr()), N, h, w, Cin, stride, int(sub_half), C.c_void_p(out.data_ptr()),
-                                     out.stride(0), _stream()))
+    L.lib().merlot_im2col3x3(x.data_ptr(), N, h, w, Cin, stride, int(sub_half), out.data_ptr(), out.stride(0), _stream())
 
 
 def group_norm_fwd(x, gamma, beta, y, stats, N, HW, Cc, groups=32, eps=1e-4, relu=True, shortcut=None):
-    L.check(L.lib().merlot_group_norm_fwd(C.c_void_p(x.data_ptr()), C.c_void_p(gamma.data_ptr()), C.c_void_p(beta.data_ptr()),
-                                          C.c_void_p(_ptr(shortcut)), C.c_void_p(y.data_ptr()), C.c_void_p(stats.data_ptr()), N, HW, Cc,
-                                          groups, C.c_float(eps), int(relu), _stream()))
+    L.lib().merlot_group_norm_fwd(x.data_ptr(), gamma.data_ptr(), beta.data_ptr(), _ptr(shortcut), y.data_ptr(), stats.data_ptr(),
+                                  N, HW, Cc, groups, eps, int(relu), _stream())
 
 
 def avgpool2_same(x, N, h, w, Cc, y):
-    L.check(L.lib().merlot_avgpool2_same(C.c_void_p(x.data_ptr()), N, h, w, Cc, C.c_void_p(y.data_ptr()), _stream()))
+    L.lib().merlot_avgpool2_same(x.data_ptr(), N, h, w, Cc, y.data_ptr(), _stream())
 
 
 def group_norm_bwd(dy, x, y, stats, gamma, dx, dshortcut, dgamma, dbeta, red, N, HW, Cc, groups=32, eps=1e-4, relu=True):
-    L.check(L.lib().merlot_group_norm_bwd(C.c_void_p(dy.data_ptr()), C.c_void_p(x.data_ptr()), C.c_void_p(_ptr(y)),
-                                          C.c_void_p(stats.data_ptr()), C.c_void_p(gamma.data_ptr()), C.c_void_p(dx.data_ptr()),
-                                          C.c_void_p(_ptr(dshortcut)), C.c_void_p(dgamma.data_ptr()), C.c_void_p(dbeta.data_ptr()),
-                                          C.c_void_p(red.data_ptr()), N, HW, Cc, groups, C.c_float(eps), int(relu), _stream()))
+    L.lib().merlot_group_norm_bwd(dy.data_ptr(), x.data_ptr(), _ptr(y), stats.data_ptr(), gamma.data_ptr(), dx.data_ptr(),
+                                  _ptr(dshortcut), dgamma.data_ptr(), dbeta.data_ptr(), red.data_ptr(), N, HW, Cc, groups, eps,
+                                  int(relu), _stream())
 
 
 def avgpool2_same_bwd(dy, N, h, w, Cc, dx):
-    L.check(L.lib().merlot_avgpool2_same_bwd(C.c_void_p(dy.data_ptr()), N, h, w, Cc, C.c_void_p(dx.data_ptr()), _stream()))
+    L.lib().merlot_avgpool2_same_bwd(dy.data_ptr(), N, h, w, Cc, dx.data_ptr(), _stream())
 
 
 def col2im3x3(dcol, N, h, w, Cin, stride, dx):
-    L.check(L.lib().merlot_col2im3x3(C.c_void_p(dcol.data_ptr()), N, h, w, Cin, stride, dcol.stride(0), C.c_void_p(dx.data_ptr()), _stream()))
+    L.lib().merlot_col2im3x3(dcol.data_ptr(), N, h, w, Cin, stride, dcol.stride(0), dx.data_ptr(), _stream())
 
 
 def ws_weights_bwd(dws, w2d, dw2d):
     rows, cout = w2d.shape
-    L.check(L.lib().merlot_ws_weights_bwd(C.c_void_p(dws.data_ptr()), dws.stride(0), C.c_void_p(w2d.data_ptr()), rows, cout,
-                                          C.c_void_p(dw2d.data_ptr()), _stream()))
+    L.lib().merlot_ws_weights_bwd(dws.data_ptr(), dws.stride(0), w2d.data_ptr(), rows, cout, dw2d.data_ptr(), _stream())
 
 
 class WsPlan:
@@ -408,7 +394,7 @@ class WsPlan:
         self.wstd_arena = torch.empty(total, dtype=torch.bfloat16, device=device)
         self.wstd = {n: self.wstd_arena[o:o + kp * c].view(kp, c) for n, (o, kp, c) in offs.items()}
         self.dws = {n: self.dws_arena[o:o + kp * c].view(kp, c) for n, (o, kp, c) in offs.items()}
-        items = (L.WsItem * len(self.names))()
+        items = (L.merlot_ws_item_t * len(self.names))()
         b0 = 0
         for i, n in enumerate(self.names):
             rows, cout = kernels[n].shape
@@ -422,90 +408,81 @@ class WsPlan:
         self.key = tuple(kernels[n].data_ptr() for n in self.names)
 
     def standardise(self):
-        L.check(L.lib().merlot_ws_weights_multi(C.c_void_p(self.items_dev.data_ptr()), len(self.names), self.n_blocks, _stream()))
+        L.lib().merlot_ws_weights_multi(self.items_dev.data_ptr(), len(self.names), self.n_blocks, _stream())
 
     def zero_grads(self):
         self.dws_arena.zero_()
 
     def backward(self):
-        L.check(L.lib().merlot_ws_weights_bwd_multi(C.c_void_p(self.items_dev.data_ptr()), len(self.names), self.n_blocks, _stream()))
+        L.lib().merlot_ws_weights_bwd_multi(self.items_dev.data_ptr(), len(self.names), self.n_blocks, _stream())
 
 
 def add_bf16(a, b, out):
-    L.check(L.lib().merlot_add_bf16(C.c_void_p(a.data_ptr()), C.c_void_p(b.data_ptr()), C.c_void_p(out.data_ptr()),
-                                    C.c_longlong(a.numel()), _stream()))
+    L.lib().merlot_add_bf16(a.data_ptr(), b.data_ptr(), out.data_ptr(), a.numel(), _stream())
 
 
 def vit_assemble_fwd(patch, pos_table, cls_emb, xsum, N, h1, w1, ncls, H):
-    L.check(L.lib().merlot_vit_assemble_fwd(C.c_void_p(patch.data_ptr()), C.c_void_p(pos_table.data_ptr()),
-                                            C.c_void_p(cls_emb.data_ptr()), C.c_void_p(xsum.data_ptr()), N, h1, w1, ncls, 64, H,
-                                            _stream()))
+    L.lib().merlot_vit_assemble_fwd(patch.data_ptr(), pos_table.data_ptr(), cls_emb.data_ptr(), xsum.data_ptr(), N, h1, w1, ncls,
+                                    64, H, _stream())
 
 
 def vit_assemble_bwd(dxsum, dpatch, N, np_, ncls, H):
-    L.check(L.lib().merlot_vit_assemble_bwd(C.c_void_p(dxsum.data_ptr()), C.c_void_p(dpatch.data_ptr()), N, np_, ncls, H, _stream()))
+    L.lib().merlot_vit_assemble_bwd(dxsum.data_ptr(), dpatch.data_ptr(), N, np_, ncls, H, _stream())
 
 
 def viz_assemble_fwd(hv, img_idx_pe, img_idx, fpos, fcls, xsum, img_trg, N, h1, w1, ncls, sp, H):
-    L.check(L.lib().merlot_viz_assemble_fwd(C.c_void_p(hv.data_ptr()), C.c_void_p(img_idx_pe.data_ptr()),
-                                            C.c_void_p(img_idx.data_ptr()), C.c_void_p(fpos.data_ptr()), C.c_void_p(fcls.data_ptr()),
-                                            C.c_void_p(xsum.data_ptr()), C.c_void_p(img_trg.data_ptr()), N, h1, w1, ncls, sp, 64, H,
-                                            _stream()))
+    L.lib().merlot_viz_assemble_fwd(hv.data_ptr(), img_idx_pe.data_ptr(), img_idx.data_ptr(), fpos.data_ptr(), fcls.data_ptr(),
+                                    xsum.data_ptr(), img_trg.data_ptr(), N, h1, w1, ncls, sp, 64, H, _stream())
 
 
 def viz_assemble_bwd(dxsum, d_img_trg, dhv, N, h1, w1, ncls, sp, H):
-    L.check(L.lib().merlot_viz_assemble_bwd(C.c_void_p(dxsum.data_ptr()), C.c_void_p(_ptr(d_img_trg)), C.c_void_p(dhv.data_ptr()),
-                                            N, h1, w1, ncls, sp, H, _stream()))
+    L.lib().merlot_viz_assemble_bwd(dxsum.data_ptr(), _ptr(d_img_trg), dhv.data_ptr(), N, h1, w1, ncls, sp, H, _stream())
 
 
 def embed_fwd(ids, emb, pos, xsum, Lseq):
-    L.check(L.lib().merlot_embed_fwd(C.c_void_p(ids.data_ptr()), C.c_void_p(emb.data_ptr()), C.c_void_p(pos.data_ptr()),
-                                     C.c_void_p(xsum.data_ptr()), C.c_longlong(ids.numel()), Lseq, emb.shape[1], _stream()))
+    L.lib().merlot_embed_fwd(ids.data_ptr(), emb.data_ptr(), pos.data_ptr(), xsum.data_ptr(), ids.numel(), Lseq, emb.shape[1],
+                             _stream())
 
 
 def group_rowsum(src, groups, per, t0, nt, idxmap, dst, H):
-    L.check(L.lib().merlot_group_rowsum(C.c_void_p(src.data_ptr()), src.stride(-2), groups, per, t0, nt, C.c_void_p(_ptr(idxmap)),
-                                        C.c_void_p(dst.data_ptr()), dst.stride(-2), H, _stream()))
+    L.lib().merlot_group_rowsum(src.data_ptr(), src.stride(-2), groups, per, t0, nt, _ptr(idxmap), dst.data_ptr(), dst.stride(-2),
+                                H, _stream())
 
 
 def segment_rowsum_scatter(src, n_seg, per, idx, dst, H):
-    L.check(L.lib().merlot_segment_rowsum_scatter(C.c_void_p(src.data_ptr()), src.stride(-2), n_seg, per, C.c_void_p(idx.data_ptr()),
-                                                  C.c_void_p(dst.data_ptr()), dst.stride(-2), H, _stream()))
+    L.lib().merlot_segment_rowsum_scatter(src.data_ptr(), src.stride(-2), n_seg, per, idx.data_ptr(), dst.data_ptr(),
+                                          dst.stride(-2), H, _stream())
 
 
 def ids_valid(ids, valid):
-    L.check(L.lib().merlot_ids_valid(C.c_void_p(ids.data_ptr()), C.c_void_p(valid.data_ptr()), C.c_longlong(ids.numel()), _stream()))
+    L.lib().merlot_ids_valid(ids.data_ptr(), valid.data_ptr(), ids.numel(), _stream())
 
 
 def joint_valid(ids, valid, B, P, Lseq):
-    L.check(L.lib().merlot_joint_valid(C.c_void_p(ids.data_ptr()), C.c_void_p(valid.data_ptr()), B, P, Lseq, _stream()))
+    L.lib().merlot_joint_valid(ids.data_ptr(), valid.data_ptr(), B, P, Lseq, _stream())
 
 
 def mlm_index(ids, masked_idx, rows, targets, B, Lseq, k, P):
-    L.check(L.lib().merlot_mlm_index(C.c_void_p(ids.data_ptr()), C.c_void_p(masked_idx.data_ptr()), C.c_void_p(rows.data_ptr()),
-                                     C.c_void_p(targets.data_ptr()), B, Lseq, k, P, _stream()))
+    L.lib().merlot_mlm_index(ids.data_ptr(), masked_idx.data_ptr(), rows.data_ptr(), targets.data_ptr(), B, Lseq, k, P, _stream())
 
 
 def temporal_labels(video_src_ids, shuffled_idx, labels, weights, B, n):
-    L.check(L.lib().merlot_temporal_labels(C.c_void_p(video_src_ids.data_ptr()), C.c_void_p(shuffled_idx.data_ptr()),
-                                           C.c_void_p(labels.data_ptr()), C.c_void_p(weights.data_ptr()), B, n, _stream()))
+    L.lib().merlot_temporal_labels(video_src_ids.data_ptr(), shuffled_idx.data_ptr(), labels.data_ptr(), weights.data_ptr(), B, n,
+                                   _stream())
 
 
 def weighted_loss(per_row, correct, weights, nz_labels, denom_mode, scale, out2, coeff):
-    L.check(L.lib().merlot_weighted_loss(C.c_void_p(per_row.data_ptr()), C.c_void_p(_ptr(correct)), C.c_void_p(_ptr(weights)),
-                                         C.c_void_p(_ptr(nz_labels)), per_row.numel(), denom_mode, C.c_float(scale),
-                                         C.c_void_p(out2.data_ptr()), C.c_void_p(_ptr(coeff)), _stream()))
+    L.lib().merlot_weighted_loss(per_row.data_ptr(), _ptr(correct), _ptr(weights), _ptr(nz_labels), per_row.numel(), denom_mode,
+                                 scale, out2.data_ptr(), _ptr(coeff), _stream())
 
 
 def small_gemm(A, sam, sak, B, sbn, sbk, Cm, M, N, K, alpha=1.0, beta=0.0):
-    L.check(L.lib().merlot_small_gemm_f32(C.c_void_p(A.data_ptr()), C.c_longlong(sam), C.c_longlong(sak), C.c_void_p(B.data_ptr()),
-                                          C.c_longlong(sbn), C.c_longlong(sbk), C.c_void_p(Cm.data_ptr()), Cm.stride(0), M, N, K,
-                                          C.c_float(alpha), C.c_float(beta), _stream()))
+    L.lib().merlot_small_gemm_f32(A.data_ptr(), sam, sak, B.data_ptr(), sbn, sbk, Cm.data_ptr(), Cm.stride(0), M, N, K, alpha,
+                                  beta, _stream())
 
 
 def axpby(x, y, a=1.0, b=1.0):
-    L.check(L.lib().merlot_axpby_f32(C.c_void_p(x.data_ptr()), C.c_void_p(y.data_ptr()), C.c_longlong(x.numel()), C.c_float(a),
-                                     C.c_float(b), _stream()))
+    L.lib().merlot_axpby_f32(x.data_ptr(), y.data_ptr(), x.numel(), a, b, _stream())
 
 
 def mask_draws(B, Lseq, num_to_mask, vocab_size, span_probs, seed, device, out=None):
@@ -516,15 +493,14 @@ def mask_draws(B, Lseq, num_to_mask, vocab_size, span_probs, seed, device, out=N
                "span_upper": torch.empty((B, max(num_to_mask, 1)), dtype=torch.int32, device=device),
                "option": torch.empty((B * Lseq,), dtype=torch.int32, device=device),
                "rand_ids": torch.empty((B * Lseq,), dtype=torch.int32, device=device)}
-    L.check(L.lib().merlot_mask_draws(C.c_void_p(out["gumbel"].data_ptr()), C.c_void_p(out["span_lower"].data_ptr()),
-                                      C.c_void_p(out["span_upper"].data_ptr()), C.c_void_p(out["option"].data_ptr()),
-                                      C.c_void_p(out["rand_ids"].data_ptr()), C.c_longlong(B * Lseq), C.c_longlong(B * num_to_mask),
-                                      int(vocab_size), C.c_float(span_probs[0]), C.c_float(span_probs[1]), C.c_uint64(seed), _stream()))
+    L.lib().merlot_mask_draws(out["gumbel"].data_ptr(), out["span_lower"].data_ptr(), out["span_upper"].data_ptr(),
+                              out["option"].data_ptr(), out["rand_ids"].data_ptr(), B * Lseq, B * num_to_mask, int(vocab_size),
+                              span_probs[0], span_probs[1], seed, _stream())
     return out
 
 
 def mask_inputs(ids, attn_summ, draws, masked_ids, masked_idx, valid_out, num_topk, num_to_mask, do_spanbert, mask_token, consts):
-    m = L.MaskDesc()
+    m = L.merlot_mask_t()
     B, Lseq = ids.shape
     m.ids, m.attn_summ, m.gumbel = ids.data_ptr(), _ptr(attn_summ), draws["gumbel"].data_ptr()
     m.span_lower, m.span_upper = _ptr(draws.get("span_lower")), _ptr(draws.get("span_upper"))
@@ -532,17 +508,16 @@ def mask_inputs(ids, attn_summ, draws, masked_ids, masked_idx, valid_out, num_to
     m.masked_ids, m.masked_idx, m.valid_out = masked_ids.data_ptr(), masked_idx.data_ptr(), _ptr(valid_out)
     m.B, m.L, m.num_topk, m.num_to_mask, m.do_spanbert, m.mask_token = B, Lseq, num_topk, num_to_mask, int(do_spanbert), mask_token
     m.w_delta, m.w_non, m.logw_top, m.logw_non, m.w_max = consts
-    L.check(L.lib().merlot_mask_inputs(C.byref(m), _stream()))
+    L.lib().merlot_mask_inputs(C.byref(m), _stream())
 
 
 def adamw_step(p, g, m, v, p_bf16, n, beta1, omb1, beta2, omb2, eps, lr_t, wd, grad_scale, zero_grad):
-    d = L.AdamDesc()
+    d = L.merlot_adamw_t()
     d.p, d.g, d.m, d.v, d.p_bf16, d.n = p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), _ptr(p_bf16), n
     d.beta1, d.one_minus_beta1, d.beta2, d.one_minus_beta2 = beta1, omb1, beta2, omb2
     d.epsilon, d.lr_t, d.weight_decay, d.grad_scale, d.zero_grad = eps, lr_t, wd, grad_scale, int(zero_grad)
-    L.check(L.lib().merlot_adamw_step(C.byref(d), _stream()))
+    L.lib().merlot_adamw_step(C.byref(d), _stream())
 
 
 def clip_by_global_norm(g, clip_norm, scratch_f64, norm_out):
-    L.check(L.lib().merlot_clip_by_global_norm(C.c_void_p(g.data_ptr()), C.c_longlong(g.numel()), C.c_float(clip_norm),
-                                               C.c_void_p(scratch_f64.data_ptr()), C.c_void_p(_ptr(norm_out)), _stream()))
+    L.lib().merlot_clip_by_global_norm(g.data_ptr(), g.numel(), clip_norm, scratch_f64.data_ptr(), _ptr(norm_out), _stream())

@@ -11,11 +11,22 @@ from merlot_b200.params import ParamStore
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
+HEADER = os.path.join(ROOT, "include", "merlot_b200.h")
 
 
-def test_library_exports_every_header_symbol():
+def _header_c_view():
+    import re
+    return re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
+
+
+def _header_functions():
+    import re
+    return sorted(set(re.findall(r"\b(merlot_[a-z0-9_]+)\s*\(", _header_c_view())))
+
+
+def test_binding_covers_every_header_symbol():
     lib = _lib.lib()
-    names = _lib.exported_symbols_from_header()
+    names = _header_functions()
     assert len(names) >= 40
     for n in names:
         assert hasattr(lib, n), n
@@ -33,27 +44,80 @@ def test_attention_bwd_dq_mode_boundary():
             assert lib.merlot_attention_bwd_workspace_bytes(B, S, heads) == max(parts, 1) * B * S * heads * 64 * 4, (S, B, heads)
 
 
-def test_ctypes_structs_match_the_header_layout(tmp_path):
-    """The descriptor structs of include/merlot_b200.h compiled by gcc (sizeof and the offset of the last member) against their
-    ctypes mirrors in merlot_b200/_lib.py: a field added on one side only would shift every later argument silently."""
+def test_generated_structs_and_constants_match_the_header(tmp_path):
+    """Every descriptor struct of include/merlot_b200.h compiled by gcc (sizeof, and offsetof / sizeof of every member) against
+    the classes merlot_b200/_lib.py generates from it: a misread type or a reordered member would shift the arguments the
+    library reads silently.  The same program prints every MERLOT_* constant, checked against its Python name."""
     import ctypes
+    import re
     import subprocess
-    pairs = [("merlot_gemm_t", _lib.GemmDesc), ("merlot_attn_t", _lib.AttnDesc), ("merlot_ln_t", _lib.LnDesc),
-             ("merlot_ln_bwd_t", _lib.LnBwdDesc), ("merlot_layer_params_t", _lib.LayerParams), ("merlot_stack_t", _lib.StackDesc),
-             ("merlot_mask_t", _lib.MaskDesc), ("merlot_adamw_t", _lib.AdamDesc), ("merlot_ws_item_t", _lib.WsItem)]
-    src = tmp_path / "sizes.c"
+    names = re.findall(r"typedef\s+struct\s*(?:\w+\s*)?\{[^{}]*\}\s*(\w+)\s*;", _header_c_view())
+    assert len(names) >= 9, names
+    macros = re.findall(r"^#define[ \t]+(MERLOT_\w+)[ \t]+\S", _header_c_view(), flags=re.M)  # those with a value
+    assert len(macros) >= 12, macros
+    src = tmp_path / "layout.c"
     lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "merlot_b200.h"', 'int main(void) {']
-    for cname, cls in pairs:
-        last = cls._fields_[-1][0]
-        lines.append(f'  printf("{cname} %zu %zu\\n", sizeof({cname}), offsetof({cname}, {last}));')
+    for cname in names:
+        lines.append(f'  printf("{cname} %zu\\n", sizeof({cname}));')
+        for f, _ in getattr(_lib, cname)._fields_:
+            lines.append(f'  printf("{cname}.{f} %zu %zu\\n", offsetof({cname}, {f}), sizeof((({cname}*)0)->{f}));')
+    for m in macros:
+        lines.append(f'  printf("{m} %lld\\n", (long long)({m}));')
     lines += ['  return 0;', '}']
     src.write_text("\n".join(lines))
-    exe = tmp_path / "sizes"
+    exe = tmp_path / "layout"
     subprocess.run(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
-    out = dict((ln.split()[0], tuple(int(v) for v in ln.split()[1:])) for ln in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.splitlines())
-    for cname, cls in pairs:
-        last = cls._fields_[-1][0]
-        assert out[cname] == (ctypes.sizeof(cls), getattr(cls, last).offset), (cname, out[cname], ctypes.sizeof(cls), getattr(cls, last).offset)
+    run = subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.splitlines()
+    out = dict((ln.split()[0], tuple(int(v) for v in ln.split()[1:])) for ln in run)
+    for cname in names:
+        cls = getattr(_lib, cname)
+        assert out[cname] == (ctypes.sizeof(cls),), (cname, out[cname], ctypes.sizeof(cls))
+        for f, t in cls._fields_:
+            got = (getattr(cls, f).offset, ctypes.sizeof(t))
+            assert out[f"{cname}.{f}"] == got, (cname, f, out[f"{cname}.{f}"], got)
+    for m in macros:  # MERLOT_GEMM_X is exported as GEMM_X, the status codes under their own names
+        py = m[len("MERLOT_"):] if m.startswith("MERLOT_GEMM_") else m
+        assert getattr(_lib, py) == out[m][0], (m, py, out[m][0])
+
+
+def test_ctypes_prototypes_match_the_header():
+    """Every merlot_* function of the header is bound with argtypes, restype and errcheck; a table of prototypes that mix
+    long long, uint64_t, float, size_t, const char* and void pins the one type mapping."""
+    import ctypes as C
+    lib = _lib.lib()
+    for n in _header_functions():
+        f = getattr(lib, n)
+        assert f.argtypes is not None and f.errcheck is not None, n
+        assert f.restype in (None, C.c_int, C.c_longlong, C.c_size_t, C.c_char_p), (n, f.restype)
+    P, LL = C.c_void_p, C.c_longlong
+    expected = {
+        "merlot_mask_draws": ([P] * 5 + [LL, LL, C.c_int, C.c_float, C.c_float, C.c_uint64, P], C.c_int),
+        "merlot_attention_bwd_workspace_bytes": ([C.c_int] * 3, C.c_size_t),
+        "merlot_last_error": ([], C.c_char_p),
+        "merlot_reset_launch_count": ([], None),
+        "merlot_small_gemm_f32": ([P, LL, LL, P, LL, LL, P] + [C.c_int] * 4 + [C.c_float, C.c_float, P], C.c_int),
+    }
+    for n, (argtypes, restype) in expected.items():
+        f = getattr(lib, n)
+        assert list(f.argtypes) == argtypes and f.restype is restype, (n, f.argtypes, f.restype)
+
+
+def test_bound_calls_check_arguments_and_status_without_a_gpu():
+    """These calls fail their host-side validation before any CUDA call, so they run on a CPU-only machine."""
+    import ctypes as C
+    lib = _lib.lib()
+    with pytest.raises(_lib.MerlotError) as e:
+        lib.merlot_gemm_bf16(None, None)
+    assert e.value.code == _lib.MERLOT_EINVAL
+    with pytest.raises(_lib.MerlotShapeError):  # N = 12 is not a multiple of 8
+        lib.merlot_dropout_apply(256, 12, 512, 12, 1, 12, 0.1, 0, 0, None)
+    with pytest.raises(C.ArgumentError):
+        lib.merlot_attention_bwd_dq_parts(600.0)
+    with pytest.raises(TypeError):
+        lib.merlot_attention_bwd_dq_parts()
+    with pytest.raises(TypeError):
+        lib.merlot_attention_bwd_dq_parts(600, 1)
+    assert lib.merlot_attention_bwd_dq_parts(600) == 0  # a non-negative int result is a value, not a status
 
 
 def test_bench_reference_arm_prints_the_contract_line():

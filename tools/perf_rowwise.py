@@ -43,7 +43,6 @@ mean, rstd = torch.randn(M).to(dev), (torch.rand(M) + 0.5).to(dev)
 gamma, beta = torch.randn(H).to(dev), torch.randn(H).to(dev)
 dgam, dbet, dbias = torch.zeros(H, device=dev), torch.zeros(H, device=dev), torch.zeros(H, device=dev)
 st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-L.merlot_layernorm_bwd_fused.argtypes = [C.c_void_p] * 11 + [C.c_void_p, C.c_longlong, C.c_int, C.c_float, C.c_uint64, C.c_uint32, C.c_void_p]
 
 
 def lnb(rows, drop, bias, res=True):
