@@ -382,6 +382,32 @@ int merlot_ws_weights_multi(const merlot_ws_item_t* items_dev, int n_items, int 
 int merlot_ws_weights_bwd_multi(const merlot_ws_item_t* items_dev, int n_items, int n_blocks, void* stream);
 int merlot_add_bf16(const void* a, const void* b, void* out, long long n, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * K14: frame preparation of the pretraining input pipeline (model/dataloader.py:72-96): uint8 HWC RGB frames ->
+ * convert_image_dtype -> resize_and_pad(do_random_scale=True, resize_method='random') (utils/model_utils.py:855-940; TF 1.15
+ * legacy resize kernels, align_corners=True) -> where(isfinite) -> brightness or contrast augment + clip
+ * (utils/model_utils.py:758-835) -> bf16 (RNE), all in float32 in the reference's operation order; see csrc/frames.cu.
+ * The caller draws and plans every frame (sizes, offsets, method, transform, factors); one descriptor per frame, in a device
+ * table.  src_u8: the frames packed back to back; out_bf16: [n, out_h, out_w, 3]; mean_ws: f32 scratch [n, 3].
+ * Every descriptor must satisfy src_h, src_w, scaled_h, scaled_w >= 1, offset_y, offset_x >= 0, method in [0, 3],
+ * augment in [0, 2] and src_offset + 3*src_h*src_w within src_u8 (the kernel reads them unchecked).
+ * ------------------------------------------------------------------------------------------------------------ */
+#define MERLOT_FRAME_NO_AUGMENT 0
+#define MERLOT_FRAME_BRIGHTNESS 1 /* x * factor[c] */
+#define MERLOT_FRAME_CONTRAST 2   /* (x - mean_c) * factor[c] + mean_c, mean over the padded image before augmenting */
+typedef struct merlot_frame {
+  long long src_offset;             /* byte offset of the frame's [src_h, src_w, 3] pixels in src_u8 */
+  int src_h, src_w;                 /* decoded size */
+  int scaled_h, scaled_w;           /* resize target (sh, sw) */
+  int offset_y, offset_x;           /* crop origin in the resized image; rows/columns past it and past (sh, sw) are zero */
+  int method;                       /* tf.image.ResizeMethod (TF1): 0 bilinear, 1 nearest, 2 bicubic, 3 area */
+  int augment;                      /* MERLOT_FRAME_* */
+  float factor_r, factor_g, factor_b;
+  int reserved;
+} merlot_frame_t;
+int merlot_frames_prepare(const merlot_frame_t* frames_dev, int n, const void* src_u8, int out_h, int out_w, float* mean_ws,
+                          void* out_bf16, void* stream);
+
 /* bench.py roofline support: time every K1 launch with CUDA events on its own stream between begin/end.
  * end() synchronises the device and returns the summed duration (ms), algorithmic FLOPs (2*M*N*K) and launch count. */
 void merlot_gemm_profile_begin(void);

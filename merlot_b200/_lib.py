@@ -33,6 +33,10 @@ GEMM_DROPOUT = 16
 GEMM_GELU_GRAD_OUT = 32
 GEMM_MUL_AUX = 64
 
+MERLOT_FRAME_NO_AUGMENT = 0
+MERLOT_FRAME_BRIGHTNESS = 1
+MERLOT_FRAME_CONTRAST = 2
+
 
 class MerlotError(RuntimeError):
     def __init__(self, code: int, msg: str):

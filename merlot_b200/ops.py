@@ -4,6 +4,7 @@ from __future__ import annotations
 import ctypes as C
 from typing import Optional
 
+import numpy as np
 import torch
 
 from . import _lib as L
@@ -415,6 +416,44 @@ class WsPlan:
 
     def backward(self):
         L.lib().merlot_ws_weights_bwd_multi(self.items_dev.data_ptr(), len(self.names), self.n_blocks, _stream())
+
+
+FRAME_FIELDS = ("src_offset", "src_h", "src_w", "scaled_h", "scaled_w", "offset_y", "offset_x", "method", "augment")
+
+
+def frame_table(plan, src_bytes: int) -> np.ndarray:
+    """merlot_frame_t descriptors of a frame plan: `plan` maps every FRAME_FIELDS key to n integers and "factor" to [n, 3]
+    floats.  The kernel reads the table unchecked, so every frame is checked here against the header's conditions."""
+    n = len(plan["src_h"])
+    t = np.zeros(n, dtype=np.dtype(L.merlot_frame_t))
+    for k in FRAME_FIELDS:
+        t[k] = np.asarray(plan[k], dtype=np.int64)
+    fac = np.asarray(plan["factor"], dtype=np.float32).reshape(n, 3)
+    t["factor_r"], t["factor_g"], t["factor_b"] = fac[:, 0], fac[:, 1], fac[:, 2]
+    ok = ((t["src_h"] >= 1) & (t["src_w"] >= 1) & (t["scaled_h"] >= 1) & (t["scaled_w"] >= 1) & (t["offset_y"] >= 0) &
+          (t["offset_x"] >= 0) & (t["method"] >= 0) & (t["method"] <= 3) & (t["augment"] >= 0) & (t["augment"] <= 2) &
+          (t["src_offset"] >= 0) & (t["src_offset"] + 3 * t["src_h"].astype(np.int64) * t["src_w"] <= src_bytes))
+    if n == 0 or not ok.all():
+        bad = np.flatnonzero(~ok)[:4].tolist()
+        raise L.MerlotShapeError(L.MERLOT_ESHAPE, f"frames_prepare: invalid frame descriptors {bad} (of {n})")
+    return t
+
+
+def frames_prepare(src: torch.Tensor, plan, out_h: int, out_w: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """K14: bf16 [n, out_h, out_w, 3] <- convert, resize_and_pad, where(isfinite), augment and cast of n uint8 HWC frames packed
+    in `src` (a uint8 CUDA tensor), as `plan` (see frame_table) says.  Enqueued on the current stream."""
+    _require_cuda(src, out)
+    assert src.dtype == torch.uint8 and src.is_contiguous()
+    table = frame_table(plan, src.numel())
+    n = len(table)
+    if out is None:
+        out = torch.empty((n, out_h, out_w, 3), dtype=torch.bfloat16, device=src.device)
+    assert out.dtype == torch.bfloat16 and out.is_contiguous() and tuple(out.shape) == (n, out_h, out_w, 3)
+    table_dev = torch.from_numpy(table.view(np.uint8)).pin_memory().to(src.device, non_blocking=True)
+    mean_ws = torch.empty(n * 3, dtype=torch.float32, device=src.device)
+    L.lib().merlot_frames_prepare(table_dev.data_ptr(), n, src.data_ptr(), out_h, out_w, mean_ws.data_ptr(), out.data_ptr(),
+                                  _stream())
+    return out
 
 
 def add_bf16(a, b, out):

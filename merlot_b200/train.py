@@ -20,6 +20,7 @@ from typing import Dict, Optional
 import torch
 
 from .config import NeatConfig
+from .dataloader import input_fn_builder, train_files
 from .modeling import MerlotModel, START
 from .optimization import build_optimizer_from_config
 from .params import ParamStore
@@ -251,20 +252,35 @@ def _step_for(config: NeatConfig):
 
 def main(argv=None):
     """`python -m merlot_b200.train configs/merlot.yaml` (or merlot_vcr.yaml) -- the role of model/train.py:9-26 and
-    downstream/vcr/train.py on synthetic data."""
+    downstream/vcr/train.py.  Pretraining reads data.train_file when it matches at least one file (dataloader.input_fn_builder)
+    and otherwise trains on synthetic batches; VCR fine-tuning always trains on synthetic batches."""
     config = NeatConfig.from_args("Train MERLOT (H100-native)", argv=argv)
     dist = DataParallel() if int(os.environ.get("WORLD_SIZE", "1")) > 1 else None
     if torch.cuda.is_available():
         torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
     builder, make_batch = _step_for(config)
     model_fn = builder(config, dist=dist)
-    per_rank = max(1, config.device.get("train_batch_size", 8) // (dist.world if dist else 1))
-    for step in range(config.optimizer.get("num_train_steps", 10)):
-        feats = make_batch(config, per_rank, seed=step + (dist.rank if dist else 0) * 100003)
-        spec = model_fn(feats, None, "train", None)
-        spec.train_op()
-        if step % 10 == 0 and (dist is None or dist.rank == 0):
-            print(f"step {step} loss {spec.loss:.4f} lr {spec.metrics['learning_rate']:.3e}", flush=True)
+    rank, world = (dist.rank, dist.world) if dist else (0, 1)
+    per_rank = max(1, config.device.get("train_batch_size", 8) // world)
+    pipeline = None
+    if make_batch is synthetic_batch and train_files(config.data):
+        pipeline = input_fn_builder(config, is_training=True, rank=rank, world=world, seed=0, batch_size=per_rank)
+    elif rank == 0:
+        print(f"data.train_file {config.data.get('train_file')!r} matches no file: training on synthetic batches"
+              if make_batch is synthetic_batch else "VCR fine-tuning: training on synthetic batches", flush=True)
+    try:
+        for step in range(config.optimizer.get("num_train_steps", 10)):
+            if pipeline is not None:
+                feats = next(pipeline)
+            else:
+                feats = make_batch(config, per_rank, seed=step + rank * 100003)
+            spec = model_fn(feats, None, "train", None)
+            spec.train_op()
+            if step % 10 == 0 and rank == 0:
+                print(f"step {step} loss {spec.loss:.4f} lr {spec.metrics['learning_rate']:.3e}", flush=True)
+    finally:
+        if pipeline is not None:
+            pipeline.close()
 
 
 if __name__ == "__main__":
