@@ -206,7 +206,8 @@ int merlot_gelu_bwd_f32(const float* dy, const float* pre, float* dx, long long 
 /* bfloat16_getter cast (utils/model_utils.py:572-602) */
 int merlot_cast_f32_to_bf16(const float* x, void* y, long long n, void* stream);
 int merlot_cast_bf16_to_f32(const void* x, float* y, long long n, void* stream);
-/* tf.math.l2_normalize(axis=-1) (model/modeling.py:43) */
+/* tf.math.l2_normalize(axis=-1) (model/modeling.py:43).  inv f32 [rows] <- rsqrt(max(sum x^2, 1e-12)), negated on rows where the
+ * clamp is active (sum x^2 < 1e-12); bwd reads |inv| and takes the clamped branch (dx = dy * |inv|) exactly on those rows. */
 int merlot_l2norm_fwd(const float* x, float* y, float* inv, int rows, int H, void* stream);
 int merlot_l2norm_bwd(const float* dy, const float* y, const float* inv, float* dx, int rows, int H, void* stream);
 /* raw_cross_entropy_with_logits (utils/model_utils.py:313-332) + argmax accuracy; bwd: dlogits = coeff[r]*(softmax-onehot) */

@@ -543,7 +543,9 @@ __global__ void cast_bf16_f32_kernel(const bf16* __restrict__ x, float* __restri
 
 // -----------------------------------------------------------------------------------------------------------------
 // l2 normalise rows: y = x * rsqrt(max(sum x^2, 1e-12))  (tf.math.l2_normalize);  one warp per row, fp32
-// bwd: dx = inv * (dy - y * sum(dy*y))   (clamp inactive branch: dx = dy * inv)
+// bwd: dx = inv * (dy - y * sum(dy*y))   (clamped rows, sum x^2 < 1e-12: dx = dy * inv)
+// The forward stores inv with its sign bit set on clamped rows, so the backward takes the branch the forward took (TF's
+// Maximum sends the gradient to sum x^2 when sum x^2 >= eps); no threshold on inv can tell the two apart near 1e-12.
 // -----------------------------------------------------------------------------------------------------------------
 __global__ void l2norm_fwd_kernel(const float* __restrict__ x, float* __restrict__ y, float* __restrict__ inv_out, int rows, int H) {
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
@@ -551,9 +553,10 @@ __global__ void l2norm_fwd_kernel(const float* __restrict__ x, float* __restrict
   float s = 0.f;
   for (int c = lane; c < H; c += 32) { const float v = x[(size_t)row * H + c]; s += v * v; }
   s = warp_sum(s);
+  const bool clamped = s < 1e-12f;
   const float inv = rsqrtf(fmaxf(s, 1e-12f));
   for (int c = lane; c < H; c += 32) y[(size_t)row * H + c] = x[(size_t)row * H + c] * inv;
-  if (lane == 0) inv_out[row] = inv;
+  if (lane == 0) inv_out[row] = clamped ? -inv : inv;
 }
 __global__ void l2norm_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ y, const float* __restrict__ inv,
                                   float* __restrict__ dx, int rows, int H) {
@@ -562,8 +565,8 @@ __global__ void l2norm_bwd_kernel(const float* __restrict__ dy, const float* __r
   float s = 0.f;
   for (int c = lane; c < H; c += 32) s += dy[(size_t)row * H + c] * y[(size_t)row * H + c];
   s = warp_sum(s);
-  const float iv = inv[row];
-  const bool clamped = iv >= 0.999e6f;  // sum x^2 <= 1e-12
+  const bool clamped = signbit(inv[row]);  // the forward's decision: sum x^2 < 1e-12
+  const float iv = fabsf(inv[row]);
   for (int c = lane; c < H; c += 32) {
     const size_t o = (size_t)row * H + c;
     dx[o] = clamped ? dy[o] * iv : iv * (dy[o] - y[o] * s);

@@ -414,34 +414,86 @@ def test_layernorm_bwd_fused(ops, rows, H, with_dres, p):
         assert rel(dbias, 2 * dx.float().sum(0)) < 1e-5
 
 
-def test_softmax_ce_and_l2norm(ops):
-    g = torch.Generator().manual_seed(0)
-    R, Cn, ld = 37, 50370, 50432
-    logits = torch.zeros(R, ld)
+def _l2norm_boundary_rows(g, H):
+    """Rows whose sum of squares sits at tf.math.l2_normalize's epsilon (1e-12, compared in fp32 on the device):
+    0, 0.5e-12 (clamped), exactly the fp32 epsilon, 1.001e-12 and 4e-12 (not clamped).  The `exactly` row has two non-zeros,
+    in lanes 0 and 1 of the kernel's warp: its fp32 sum is fl(fl(a^2) + fl(b^2)) == float32(1e-12) in any order, while the
+    float64 sum of the oracle is >= 1e-12, so both sides take Maximum's not-clamped branch (the gradient goes to sum x^2 when
+    it is >= eps).  The other rows spread over all H columns; their sums are 1e-3 or more away from the epsilon."""
+    rows = torch.zeros(5, H)
+    for i, s2 in ((1, 0.5e-12), (3, 1.001e-12), (4, 4e-12)):
+        u = torch.randn(H, generator=g, dtype=torch.float64)
+        rows[i] = (u * (s2 ** 0.5 / u.norm())).float()
+    a, b = np.float32(8.944272167354939e-07), np.float32(4.4721355152432807e-07)
+    assert np.float32(np.float32(a * a) + np.float32(b * b)) == np.float32(1e-12) and float(a) ** 2 + float(b) ** 2 >= 1e-12
+    rows[2, 0], rows[2, 1] = float(a), float(b)
+    return rows
+
+
+# (classes, logits row stride, dlogits dtype, argmax ties): the MLM head's vocabulary with bf16 dlogits (padded to ld 50432),
+# the contrastive / temporal heads' small C
+CE_CASES = [(50370, 50432, torch.float32, False), (50370, 50432, torch.bfloat16, True), (4, 4, torch.float32, True),
+            (32, 32, torch.bfloat16, True), (32, 40, torch.float32, False)]
+
+
+def _softmax_ce_case(ops, Cn, ld, d_dtype, ties):
+    """One CE_CASES entry: raw_cross_entropy_with_logits (utils/model_utils.py:313-332) + argmax accuracy, and its backward into
+    fp32 or bf16 dlogits (padded columns exactly 0; bf16 = the fp32 result rounded once).  Ties: several exact maxima in
+    different warps, in the same thread and with the label on a later one -- tf.argmax keeps the first."""
+    case = (Cn, ld, d_dtype, ties)
+    g = torch.Generator().manual_seed(Cn + ld)
+    R = 37
+    logits = torch.full((R, ld), 1e4)  # padding columns are never read
     logits[:, :Cn] = torch.randn(R, Cn, generator=g) * 3
     labels = torch.randint(0, Cn, (R,), generator=g, dtype=torch.int32)
+    if ties:
+        spots = [[5, 1000], [37, 290, 700], [100, 356], [Cn - 1, 0]] if Cn > 1000 else [[1, Cn - 1], [0, Cn // 2], [2, 3]]
+        for r, cols in enumerate(spots):
+            logits[r, :Cn] = torch.randn(Cn, generator=g)
+            logits[r, cols] = 9.0
+            labels[r] = cols[-1] if r % 2 else cols[0]
     lr = logits[:, :Cn].clone().requires_grad_(True)
     per_ref = O.raw_cross_entropy_with_logits(lr, labels)
     per, lse, corr = (torch.empty(R, device=DEV) for _ in range(3))
     ops.softmax_ce_fwd(logits.to(DEV), labels.to(DEV), Cn, per, lse, corr)
-    assert torch.allclose(per.cpu(), per_ref.detach(), rtol=1e-5, atol=1e-5)
-    assert torch.equal(corr.cpu(), (lr.argmax(-1) == labels).float())
+    assert torch.allclose(per.cpu(), per_ref.detach(), rtol=1e-5, atol=1e-5), case
+    assert torch.equal(corr.cpu(), (lr.argmax(-1) == labels).float()), case
+    if ties:
+        assert corr.cpu()[1] == 0.0 and corr.cpu()[0] == 1.0, case  # label on the second maximum / on the first
     coeff = torch.rand(R, generator=g)
     (per_ref * coeff).sum().backward()
-    dlog = torch.empty(R, ld, dtype=torch.float32, device=DEV)
+    dlog = torch.full((R, ld), float("nan"), dtype=torch.float32, device=DEV)
     ops.softmax_ce_bwd(logits.to(DEV), labels.to(DEV), Cn, lse, coeff.to(DEV), dlog)
-    assert rel(dlog[:, :Cn], lr.grad) < 1e-5 and float(dlog[:, Cn:].abs().max()) == 0.0
-    x = torch.randn(32, 768, generator=g)
-    xr = x.clone().requires_grad_(True)
+    assert rel(dlog[:, :Cn], lr.grad) < 1e-5 and not dlog[:, Cn:].any(), case
+    if d_dtype == torch.bfloat16:
+        dlb = torch.full((R, ld), float("nan"), dtype=torch.bfloat16, device=DEV)
+        ops.softmax_ce_bwd(logits.to(DEV), labels.to(DEV), Cn, lse, coeff.to(DEV), dlb)
+        assert torch.equal(dlb, dlog.bfloat16()), case  # padded columns included: exactly 0
+        assert rel(dlb[:, :Cn], lr.grad) < 4e-3, case   # one bf16 rounding
+
+
+def test_softmax_ce_and_l2norm(ops):
+    """Softmax cross-entropy for every CE_CASES entry (_softmax_ce_case), then l2_normalize forward / backward on random rows
+    and on the epsilon boundary rows of _l2norm_boundary_rows, dx per row against autograd of O.l2_normalize in float64."""
+    for case in CE_CASES:
+        _softmax_ce_case(ops, *case)
+    g = torch.Generator().manual_seed(0)
+    H = 768
+    x = torch.cat([torch.randn(32, H, generator=g), _l2norm_boundary_rows(g, H)])
+    n = x.shape[0]
+    xr = x.double().requires_grad_(True)
     y_ref = O.l2_normalize(xr)
-    y, inv = torch.empty(32, 768, device=DEV), torch.empty(32, device=DEV)
+    y, inv = torch.empty(n, H, device=DEV), torch.empty(n, device=DEV)
     ops.l2norm_fwd(x.to(DEV), y, inv)
     assert rel(y, y_ref) < 1e-6
-    dy = torch.randn(32, 768, generator=g)
-    y_ref.backward(dy)
-    dx = torch.empty(32, 768, device=DEV)
+    dy = torch.randn(n, H, generator=g, dtype=torch.float64)
+    dy = (dy + 30.0 * y_ref.detach()).float()  # a component along y: the clamped branch drops its projection
+    y_ref.backward(dy.double())
+    dx = torch.empty(n, H, device=DEV)
     ops.l2norm_bwd(dy.to(DEV), y, inv, dx)
-    assert rel(dx, xr.grad) < 1e-5
+    dxc = dx.cpu().double()
+    for r in range(n):
+        assert rel(dxc[r], xr.grad[r]) < 1e-5, (r, rel(dxc[r], xr.grad[r]))
 
 
 # ---------------------------------------------------------------------------------------------------------------

@@ -203,6 +203,29 @@ def test_pool_col2im_ws_backward(ops):
     assert torch.equal(out.cpu(), (a.float() + b.float()).bfloat16())
 
 
+def test_ws_weights_multi_equals_per_kernel_launches(ops):
+    """merlot_ws_weights_multi / merlot_ws_weights_bwd_multi (ops.WsPlan: every conv kernel of the stem in one launch each) run
+    the same per-channel code as merlot_ws_weights / merlot_ws_weights_bwd: bit for bit the per-kernel results, for kernels
+    whose channel counts are not multiples of the 32-channel block (so blocks of one item end mid-way) and whose row counts
+    need padding; the gradients accumulate into non-zero buffers."""
+    g = torch.Generator().manual_seed(11)
+    shapes = {"a": (27, 40), "b": (576, 64), "c": (64, 24), "d": (9 * 16, 100)}
+    kernels = {n: (torch.randn(r, c, generator=g) * 0.2 + 0.05).to(DEV) for n, (r, c) in shapes.items()}
+    grads = {n: torch.full(s, 0.5, device=DEV) for n, s in shapes.items()}
+    plan = ops.WsPlan(kernels, grads, DEV)
+    plan.standardise()
+    for n, (r, c) in shapes.items():
+        kp = (r + 7) // 8 * 8
+        assert torch.equal(plan.wstd[n], ops.ws_weights(kernels[n], kp)), n
+    for n, (r, c) in shapes.items():
+        plan.dws[n].copy_(torch.randn(plan.dws[n].shape, generator=g))
+    plan.backward()
+    for n, (r, c) in shapes.items():
+        dw = torch.full((r, c), 0.5, device=DEV)
+        ops.ws_weights_bwd(plan.dws[n][:r], kernels[n], dw)
+        assert torch.equal(grads[n], dw), n
+
+
 def _stem_model(tiny_cfg, h0, w0, batch=2, nc=2, save=True):
     from merlot_b200.modeling import MerlotModel
     from tests.test_gpu_model import build, synth

@@ -33,6 +33,70 @@ def test_binding_covers_every_header_symbol():
     assert lib.merlot_abi_version() == 1
 
 
+# Header functions no tests/test_gpu_*.py has to call by name.  Pure queries and sizes return host values that the GPU tests
+# use without asserting them one by one (test_attention_bwd_dq_mode_boundary pins the dQ pair); the stack drivers run three
+# times in every whole-model step of test_gpu_model.py, test_gpu_fullsize.py and test_gpu_vcr_train.py.
+UNTESTED_BY_NAME_OK = {
+    "merlot_abi_version", "merlot_last_error", "merlot_set_sm_reserve",   # queries / process settings
+    "merlot_launch_count", "merlot_reset_launch_count",                   # launch counters
+    "merlot_gemm_profile_begin", "merlot_gemm_profile_end",               # bench.py's K1 profiler pair
+    "merlot_stack_forward", "merlot_stack_backward",                      # whole transformer stacks
+}
+
+
+def _calls_in(path):
+    """Names of every called attribute or function in a Python file's code (not in its comments or strings)."""
+    import ast
+    names = set()
+    for node in ast.walk(ast.parse(open(path).read())):
+        if isinstance(node, ast.Call):
+            f = node.func
+            names.add(f.attr if isinstance(f, ast.Attribute) else getattr(f, "id", None))
+    return names
+
+
+def _ops_wrappers():
+    """{wrapper name: merlot_* functions it calls} for every function and method of merlot_b200/ops.py; a method is listed
+    as Class.method."""
+    import ast
+    tree = ast.parse(open(os.path.join(ROOT, "merlot_b200", "ops.py")).read())
+    out = {}
+
+    def add(fn, key):
+        out[key] = {n.attr for n in ast.walk(fn) if isinstance(n, ast.Attribute) and n.attr.startswith("merlot_")}
+    for node in tree.body:
+        if isinstance(node, ast.FunctionDef):
+            add(node, node.name)
+        elif isinstance(node, ast.ClassDef):
+            for m in node.body:
+                if isinstance(m, ast.FunctionDef):
+                    add(m, f"{node.name}.{m.name}")
+    return out
+
+
+def test_every_header_function_is_called_by_a_gpu_test():
+    """Each merlot_* function of include/merlot_b200.h is called by some tests/test_gpu_*.py, either by name or through an
+    ops.py wrapper that calls it (a method counts where its class is constructed in the same file).  A new entry point without
+    a direct test, or the removal of the last test of one, fails here.  Exceptions: UNTESTED_BY_NAME_OK and the *_bytes /
+    *_dq_parts size queries."""
+    import glob
+    wrappers = _ops_wrappers()
+    covered = set()
+    files = sorted(glob.glob(os.path.join(HERE, "test_gpu_*.py")))
+    assert len(files) >= 8, files
+    for path in files:
+        calls = _calls_in(path)
+        covered |= {c for c in calls if c and c.startswith("merlot_")}
+        for key, fns in wrappers.items():
+            cls, _, meth = key.rpartition(".")
+            if (meth in calls) and (not cls or cls in calls):
+                covered |= fns
+    exempt = {n for n in _header_functions() if n in UNTESTED_BY_NAME_OK or n.endswith(("_bytes", "_dq_parts"))}
+    assert exempt >= {n for n in UNTESTED_BY_NAME_OK}, "UNTESTED_BY_NAME_OK names a function the header no longer has"
+    missing = [n for n in _header_functions() if n not in covered and n not in exempt]
+    assert not missing, f"header functions no GPU test calls: {missing}"
+
+
 def test_attention_bwd_dq_mode_boundary():
     """merlot_attention_bwd reduces dQ through per-key-tile fp32 slices while the sequence has at most 4 tiles of 128 keys
     (S <= 512) and atomically into one slice beyond (0 = atomic mode); the workspace a caller allocates follows the mode:
