@@ -409,6 +409,21 @@ typedef struct merlot_frame {
 int merlot_frames_prepare(const merlot_frame_t* frames_dev, int n, const void* src_u8, int out_h, int out_w, float* mean_ws,
                           void* out_bf16, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * K15: CRC-32C of many device byte ranges in one launch -- the per-tensor checksum of a TensorFlow V2 checkpoint
+ * (BundleEntryProto.crc32c, tensorflow/core/util/tensor_bundle) computed where the tensors already are; see csrc/crc32c.cu.
+ * Standard CRC-32C (Castagnoli, reflected polynomial 0x82F63B78, init and xor-out 0xFFFFFFFF), unmasked:
+ * crc_out_dev[i] = crc32c(segs[i].ptr[0 .. bytes)); "123456789" gives 0xE3069283 and a 0-byte segment gives 0.
+ * segs_dev is a device table of n segments.  A segment may start at any byte address, have any length >= 0 and overlap
+ * others; ptr must be readable for `bytes` bytes (the kernel reads the table unchecked).  Integer arithmetic only: the result
+ * is bit-exact and does not depend on the launch shape.  crc_out_dev is overwritten (it is zeroed, then accumulated).
+ * ------------------------------------------------------------------------------------------------------------ */
+typedef struct merlot_crc_seg {
+  const void* ptr;
+  long long bytes;
+} merlot_crc_seg_t;
+int merlot_crc32c_multi(const merlot_crc_seg_t* segs_dev, int n, unsigned* crc_out_dev, void* stream);
+
 /* bench.py roofline support: time every K1 launch with CUDA events on its own stream between begin/end.
  * end() synchronises the device and returns the summed duration (ms), algorithmic FLOPs (2*M*N*K) and launch count. */
 void merlot_gemm_profile_begin(void);

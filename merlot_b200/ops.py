@@ -456,6 +456,29 @@ def frames_prepare(src: torch.Tensor, plan, out_h: int, out_w: int, out: Optiona
     return out
 
 
+def crc32c_multi(views, out: Optional[torch.Tensor] = None):
+    """K15: standard CRC-32C (unmasked) of every uint8 CUDA view in `views`, in one launch.  Views may start at any byte,
+    be empty or overlap.  With `out` (an int32 CUDA tensor of len(views) entries) the CRCs stay on the device, enqueued on the
+    current stream, and `out` is returned; otherwise this synchronises and returns a list of ints."""
+    n = len(views)
+    if n == 0:
+        return out if out is not None else []
+    table = np.zeros(n, dtype=np.dtype(L.merlot_crc_seg_t))
+    for i, v in enumerate(views):
+        _require_cuda(v)
+        if v.dtype != torch.uint8 or v.dim() != 1 or (v.numel() > 1 and v.stride(0) != 1):
+            raise L.MerlotShapeError(L.MERLOT_ESHAPE, f"crc32c_multi: view {i} is not a contiguous 1-D uint8 tensor")
+        table["ptr"][i], table["bytes"][i] = v.data_ptr(), v.numel()
+    dev = views[0].device
+    result = out if out is not None else torch.empty(n, dtype=torch.int32, device=dev)
+    assert result.dtype == torch.int32 and result.is_cuda and result.numel() == n and result.is_contiguous()
+    table_dev = torch.from_numpy(table.view(np.uint8)).pin_memory().to(dev, non_blocking=True)
+    L.lib().merlot_crc32c_multi(table_dev.data_ptr(), n, result.data_ptr(), _stream())
+    if out is not None:
+        return out
+    return (result.cpu().numpy().view(np.uint32)).tolist()
+
+
 def add_bf16(a, b, out):
     L.lib().merlot_add_bf16(a.data_ptr(), b.data_ptr(), out.data_ptr(), a.numel(), _stream())
 

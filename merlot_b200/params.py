@@ -12,10 +12,14 @@ Storage differs from the TF variables in three places (converted by load_tf_dict
 
 `task` selects the variable set of one reference graph: "pretrain" (model/modeling.py model_fn, every head) or "vcr"
 (downstream/vcr/modeling.py model_fn: MerlotModel(mask_input=False) + the answer / rationale classifier towers).
+
+save_checkpoint / restore_checkpoint write and read the whole training state (parameters, Adam slots, global_step) as the
+TensorFlow V2 checkpoints the reference's Estimator keeps in output_dir.
 """
 from __future__ import annotations
 
 import math
+import os
 import re
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Tuple
@@ -336,30 +340,145 @@ class ParamStore:
         from .tf_checkpoint import load_checkpoint
         return self.load_tf_dict(load_checkpoint(prefix), strict=False)
 
-    def to_tf_dict(self, which: str = "p") -> Dict[str, torch.Tensor]:
-        buf = {"p": self.p, "g": self.g}[which]
-        out = {}
+    def tf_views(self, buf: torch.Tensor) -> List[Tuple[Entry, str, torch.Tensor]]:
+        """(entry, reference name, view of `buf` in the reference variable's shape) for every reference variable, in arena
+        entry order: q/k/v split into column views, zero-padded columns (`ref_cols`) left out, conv kernels HWIO, position
+        tables [1, 64, 64, H], CLS embeddings [1, n, H].  `buf` is any arena (p, g, m, v); views may be non-contiguous."""
+        out = []
         for e in self.entries.values():
-            t = self._view(buf, e.name).detach().float().cpu()
+            t = self._view(buf, e.name)
             if len(e.tf_names) == 3:
-                for nm, part in zip(e.tf_names, t.chunk(3, dim=-1)):
-                    out[nm] = part.contiguous()
-            elif e.ref_cols:
-                out[e.tf_names[0]] = t[..., :e.ref_cols].contiguous()
+                out.extend((e, nm, part) for nm, part in zip(e.tf_names, t.chunk(3, dim=-1)))
+                continue
+            if e.ref_cols:
+                t = t[..., :e.ref_cols]
             elif e.name.endswith("vision_transformer/conv2d/kernel"):
                 Pp = self.cfg["patch_size"]
-                out[e.tf_names[0]] = t.reshape(Pp, Pp, 3, -1)
+                t = t.reshape(Pp, Pp, 3, -1)
             elif _CONV_KERNEL.search(e.name):  # hybrid stem: [kh*kw*cin, cout] -> HWIO
                 kh = {n_: s_ for n_, s_ in stem_variables("vision_backbone/vision_transformer", self.cfg["resnet_layers"], 64,
                                                           self.cfg["hidden_size"])}[e.name][0]
-                out[e.tf_names[0]] = t.reshape(kh, kh, t.shape[0] // (kh * kh), -1)
+                t = t.reshape(kh, kh, t.shape[0] // (kh * kh), -1)
             elif e.name.endswith("/pos_embs"):
-                out[e.tf_names[0]] = t.reshape(1, 64, 64, -1)
+                t = t.reshape(1, 64, 64, -1)
             elif e.name.endswith("/cls_emb"):
-                out[e.tf_names[0]] = t.reshape(1, t.shape[0], -1)
-            else:
-                out[e.tf_names[0]] = t
+                t = t.reshape(1, t.shape[0], -1)
+            out.append((e, e.tf_names[0], t))
         return out
+
+    def to_tf_dict(self, which: str = "p") -> Dict[str, torch.Tensor]:
+        buf = {"p": self.p, "g": self.g}[which]
+        return {nm: t.detach().float().cpu().contiguous() for _, nm, t in self.tf_views(buf)}
+
+    # ---- full training state as a TensorFlow V2 checkpoint ----
+    def slot_entries(self, skip=()) -> List[Entry]:
+        """Entries whose reference variables own Adam slots (`<name>/adam_m`, `<name>/adam_v`).  The reference's
+        apply_gradients creates them for every variable it updates (utils/optimization.py:339-383): a trainable variable --
+        not in a learning-rate-0 group, those are removed from tvars (:149-156) -- whose gradient is not None (:343-344).
+        `skip` names the entries whose gradient is None in the training graph (the training step's `skip` list)."""
+        skip = set(skip)
+        unknown = skip - set(self.entries)
+        if unknown:
+            raise KeyError(f"skip names entries the store does not have: {sorted(unknown)}")
+        return [e for e in self.entries.values() if e.hyper[0] != 0 and e.name not in skip]
+
+    def _checkpoint_tensors(self, skip):
+        """(name, TF dtype, device view) of every variable of a checkpoint of this store, in data-file order: global_step,
+        the fp32 parameters, then the bf16 slots (every offset stays a multiple of its element size)."""
+        from .tf_checkpoint import DT_BFLOAT16, DT_FLOAT
+        if not hasattr(self, "m"):
+            raise ValueError("checkpoints hold the optimizer state: build the ParamStore with with_optimizer_state=True")
+        slots = {e.name for e in self.slot_entries(skip)}
+        views = self.tf_views(self.p)
+        out = [(nm, DT_FLOAT, t) for _, nm, t in views]
+        for suffix, buf in (("adam_m", self.m), ("adam_v", self.v)):
+            out += [(f"{nm}/{suffix}", DT_BFLOAT16, t) for e, nm, t in self.tf_views(buf) if e.name in slots]
+        return out
+
+    def save_checkpoint(self, prefix: str, skip=()) -> Dict[str, float]:
+        """Write the training state as the TensorFlow V2 checkpoint `prefix` (model.ckpt-<step> of the reference's Estimator):
+        every variable under its reference name (as to_tf_dict maps it), the bf16 `adam_m` / sign-packed `adam_v` slots of
+        slot_entries(skip) bit for bit, and `global_step` (int64).  The data file is gathered on the device, checksummed
+        there by one K15 launch, copied to pinned host memory at once and written by tf_checkpoint.write_bundle.  Extra
+        device memory: one buffer of the data file's size.  Returns the seconds each phase took and the bytes written."""
+        import time
+        from .tf_checkpoint import DT_INT64, write_bundle
+        t0 = time.perf_counter()
+        tensors = [("global_step", DT_INT64, torch.tensor(self.global_step, dtype=torch.int64, device=self.device))]
+        tensors += self._checkpoint_tensors(skip)
+        sizes = [t.numel() * t.element_size() for _, _, t in tensors]
+        offs = [0]
+        for s in sizes:
+            offs.append(offs[-1] + s)
+        stage = torch.empty(offs[-1], dtype=torch.uint8, device=self.device)
+        for (_, _, t), o, s in zip(tensors, offs, sizes):
+            stage[o:o + s].view(t.dtype).view(t.shape).copy_(t)
+        torch.cuda.synchronize(self.device)
+        t1 = time.perf_counter()
+        crcs = ops.crc32c_multi([stage[o:o + s] for o, s in zip(offs, sizes)])
+        t2 = time.perf_counter()
+        host = torch.empty(offs[-1], dtype=torch.uint8, pin_memory=True)
+        host.copy_(stage)
+        del stage
+        t3 = time.perf_counter()
+        arr = host.numpy()
+        write_bundle(prefix, [(nm, dt, tuple(t.shape), arr[o:o + s], c)
+                              for (nm, dt, t), o, s, c in zip(tensors, offs, sizes, crcs)])
+        t4 = time.perf_counter()
+        return {"stage_s": t1 - t0, "crc_s": t2 - t1, "d2h_s": t3 - t2, "write_s": t4 - t3, "bytes": float(offs[-1])}
+
+    def restore_checkpoint(self, prefix: str, skip=()) -> None:
+        """Restore p, m, v and global_step from a checkpoint written by save_checkpoint (or by the reference's Saver), then
+        refresh the bf16 copy.  The data file is copied to the device whole and every tensor's CRC-32C is checked there (K15);
+        a mismatch raises CheckpointFormatError naming the tensor.  Like Saver.restore, a variable or slot this store needs
+        that the checkpoint lacks raises, as does a shape or dtype mismatch; variables the store does not have are ignored.
+        Padding columns and padding elements restore as zero; slots of variables outside slot_entries(skip) restore as zero.
+        (load_checkpoint is the other operation: init_checkpoint's restore-by-name of model variables.)"""
+        import numpy as np
+        from .tf_checkpoint import DT_INT64, CheckpointFormatError, _index, mask_crc
+        header, entries = _index(prefix, True)
+        want = [("global_step", DT_INT64, None)] + self._checkpoint_tensors(skip)
+        missing = [nm for nm, _, _ in want if nm not in entries]
+        if missing:
+            raise CheckpointFormatError(f"{prefix}: {len(missing)} variables the store needs are not in the checkpoint: "
+                                        f"{', '.join(missing[:8])}{' ...' if len(missing) > 8 else ''}")
+        for nm, dt, t in want:
+            e = entries[nm]
+            shape = [] if t is None else list(t.shape)
+            if int(e["dtype"]) != dt or [int(d) for d in e["shape"]] != shape:
+                raise CheckpointFormatError(f"{nm}: checkpoint has dtype {e['dtype']} shape {e['shape']}, the store needs "
+                                            f"dtype {dt} shape {shape}")
+            if e["slices"]:
+                raise NotImplementedError(f"{nm}: partitioned (sliced) variables are not supported")
+        if header["num_shards"] != 1 or any(int(e["shard_id"]) for e in entries.values()):
+            raise NotImplementedError(f"{prefix}: sharded checkpoints are not supported")
+        path = f"{prefix}.data-00000-of-00001"
+        size = os.path.getsize(path)
+        for nm, e in entries.items():
+            if int(e["offset"]) < 0 or int(e["size"]) < 0 or int(e["offset"]) + int(e["size"]) > size:
+                raise CheckpointFormatError(f"{nm}: data shard is shorter than the index says")
+        host = torch.empty(size, dtype=torch.uint8, pin_memory=True)
+        with open(path, "rb") as f:
+            if f.readinto(memoryview(host.numpy())) != size:
+                raise CheckpointFormatError(f"{path}: short read")
+        data = host.to(self.device)
+        checked = sorted((nm, e) for nm, e in entries.items() if e["crc32c"] is not None)
+        crcs = ops.crc32c_multi([data[int(e["offset"]):int(e["offset"]) + int(e["size"])] for _, e in checked])
+        for (nm, e), c in zip(checked, crcs):
+            if mask_crc(c) != e["crc32c"]:
+                raise CheckpointFormatError(f"{nm}: tensor checksum mismatch")
+        with torch.no_grad():
+            for buf in (self.p, self.m, self.v):
+                buf.zero_()
+            for nm, _, t in want[1:]:
+                o, s = int(entries[nm]["offset"]), int(entries[nm]["size"])
+                src = data[o:o + s]
+                if o % t.element_size():
+                    src = src.clone()
+                t.copy_(src.view(t.dtype).view(t.shape))
+        o = int(entries["global_step"]["offset"])
+        self.global_step = int(np.frombuffer(host.numpy()[o:o + 8].tobytes(), dtype="<i8")[0])
+        self.sync_bf16()
 
     def init_reference(self, seed: int = 0):
         """Reference initialisers (truncated normal 0.02 / variance-scaling patch kernel / LN 1,0 / zero biases; the VCR

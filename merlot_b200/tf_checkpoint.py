@@ -10,7 +10,9 @@ here, so this module reads the on-disk format directly:
   <prefix>.data-SSSSS-of-NNNNN      the raw little-endian tensor bytes, addressed by (shard_id, offset, size)
 
 `list_variables(prefix)` mirrors tf.train.list_variables; `load_checkpoint(prefix)` returns {name: torch.Tensor};
-`ParamStore.load_tf_dict(..., strict=False)` applies the reference's by-name semantics.
+`ParamStore.load_tf_dict(..., strict=False)` applies the reference's by-name semantics.  `write_bundle` writes the same
+format (what ParamStore.save_checkpoint uses), and `update_checkpoint_state` / `latest_checkpoint` keep the `checkpoint`
+state file of a model directory.
 
 UNPINNED against TensorFlow-written files: no checkpoint and no TensorFlow exist in this environment; the reader follows
 the published formats (leveldb table_format.md, tensorflow/core/protobuf/tensor_bundle.proto, tensor_shape.proto, snappy
@@ -364,3 +366,211 @@ def load_checkpoint(prefix: str, names: Optional[Iterable[str]] = None, verify_c
             t = torch.from_numpy(arr.copy())
         out[name] = t
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# writer (the same formats; what tf.train.Saver writes for a single-shard V2 checkpoint)
+# ---------------------------------------------------------------------------------------------------------------
+DT_FLOAT = 1
+DT_INT64 = 9
+_ITEMSIZE = {DT_FLOAT: 4, DT_BFLOAT16: 2, DT_INT64: 8}
+BLOCK_SIZE = 262144       # TensorFlow's table::Options.block_size: a data block is closed once it reaches this many bytes
+RESTART_INTERVAL = 16     # table::Options.block_restart_interval
+
+
+def _varint(v: int) -> bytes:
+    out = bytearray()
+    while True:
+        b = v & 0x7F
+        v >>= 7
+        if v:
+            out.append(b | 0x80)
+        else:
+            out.append(b)
+            return bytes(out)
+
+
+def _pb(field: int, wire: int, payload: bytes) -> bytes:
+    return _varint((field << 3) | wire) + payload
+
+
+def _pb_bytes(field: int, payload: bytes) -> bytes:
+    return _pb(field, 2, _varint(len(payload)) + payload)
+
+
+def _header_proto() -> bytes:
+    """BundleHeaderProto{num_shards: 1, endianness: LITTLE (0, the proto3 default, not serialised), version{producer: 1}}."""
+    return _pb(1, 0, _varint(1)) + _pb_bytes(3, _pb(1, 0, _varint(1)))
+
+
+def _entry_proto(dtype: int, shape, offset: int, size: int, masked_crc: int) -> bytes:
+    """BundleEntryProto of shard 0; proto3 leaves zero scalars out, the crc32c is always written."""
+    dims = b"".join(_pb_bytes(2, _pb(1, 0, _varint(d)) if d else b"") for d in shape)
+    out = _pb(1, 0, _varint(dtype)) + _pb_bytes(2, dims)
+    if offset:
+        out += _pb(4, 0, _varint(offset))
+    if size:
+        out += _pb(5, 0, _varint(size))
+    return out + _pb(6, 5, struct.pack("<I", masked_crc))
+
+
+def _block(items: List[Tuple[bytes, bytes]], restart_interval: int) -> bytes:
+    """leveldb block: prefix-compressed entries with a full key every `restart_interval` entries, then the restart array."""
+    buf, restarts, last = bytearray(), [], b""
+    for i, (k, v) in enumerate(items):
+        shared = 0
+        if i % restart_interval == 0:
+            restarts.append(len(buf))
+        else:
+            n = min(len(k), len(last))
+            while shared < n and k[shared] == last[shared]:
+                shared += 1
+        buf += _varint(shared) + _varint(len(k) - shared) + _varint(len(v)) + k[shared:] + v
+        last = k
+    for r in restarts or [0]:  # an empty block still has one restart point (leveldb BlockBuilder)
+        buf += struct.pack("<I", r)
+    buf += struct.pack("<I", len(restarts or [0]))
+    return bytes(buf)
+
+
+def table_bytes(items: List[Tuple[bytes, bytes]], block_size: int = BLOCK_SIZE) -> bytes:
+    """A leveldb table of (key, value) pairs in strictly increasing key order: uncompressed data blocks, an empty metaindex
+    block, an index block whose keys are each data block's last key, every block followed by its type byte and masked CRC,
+    and the 48-byte footer."""
+    out = bytearray()
+
+    def emit(block: bytes) -> bytes:
+        off = len(out)
+        out.extend(block)
+        out.append(0)  # kNoCompression
+        out.extend(struct.pack("<I", mask_crc(crc32c(block + b"\x00"))))
+        return _varint(off) + _varint(len(block))
+
+    index, pending, size = [], [], 0
+    for i, (k, v) in enumerate(items):
+        if i and k <= items[i - 1][0]:
+            raise ValueError(f"table keys must be strictly increasing: {items[i - 1][0]!r} then {k!r}")
+        pending.append((k, v))
+        size += len(k) + len(v) + 8
+        if size >= block_size:
+            index.append((pending[-1][0], emit(_block(pending, RESTART_INTERVAL))))
+            pending, size = [], 0
+    if pending:
+        index.append((pending[-1][0], emit(_block(pending, RESTART_INTERVAL))))
+    meta = emit(_block([], 1))
+    idx = emit(_block(index, 1))
+    footer = meta + idx
+    return bytes(out) + footer + b"\x00" * (40 - len(footer)) + struct.pack("<Q", TABLE_MAGIC)
+
+
+def _fsync_dir(path: str) -> None:
+    fd = os.open(path, os.O_RDONLY)
+    try:
+        os.fsync(fd)
+    finally:
+        os.close(fd)
+
+
+def write_bundle(prefix: str, entries, block_size: int = BLOCK_SIZE) -> None:
+    """Write the single-shard V2 checkpoint `<prefix>.data-00000-of-00001` + `<prefix>.index`.
+
+    `entries`: (name, dtype, shape, data, crc32c) with dtype DT_FLOAT, DT_BFLOAT16 or DT_INT64, `data` the tensor's
+    little-endian bytes (bytes or any buffer, e.g. a slice of a pinned host array) and `crc32c` its unmasked CRC-32C or None
+    to compute it here.  The data file holds the tensors back to back in the given order; the index lists them by name.
+    Both files are written under temporary names and fsynced; the data file is renamed into place first and the index last,
+    so an interrupted write never leaves an index that points into a missing or partial data file."""
+    d = os.path.dirname(os.path.abspath(prefix))
+    data_path, index_path = f"{prefix}.data-00000-of-00001", f"{prefix}.index"
+    items, offset, names = [(b"", _header_proto())], 0, set()
+    for name, dtype, shape, data, crc in entries:
+        if dtype not in _ITEMSIZE:
+            raise ValueError(f"{name}: unsupported dtype {dtype}")
+        if name == "" or name in names:
+            raise ValueError(f"duplicate or empty tensor name {name!r}")
+        names.add(name)
+        size = memoryview(data).nbytes
+        if size != _ITEMSIZE[dtype] * int(np.prod(shape, dtype=np.int64)):
+            raise ValueError(f"{name}: {size} bytes for shape {list(shape)} of dtype {dtype}")
+        if crc is None:
+            crc = crc32c(data)
+        items.append((name.encode("utf-8"), _entry_proto(dtype, [int(s) for s in shape], offset, size, mask_crc(int(crc)))))
+        offset += size
+    items.sort(key=lambda kv: kv[0])
+    index = table_bytes(items, block_size)
+    tag = f".tempstate{os.getpid()}"
+    try:
+        with open(data_path + tag, "wb") as f:
+            for _, _, _, data, _ in entries:
+                f.write(data)
+            f.flush()
+            os.fsync(f.fileno())
+        with open(index_path + tag, "wb") as f:
+            f.write(index)
+            f.flush()
+            os.fsync(f.fileno())
+        os.replace(data_path + tag, data_path)
+        os.replace(index_path + tag, index_path)
+    finally:
+        for p in (data_path + tag, index_path + tag):
+            if os.path.exists(p):
+                os.remove(p)
+    _fsync_dir(d)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# the `checkpoint` state file (tf.train.CheckpointState as a text proto)
+# ---------------------------------------------------------------------------------------------------------------
+STATE_FILE = "checkpoint"
+
+
+def _quote(s: str) -> str:
+    return '"' + s.replace("\\", "\\\\").replace('"', '\\"') + '"'
+
+
+def _read_state(directory: str) -> Tuple[Optional[str], List[str]]:
+    path = os.path.join(directory, STATE_FILE)
+    if not os.path.exists(path):
+        return None, []
+    latest, every = None, []
+    with open(path, "r", encoding="utf-8") as f:
+        for line in f:
+            key, sep, val = line.strip().partition(":")
+            val = val.strip()
+            if not sep or len(val) < 2 or val[0] != '"' or val[-1] != '"':
+                continue
+            val = val[1:-1].replace('\\"', '"').replace("\\\\", "\\")
+            if key == "model_checkpoint_path":
+                latest = val
+            elif key == "all_model_checkpoint_paths":
+                every.append(val)
+    return latest, every
+
+
+def update_checkpoint_state(directory: str, prefix: str) -> None:
+    """Name `prefix` the latest checkpoint of `directory` and append it to all_model_checkpoint_paths (every earlier one is
+    kept).  Paths inside `directory` are written relative to it.  The file is replaced atomically: call this only once the
+    bundle itself is durable, so that a crash during a save leaves the previous checkpoint as the latest."""
+    d = os.path.abspath(directory)
+    p = os.path.abspath(prefix)
+    rel = os.path.relpath(p, d) if os.path.commonpath([d, p]) == d else p
+    _, every = _read_state(d)
+    every = [x for x in every if x != rel] + [rel]
+    text = f"model_checkpoint_path: {_quote(rel)}\n" + "".join(f"all_model_checkpoint_paths: {_quote(x)}\n" for x in every)
+    path = os.path.join(d, STATE_FILE)
+    tmp = path + f".tmp{os.getpid()}"
+    with open(tmp, "w", encoding="utf-8") as f:
+        f.write(text)
+        f.flush()
+        os.fsync(f.fileno())
+    os.replace(tmp, path)
+    _fsync_dir(d)
+
+
+def latest_checkpoint(directory: str) -> Optional[str]:
+    """tf.train.latest_checkpoint: the prefix the state file names (relative paths are taken relative to `directory`), or
+    None when there is no state file or its checkpoint has no index file."""
+    latest, _ = _read_state(directory)
+    if not latest:
+        return None
+    p = latest if os.path.isabs(latest) else os.path.join(directory, latest)
+    return p if os.path.exists(p + ".index") else None

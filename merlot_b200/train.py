@@ -250,26 +250,69 @@ def _step_for(config: NeatConfig):
     return model_fn_builder, synthetic_batch
 
 
+def variables_without_gradient(model_cfg: dict, store: ParamStore):
+    """Entries whose gradient is None in the training graph, so the reference's apply_gradients neither updates them nor
+    creates their Adam slots: the `skip` list model_fn_builder hands AdamW (no viz_viz temporal head without image
+    shuffling, no temporal heads at temporal_coef 0).  The VCR graph reaches every variable of its store."""
+    if store.task == "vcr":
+        return []
+    if model_cfg.get("temporal_coef", 1.0) > 0.0:
+        return [] if model_cfg.get("image_shuffle_prob", 0) > 0 else [n for n in store.entries if n.startswith("viz_viz_temporal/")]
+    return [n for n in store.entries if "_temporal/" in n]
+
+
 def main(argv=None):
     """`python -m merlot_b200.train configs/merlot.yaml` (or merlot_vcr.yaml) -- the role of model/train.py:9-26 and
     downstream/vcr/train.py.  Pretraining reads data.train_file when it matches at least one file (dataloader.input_fn_builder)
-    and otherwise trains on synthetic batches; VCR fine-tuning always trains on synthetic batches."""
+    and otherwise trains on synthetic batches; VCR fine-tuning always trains on synthetic batches.
+
+    Checkpoints, as the reference's Estimator keeps them (utils/neat_config.py:136-141): when device.output_dir already names
+    a latest checkpoint, every rank restores it (parameters, Adam slots, global_step; this takes precedence over
+    init_checkpoint) and training continues from its global_step to num_train_steps.  model.ckpt-<global_step> is written
+    whenever global_step is a multiple of device.iterations_per_loop (default 1000) and after the last step, and every
+    checkpoint is kept.  Rank 0 writes; all ranks then meet at a barrier.  The input pipeline's position is not saved: a
+    resumed run seeds it with the restored global_step so that it does not replay the first batches."""
     config = NeatConfig.from_args("Train MERLOT (H100-native)", argv=argv)
+    output_dir = str(config.device["output_dir"])
+    if "://" in output_dir:
+        raise ValueError(f"device.output_dir {output_dir!r}: only local directories are supported for checkpoints")
     dist = DataParallel() if int(os.environ.get("WORLD_SIZE", "1")) > 1 else None
     if torch.cuda.is_available():
         torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
+    from .tf_checkpoint import latest_checkpoint, update_checkpoint_state
     builder, make_batch = _step_for(config)
     model_fn = builder(config, dist=dist)
+    store = model_fn.store
+    skip = variables_without_gradient(config.model, store)
     rank, world = (dist.rank, dist.world) if dist else (0, 1)
+    resume = latest_checkpoint(output_dir)
+    if resume:
+        store.restore_checkpoint(resume, skip=skip)
+        if rank == 0:
+            print(f"restored {resume}: continuing from global_step {store.global_step}", flush=True)
+    num_steps = config.optimizer.get("num_train_steps", 10)
+    every = int(config.device.get("iterations_per_loop", 1000))
+
+    def save():
+        if rank == 0:
+            os.makedirs(output_dir, exist_ok=True)
+            prefix = os.path.join(output_dir, f"model.ckpt-{store.global_step}")
+            store.save_checkpoint(prefix, skip=skip)
+            update_checkpoint_state(output_dir, prefix)
+            print(f"saved {prefix}", flush=True)
+        if dist is not None:
+            dist.barrier()
+
     per_rank = max(1, config.device.get("train_batch_size", 8) // world)
     pipeline = None
     if make_batch is synthetic_batch and train_files(config.data):
-        pipeline = input_fn_builder(config, is_training=True, rank=rank, world=world, seed=0, batch_size=per_rank)
+        pipeline = input_fn_builder(config, is_training=True, rank=rank, world=world, seed=store.global_step if resume else 0,
+                                    batch_size=per_rank)
     elif rank == 0:
         print(f"data.train_file {config.data.get('train_file')!r} matches no file: training on synthetic batches"
               if make_batch is synthetic_batch else "VCR fine-tuning: training on synthetic batches", flush=True)
     try:
-        for step in range(config.optimizer.get("num_train_steps", 10)):
+        for step in range(store.global_step, num_steps):
             if pipeline is not None:
                 feats = next(pipeline)
             else:
@@ -278,6 +321,8 @@ def main(argv=None):
             spec.train_op()
             if step % 10 == 0 and rank == 0:
                 print(f"step {step} loss {spec.loss:.4f} lr {spec.metrics['learning_rate']:.3e}", flush=True)
+            if store.global_step % every == 0 or store.global_step == num_steps:
+                save()
     finally:
         if pipeline is not None:
             pipeline.close()
