@@ -61,6 +61,8 @@ void merlot_reset_launch_count(void);
  *   MUL_AUX (v *= aux[m,n], one multiply) instead of MUL_DGELU (v *= gelu_erf'(aux[m,n]), ~17 instructions per element in an
  *   epilogue that is issue-bound).
  *   ATOMIC: fp32 red.add into out (split-K wgrad accumulation; out must be pre-zeroed or hold the running sum).
+ *   GENERIC_EPILOGUE: run the general epilogue even where the register/TMA-store one applies (same results, bitwise for
+ *   bf16 outputs; for comparing the two).
  * ------------------------------------------------------------------------------------------------------------ */
 #define MERLOT_GEMM_OUT_F32 1u
 #define MERLOT_GEMM_ATOMIC 2u
@@ -69,6 +71,7 @@ void merlot_reset_launch_count(void);
 #define MERLOT_GEMM_DROPOUT 16u
 #define MERLOT_GEMM_GELU_GRAD_OUT 32u
 #define MERLOT_GEMM_MUL_AUX 64u
+#define MERLOT_GEMM_GENERIC_EPILOGUE 128u
 
 typedef struct merlot_gemm {
   int M, N, K;

@@ -32,6 +32,7 @@ GEMM_MUL_DGELU = 8
 GEMM_DROPOUT = 16
 GEMM_GELU_GRAD_OUT = 32
 GEMM_MUL_AUX = 64
+GEMM_GENERIC_EPILOGUE = 128
 
 MERLOT_FRAME_NO_AUGMENT = 0
 MERLOT_FRAME_BRIGHTNESS = 1

@@ -1,7 +1,8 @@
 // K1: persistent, warp-specialised bf16 GEMM for sm_90a (kernel in gemm_kernel.cuh).
 //   warp 0           : TMA producer (one elected lane) -- A/B tiles -> 128B-swizzled smem ring (full/empty mbarriers)
-//   warpgroups 1, 2  : wgmma 64 x BN x 16 each (fp32 accumulators in registers) -> fused epilogue -> vectorised global stores
-// Host side: argument checks, tile width, split-K, tensor maps.
+//   warpgroups 1, 2  : wgmma 64 x BN x 16 each (fp32 accumulators in registers) -> fused epilogue -> TMA stores (fast kinds)
+//                      or vectorised global stores (generic epilogue)
+// Host side: argument checks, tile width, split-K, epilogue kind, tensor maps.
 //
 // Replaces the reference's tf.layers.dense / tf.matmul call sites listed in include/merlot_b200.h (K1).
 #include "gemm_common.cuh"
@@ -38,8 +39,27 @@ void gemm_prof_after(void* tok, cudaStream_t stream) {
 
 namespace mb {
 template <int BN>
-int launch_gemm_bn(bool a_mn, bool b_mn, const CUtensorMap& ta, const CUtensorMap& tb, const GemmDev& p, int grid,
-                   cudaStream_t stream);  // gemm_bn{128,192,256}.cu
+int launch_gemm_bn(bool a_mn, bool b_mn, int kind, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to,
+                   const CUtensorMap& to2, const GemmDev& p, int grid, cudaStream_t stream);  // gemm_bn{128,192,256}.cu
+
+// The fast epilogue (EpiKind, gemm_common.cuh) for this launch, or EPI_GENERIC.  It needs alpha = 1, whole 8-column groups
+// (N % 8 == 0), a bias that float2 loads can read, and outputs TMA can address (16-byte base, 16-byte row pitch).  The
+// flag word seen here has DROPOUT cleared when p = 0.
+static int epilogue_kind(const merlot_gemm_t* g, uint32_t flags, int bn) {
+  if ((flags & (MERLOT_GEMM_GENERIC_EPILOGUE | MERLOT_GEMM_MUL_DGELU)) || g->alpha != 1.f || (g->N % 8) != 0 ||
+      ((uintptr_t)g->bias % 8) != 0)
+    return EPI_GENERIC;
+  if (flags & MERLOT_GEMM_OUT_F32) {
+    const bool red_only = (flags & MERLOT_GEMM_ATOMIC) && !(flags & ~(MERLOT_GEMM_OUT_F32 | MERLOT_GEMM_ATOMIC)) && !g->bias &&
+                          !g->resid;
+    return (red_only && bn == 256 && ((uintptr_t)g->out % 16) == 0 && (g->ld_out % 4) == 0) ? EPI_RED_F32 : EPI_GENERIC;
+  }
+  if (flags & MERLOT_GEMM_GELU)
+    return (g->out2 && !g->resid && !(flags & (MERLOT_GEMM_DROPOUT | MERLOT_GEMM_MUL_AUX))) ? EPI_GELU2 : EPI_GENERIC;
+  // Plain, bias, residual and dropout bf16 outputs stay generic: through per-warp TMA stores they measured slower (up to
+  // 1.7x on the joint encoder's N = 768 GEMMs), with no side input whose latency the fast path would hide.
+  return (flags == MERLOT_GEMM_MUL_AUX && !g->bias && !g->resid) ? EPI_MUL_AUX : EPI_GENERIC;
+}
 }
 
 using namespace mb;
@@ -143,9 +163,27 @@ extern "C" int merlot_gemm_bf16(const merlot_gemm_t* g, void* stream_) {
   const int grid = (int)(tiles < sms ? tiles : sms);
   if ((g->flags & MERLOT_GEMM_GELU) && g->out2 && !out_f32)
     MB_REQUIRE(((uintptr_t)g->out2 % 16) == 0, MERLOT_ESHAPE, "gemm: out2 must be 16-byte aligned");
-  if (bn == 256) return launch_gemm_bn<256>(g->a_mn_major != 0, g->b_mn_major != 0, ta, tb, p, grid, stream);
-  if (bn == 192) return launch_gemm_bn<192>(g->a_mn_major != 0, g->b_mn_major != 0, ta, tb, p, grid, stream);
-  return launch_gemm_bn<128>(g->a_mn_major != 0, g->b_mn_major != 0, ta, tb, p, grid, stream);
+
+  // fast epilogue: output tensor maps, one warp's [16 rows][128 B] sub-tile per box; TMA clips at M and N
+  const int kind = epilogue_kind(g, p.flags, bn);
+  CUtensorMap to, to2;
+  memset(&to, 0, sizeof(to));
+  memset(&to2, 0, sizeof(to2));
+  if (kind == EPI_RED_F32) {
+    rc = make_tmap_f32_2d(&to, g->out, (uint64_t)g->N, (uint64_t)g->M, (uint64_t)g->ld_out, 32, 16);
+    if (rc) return rc;
+  } else if (kind != EPI_GENERIC) {
+    rc = make_tmap_bf16_2d(&to, g->out, (uint64_t)g->N, (uint64_t)g->M, (uint64_t)g->ld_out, 64, 16);
+    if (rc) return rc;
+    if (kind == EPI_GELU2) {
+      rc = make_tmap_bf16_2d(&to2, g->out2, (uint64_t)g->N, (uint64_t)g->M, (uint64_t)g->ld_out2, 64, 16);
+      if (rc) return rc;
+    }
+  }
+  const bool a_mn = g->a_mn_major != 0, b_mn = g->b_mn_major != 0;
+  if (bn == 256) return launch_gemm_bn<256>(a_mn, b_mn, kind, ta, tb, to, to2, p, grid, stream);
+  if (bn == 192) return launch_gemm_bn<192>(a_mn, b_mn, kind, ta, tb, to, to2, p, grid, stream);
+  return launch_gemm_bn<128>(a_mn, b_mn, kind, ta, tb, to, to2, p, grid, stream);
 }
 
 extern "C" void merlot_gemm_profile_begin(void) {

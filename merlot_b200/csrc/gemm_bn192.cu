@@ -2,5 +2,6 @@
 #include "gemm_kernel.cuh"
 
 namespace mb {
-template int launch_gemm_bn<192>(bool, bool, const CUtensorMap&, const CUtensorMap&, const GemmDev&, int, cudaStream_t);
+template int launch_gemm_bn<192>(bool, bool, int, const CUtensorMap&, const CUtensorMap&, const CUtensorMap&, const CUtensorMap&,
+                                  const GemmDev&, int, cudaStream_t);
 }

@@ -10,7 +10,7 @@ constexpr int BLOCK_M = 128;  // two consumer warpgroups x 64 rows (one m64 wgmm
 constexpr int BLOCK_K = 64;   // 64 bf16 = 128 B = one swizzle atom
 constexpr int GEMM_THREADS = 384;  // warpgroup 0: TMA producer (one lane); warpgroups 1, 2: wgmma + epilogue
 constexpr int SMEM_LIMIT = 232448 - 1024 - 256;  // 227 KB minus alignment slack and barriers
-constexpr int STAGING_BYTES = 8 * 4096;          // 8 consumer warps x one [16 rows][64 fp32] epilogue slot
+constexpr int STAGING_BYTES = 8 * 4096;          // 8 consumer warps x one [16 rows][64 fp32] epilogue slot (fast kinds: 2 x 2 KB)
 
 struct GemmDev {
   int M, N, K;
@@ -162,6 +162,93 @@ __device__ __forceinline__ void epi_store_direct(const GemmDev& p, int row, int 
     store_bf16x8(reinterpret_cast<bf16*>(p.out2) + (size_t)row * p.ld_out2 + col, col, p.N, v);
   } else {
     store_bf16x8(reinterpret_cast<bf16*>(p.out) + (size_t)row * p.ld_out + col, col, p.N, v);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Fast epilogue: the math runs on the wgmma accumulator registers, results leave through a per-warp smem sub-tile and a TMA
+// store.  One kind per kernel instance, so each instance carries only its own path (gemm.cu picks the kind; everything
+// else runs the generic epilogue).
+//   EPI_MUL_AUX: bf16 out = acc * aux (the FFN2 dgrad times the saved GeLU')
+//   EPI_GELU2:   bf16 out = pre-activation or gelu'(pre), bf16 out2 = gelu(pre); pre = acc (+ bias)
+//   EPI_RED_F32: fp32 out += acc by TMA reduce-add (split-K wgrads)
+// Per warp: 16 rows x BN, processed in 16-column steps (8 accumulators per thread: at BN = 256 the 128 live accumulators
+// leave no room for more without spilling); two 2 KB [16 rows][128 B] 128B-swizzled staging buffers.
+// ---------------------------------------------------------------------------------------------------------------------
+enum EpiKind : int { EPI_GENERIC = 0, EPI_MUL_AUX = 1, EPI_GELU2 = 2, EPI_RED_F32 = 3 };
+constexpr int EPI_COLS = 16;
+
+// The side input (aux) of one 16-column step in accumulator layout: s[2j] / s[2j + 1] = bf16x2 at row row_a /
+// row_a + 8, columns col0 + 8j + 2q + {0, 1}.  Zero outside [M, N) (those results are clipped by the store).
+__device__ __forceinline__ void epi_load_side(const GemmDev& p, const bf16* side, int ld, int row_a, int col0, int q,
+                                              uint32_t (&s)[4]) {
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const int col = col0 + 8 * j;
+    const bf16* a = side + (size_t)row_a * ld + col + 2 * q;
+    s[2 * j] = (col < p.N && row_a < p.M) ? __ldg(reinterpret_cast<const unsigned int*>(a)) : 0u;
+    s[2 * j + 1] = (col < p.N && row_a + 8 < p.M) ? __ldg(reinterpret_cast<const unsigned int*>(a + (size_t)8 * ld)) : 0u;
+  }
+}
+
+// epi_math8's operations, in its order, on one step in accumulator layout: v[4j + 2s + e] is (row_a + 8s, col0 + 8j + 2q + e).
+template <int KIND>
+__device__ __forceinline__ void epi_math_frag(const GemmDev& p, int row_a, int col0, int lane, const uint32_t (&side)[4],
+                                              float (&v)[8], float (&pre)[8]) {
+  const int q = lane & 3;
+  if (p.bias != nullptr) {
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      if (col0 + 8 * j < p.N) {
+        const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 8 * j + 2 * q));
+        v[4 * j] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.x; v[4 * j + 3] += b.y;
+      }
+    }
+  }
+  if (KIND == EPI_GELU2) {
+    if (p.flags & MERLOT_GEMM_GELU_GRAD_OUT) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        float e;
+        const float cdf = normal_cdf_fast(v[i], &e);
+        pre[i] = fmaf(v[i] * 0.39894228040143267794f, e, cdf);
+        v[i] = v[i] * cdf;
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        pre[i] = v[i];
+        v[i] = gelu_erf_fast(v[i]);
+      }
+    }
+  }
+  if (KIND == EPI_MUL_AUX) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 f = unpack_bf16x2(side[j]);
+      v[2 * j] *= f.x; v[2 * j + 1] *= f.y;
+    }
+  }
+}
+
+// bf16 step h -> columns [16 (h % 4), 16 (h % 4) + 16) of a [16][64] 128B-swizzled sub-tile (one stmatrix.x4)
+__device__ __forceinline__ void epi_stage_bf16(uint32_t buf, int h, int lane, const float (&v)[8]) {
+  const int mi = lane >> 3;
+  const uint32_t row = (lane & 7) + 8 * (mi & 1);
+  stmatrix_x4(buf + sw128_offset(row, 2 * (h & 3) + (mi >> 1)), pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]),
+              pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
+}
+
+// fp32 step h -> columns [16 (h % 2), 16 (h % 2) + 16) of a [16][32] 128B-swizzled sub-tile
+__device__ __forceinline__ void epi_stage_f32(uint32_t buf, int h, int lane, const float (&v)[8]) {
+  const uint32_t r = lane >> 2, q = lane & 3;
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+      const uint32_t a = buf + sw128_offset(r + 8 * s, 4 * (h & 1) + 2 * j + (q >> 1)) + 8 * (q & 1);
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(v[4 * j + 2 * s]), "f"(v[4 * j + 2 * s + 1]) : "memory");
+    }
   }
 }
 

@@ -63,15 +63,15 @@ static PFN_encodeTiled get_encode() {
   return fn;
 }
 
-int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t outer, uint64_t ld_elems,
-                      uint32_t box_inner, uint32_t box_outer) {
+static int make_tmap_2d(CUtensorMap* out, CUtensorMapDataType dtype, uint64_t elem_bytes, const void* base, uint64_t inner,
+                        uint64_t outer, uint64_t ld_elems, uint32_t box_inner, uint32_t box_outer) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) return set_error(MERLOT_ECUDA, "cuTensorMapEncodeTiled entry point not available (no CUDA driver?)");
   cuuint64_t dims[2] = {inner, outer};
-  cuuint64_t strides[1] = {ld_elems * 2};
+  cuuint64_t strides[1] = {ld_elems * elem_bytes};
   cuuint32_t box[2] = {box_inner, box_outer};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
+  CUresult r = enc(out, dtype, 2, const_cast<void*>(base), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
@@ -80,6 +80,16 @@ int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64
                      (int)r, base, (unsigned long long)inner, (unsigned long long)outer, (unsigned long long)ld_elems,
                      box_inner, box_outer);
   return MERLOT_OK;
+}
+
+int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t outer, uint64_t ld_elems,
+                      uint32_t box_inner, uint32_t box_outer) {
+  return make_tmap_2d(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, inner, outer, ld_elems, box_inner, box_outer);
+}
+
+int make_tmap_f32_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t outer, uint64_t ld_elems,
+                     uint32_t box_inner, uint32_t box_outer) {
+  return make_tmap_2d(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, base, inner, outer, ld_elems, box_inner, box_outer);
 }
 
 int make_tmap_bf16_3d(CUtensorMap* out, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t ld1,

@@ -42,6 +42,9 @@ void count_launch(int n = 1);
 // 2-D bf16 tensor map, 128B swizzle, zero OOB fill. dims/box are {inner, outer}; ld = outer stride in elements.
 int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t outer, uint64_t ld_elems,
                       uint32_t box_inner, uint32_t box_outer);
+// the same for fp32 elements
+int make_tmap_f32_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t outer, uint64_t ld_elems,
+                     uint32_t box_inner, uint32_t box_outer);
 // 3-D bf16 tensor map (inner, mid, outer) with element strides ld_mid / ld_outer.
 int make_tmap_bf16_3d(CUtensorMap* out, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t ld1,
                       uint64_t ld2, uint32_t b0, uint32_t b1, uint32_t b2);

@@ -30,12 +30,13 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn_major: bool = False, b_mn_maj
          gelu: bool = False, out_pre: Optional[torch.Tensor] = None, dgelu_aux: Optional[torch.Tensor] = None,
          gelu_grad_out: bool = False, mul_aux: Optional[torch.Tensor] = None,
          alpha: float = 1.0, atomic: bool = False, dropout_p: float = 0.0, dropout_seed: int = 0,
-         dropout_site: int = 0, splits: int = 0, block_n: int = 0,
+         dropout_site: int = 0, splits: int = 0, block_n: int = 0, generic_epilogue: bool = False,
          M: Optional[int] = None, N: Optional[int] = None, K: Optional[int] = None) -> torch.Tensor:
     """C[M,N] = epilogue(alpha * A @ B^T) on wgmma tensor cores (see include/merlot_b200.h, K1).
 
     a: [M,K] (or [K,M] when a_mn_major); b: [N,K] (or [K,N] when b_mn_major); both bf16, row-major, 2-D.
     With gelu=True and out_pre given: out_pre <- pre-activation, return value <- gelu(pre).
+    generic_epilogue=True forces the general epilogue path (to compare it with the fast one).
     """
     _require_cuda(a, b, out, bias, resid, out_pre, dgelu_aux, mul_aux)
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16 and a.dim() == 2 and b.dim() == 2
@@ -87,6 +88,8 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn_major: bool = False, b_mn_maj
         g.resid, g.ld_resid = resid.data_ptr(), resid.stride(0)
     if dropout_p > 0.0:
         flags |= L.GEMM_DROPOUT
+    if generic_epilogue:
+        flags |= L.GEMM_GENERIC_EPILOGUE
     g.alpha = alpha
     g.flags = flags
     g.dropout_p, g.dropout_seed, g.dropout_site = dropout_p, dropout_seed, dropout_site

@@ -1,4 +1,6 @@
-"""Isolated timings of the ViT-size GEMMs WITH their real epilogues (bias / gelu dual / resid+dropout / dgelu)."""
+"""Isolated timings of the layer GEMMs WITH their real epilogues (bias / gelu dual / resid+dropout / dgelu), at the ViT row count
+(M = 8512) and the joint encoder's (M = 3168), plus the split-K wgrads and a K sweep of the FFN1 shape: the sweep's intercept
+at K = 0 estimates the fixed per-tile cost (epilogue, pipeline fill) that does not scale with K."""
 import sys
 
 import torch
@@ -8,7 +10,9 @@ from merlot_b200 import ops  # noqa: E402
 
 dev = "cuda"
 g = torch.Generator().manual_seed(0)
-M, H, I = 8512, 768, 3072
+M = int(sys.argv[1]) if len(sys.argv) > 1 else 8512
+H, I = 768, 3072
+print(f"M = {M}", flush=True)
 
 
 def t(name, fn, flops):
@@ -57,3 +61,18 @@ t("QKV-dgrad plain (N=768,K=2304)", lambda: ops.gemm(oqkv, wqkv, out=oh, M=M, N=
 for name, A, W, K_ in (("FFN1-dgrad K=3072", xi, w1, I), ("QKV-dgrad K=2304", oqkv, wqkv, 3 * H), ("out-proj dgrad K=768", x, wo, H)):
     for bn in (128, 192, 256):
         t(f"{name} block_n={bn}", lambda: ops.gemm(A, W, out=oh, M=M, N=H, K=K_, block_n=bn), 2.0 * M * H * K_)
+
+# wgrads (fp32 reduce-add into the gradient arena, automatic split-K)
+gw1 = torch.zeros(H, I, dtype=torch.float32, device=dev)
+gw2 = torch.zeros(I, H, dtype=torch.float32, device=dev)
+gwo = torch.zeros(H, H, dtype=torch.float32, device=dev)
+t("FFN1 wgrad (768 x 3072, K=M)", lambda: ops.gemm(x, oi, a_mn_major=True, b_mn_major=True, out=gw1, atomic=True, M=H, N=I, K=M), 2.0 * M * I * H)
+t("FFN2 wgrad (3072 x 768, K=M)", lambda: ops.gemm(xi, oh, a_mn_major=True, b_mn_major=True, out=gw2, atomic=True, M=I, N=H, K=M), 2.0 * M * I * H)
+t("out-proj wgrad (768 x 768, K=M)", lambda: ops.gemm(x, oh, a_mn_major=True, b_mn_major=True, out=gwo, atomic=True, M=H, N=H, K=M), 2.0 * M * H * H)
+
+# K sweep of FFN1 (N = 3072): time = fixed + K * slope; the fixed part is what the epilogue and the pipeline fill cost
+for name, kw in (("plain", dict()), ("+bias+gelu (gelu'+act)", dict(bias=b1, gelu=True, out_pre=oi2, gelu_grad_out=True))):
+    for K_ in (768, 1536, 3072):
+        xk = xi[:, :K_]
+        wk = (torch.randn(K_, I, generator=g) * 0.05).bfloat16().to(dev)
+        t(f"FFN1 {name} K={K_}", lambda: ops.gemm(xk, wk, b_mn_major=True, out=oi, **kw), 2.0 * M * I * K_)
