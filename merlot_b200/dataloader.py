@@ -27,11 +27,12 @@ from __future__ import annotations
 import collections
 import glob
 import io
+import itertools
 import math
 import queue
 import threading
 from concurrent.futures import ThreadPoolExecutor
-from typing import Dict, List, Optional, Sequence
+from typing import Dict, Iterator, List, Optional, Sequence
 
 import numpy as np
 import torch
@@ -230,15 +231,127 @@ def shard_files(files: Sequence[str], rank: int, world: int) -> List[str]:
     return list(files)
 
 
-class InputPipeline:
+def interleave_records(names: Iterator[str], cycle_length: int, files: Sequence[str], stop: Optional[threading.Event] = None):
+    """parallel_interleave(cycle_length, block_length=1) of TFRecord files: one record from each of `cycle_length` open files in
+    turn, a file that ends replaced by the next of `names`.  Ends when `names` (finite for evaluation) and every open file are
+    exhausted or `stop` is set; raises ValueError when no file of `files` yields a record."""
+    readers = collections.deque(read_records(n) for n in itertools.islice(names, cycle_length))
+    ended_in_a_row = 0
+    while readers and not (stop is not None and stop.is_set()):
+        r = readers.popleft()
+        try:
+            rec = next(r)
+        except StopIteration:
+            ended_in_a_row += 1
+            if ended_in_a_row > len(files) + cycle_length:
+                raise ValueError(f"no records in {list(files)}")
+            name = next(names, None)
+            if name is not None:
+                readers.append(read_records(name))
+            continue
+        ended_in_a_row = 0
+        readers.append(r)
+        yield rec
+
+
+def stage_frames(frames: Sequence[np.ndarray]):
+    """Packs decoded uint8 [h, w, 3] frames into one pinned host buffer for one copy to the device.  Returns (staging,
+    byte offset of every frame, [n, 2] heights and widths)."""
+    sizes = np.array([f.size for f in frames], dtype=np.int64)
+    offsets = np.concatenate([[0], np.cumsum(sizes)[:-1]])
+    staging = torch.empty(int(sizes.sum()), dtype=torch.uint8, pin_memory=True)
+    host = staging.numpy()
+    for f, o, s in zip(frames, offsets, sizes):
+        host[o:o + s] = f.reshape(-1)
+    return staging, offsets, np.array([f.shape[:2] for f in frames], dtype=np.int64)
+
+
+class DevicePipeline:
+    """Base of the input pipelines: a background thread runs `_produce()` -- a generator of (feature dict, info) whose device
+    work is enqueued on a data stream of its own -- with a pool of `num_threads` JPEG decoders at hand.  Up to `prefetch`
+    prepared batches wait in a queue, so batch k+1 is prepared while step k runs; the consumer's stream waits on the batch's
+    event (no host synchronisation).  Iteration stops when `_produce()` ends.  `close()` stops and joins the thread.
+    `last_info` holds the info behind the batch returned last (tests, debugging)."""
+
+    def __init__(self, device, num_threads: int, prefetch: int):
+        self.device = torch.device(device if device is not None else torch.cuda.current_device())
+        self.last_info = None
+        self._queue = queue.Queue(maxsize=prefetch)
+        self._stop = threading.Event()
+        self._pool = ThreadPoolExecutor(max_workers=num_threads, thread_name_prefix="merlot-jpeg")
+        self._stream = torch.cuda.Stream(self.device)
+        self._thread = threading.Thread(target=self._run, name="merlot-input", daemon=True)
+        self._thread.start()
+
+    def _produce(self):
+        raise NotImplementedError
+
+    def _run(self):
+        try:
+            with torch.cuda.device(self.device), torch.cuda.stream(self._stream):
+                for feats, info in self._produce():
+                    ev = torch.cuda.Event()
+                    ev.record(self._stream)
+                    if not self._put((feats, ev, info)):
+                        return
+                self._put(None)  # the end of a finite input
+        except BaseException as e:  # handed to the consumer, raised by __next__
+            self._put(e)
+
+    def _put(self, item) -> bool:
+        while not self._stop.is_set():
+            try:
+                self._queue.put(item, timeout=0.1)
+                return True
+            except queue.Full:
+                pass
+        return False
+
+    def __iter__(self):
+        return self
+
+    def __next__(self) -> Dict[str, torch.Tensor]:
+        if self._stop.is_set():
+            raise StopIteration
+        item = self._queue.get()
+        if item is None:
+            self._stop.set()
+            raise StopIteration
+        if isinstance(item, BaseException):
+            raise item
+        feats, ev, self.last_info = item
+        cur = torch.cuda.current_stream(self.device)
+        cur.wait_event(ev)
+        for t in feats.values():
+            if isinstance(t, torch.Tensor) and t.is_cuda:
+                t.record_stream(cur)  # the data stream's allocations stay alive until the consumer's use of them is done
+        return feats
+
+    def close(self):
+        self._stop.set()
+        while self._thread.is_alive():
+            try:
+                self._queue.get(timeout=0.1)
+            except queue.Empty:
+                pass
+        self._thread.join()
+        self._pool.shutdown(wait=True, cancel_futures=True)
+        self._stream.synchronize()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+
+class InputPipeline(DevicePipeline):
     """Iterator of training batches in the feature dict model_fn takes (images [b*n, H, W, 3] bf16, input_ids [b, n, L],
     video_src_ids, shuffled_idx_img, plus youtube_id, chunk_num, mean_time and is_eoc), on `device`.
 
-    A background thread reads and shuffles records, parses them and hands the JPEGs to a pool of `num_threads` decoders; it
-    packs a batch's frames into one pinned staging buffer, copies it to the device and runs K14 and `process_example` on a
-    data stream of its own.  Up to two prepared batches wait in a queue, so batch k+1 is prepared while step k runs; the
-    consumer's stream waits on the batch's event (no host synchronisation).  `close()` stops and joins the thread.
-    `last_info` holds the records and draws behind the batch returned last (tests, debugging)."""
+    The background thread (DevicePipeline) reads and shuffles records, parses them and hands the JPEGs to the decoder pool;
+    it packs a batch's frames into one pinned staging buffer, copies it to the device and runs K14 and `process_example` on
+    the data stream.  `last_info` holds the records and draws behind the batch returned last (tests, debugging)."""
 
     def __init__(self, config, files: Sequence[str], batch_size: int, rank: int = 0, seed: int = 0, device=None, prefetch: int = 2):
         self.data_cfg, self.model_cfg = dict(config.data), dict(config.model)
@@ -250,15 +363,8 @@ class InputPipeline:
         num_threads = self.data_cfg.get("num_threads", 64)
         self.cycle_length = min(num_threads, len(self.files))
         self.shuffle_buffer_size = self.data_cfg.get("shuffle_buffer_size", 256)
-        self.device = torch.device(device if device is not None else torch.cuda.current_device())
         self.rng = np.random.default_rng([seed, rank])
-        self.last_info = None
-        self._queue = queue.Queue(maxsize=prefetch)
-        self._stop = threading.Event()
-        self._pool = ThreadPoolExecutor(max_workers=num_threads, thread_name_prefix="merlot-jpeg")
-        self._stream = torch.cuda.Stream(self.device)
-        self._thread = threading.Thread(target=self._run, name="merlot-input", daemon=True)
-        self._thread.start()
+        super().__init__(device, num_threads, prefetch)
 
     # -- record stream: list_files -> repeat -> parallel_interleave(cycle_length) -> shuffle (:153-184) --
     def _file_names(self):
@@ -266,22 +372,7 @@ class InputPipeline:
             yield from (self.files[i] for i in self.rng.permutation(len(self.files)))
 
     def _records(self):
-        names = self._file_names()
-        readers = collections.deque(read_records(next(names)) for _ in range(self.cycle_length))
-        ended_in_a_row = 0
-        while not self._stop.is_set():
-            r = readers.popleft()
-            try:
-                rec = next(r)
-            except StopIteration:
-                ended_in_a_row += 1
-                if ended_in_a_row > len(self.files) + self.cycle_length:
-                    raise ValueError(f"no records in {self.files}")
-                readers.append(read_records(next(names)))
-                continue
-            ended_in_a_row = 0
-            readers.append(r)
-            yield rec
+        return interleave_records(self._file_names(), self.cycle_length, self.files, self._stop)
 
     def _shuffled(self):
         buf, size = [], self.shuffle_buffer_size
@@ -304,14 +395,7 @@ class InputPipeline:
         text = [parse_text(ex, n, self.chunk_text_len, bool(c)) for ex, c in zip(examples, do_clean)]
         draws = frame_draws(self.rng, b * n, self.data_cfg)
         process_seed = int(self.rng.integers(1 << 62))
-        frames = [d.result() for d in decodes]
-        sizes = np.array([f.size for f in frames], dtype=np.int64)
-        offsets = np.concatenate([[0], np.cumsum(sizes)[:-1]])
-        staging = torch.empty(int(sizes.sum()), dtype=torch.uint8, pin_memory=True)
-        host = staging.numpy()
-        for f, o, s in zip(frames, offsets, sizes):
-            host[o:o + s] = f.reshape(-1)
-        hw = np.array([f.shape[:2] for f in frames], dtype=np.int64)
+        staging, offsets, hw = stage_frames([d.result() for d in decodes])
         plan = plan_frames(hw[:, 0], hw[:, 1], self.out_size, draws["scale"], draws["u_y"], draws["u_x"])
         plan.update(src_offset=offsets, src_h=hw[:, 0], src_w=hw[:, 1], method=draws["method"], augment=draws["augment"],
                     factor=draws["factor"])
@@ -329,61 +413,10 @@ class InputPipeline:
                 "process_draws": {k: v.cpu() for k, v in pdraws.items()}}
         return feats, info
 
-    def _run(self):
-        try:
-            with torch.cuda.device(self.device), torch.cuda.stream(self._stream):
-                recs = self._shuffled()
-                while not self._stop.is_set():
-                    records = [next(recs) for _ in range(self.batch_size)]  # batch(drop_remainder=True) of a repeated stream
-                    feats, info = self._batch(records)
-                    ev = torch.cuda.Event()
-                    ev.record(self._stream)
-                    if not self._put((feats, ev, info)):
-                        return
-        except BaseException as e:  # handed to the consumer, raised by __next__
-            self._put(e)
-
-    def _put(self, item) -> bool:
+    def _produce(self):
+        recs = self._shuffled()
         while not self._stop.is_set():
-            try:
-                self._queue.put(item, timeout=0.1)
-                return True
-            except queue.Full:
-                pass
-        return False
-
-    def __iter__(self):
-        return self
-
-    def __next__(self) -> Dict[str, torch.Tensor]:
-        if self._stop.is_set():
-            raise StopIteration
-        item = self._queue.get()
-        if isinstance(item, BaseException):
-            raise item
-        feats, ev, self.last_info = item
-        cur = torch.cuda.current_stream(self.device)
-        cur.wait_event(ev)
-        for t in feats.values():
-            t.record_stream(cur)  # the data stream's allocations stay alive until the consumer's use of them is done
-        return feats
-
-    def close(self):
-        self._stop.set()
-        while self._thread.is_alive():
-            try:
-                self._queue.get(timeout=0.1)
-            except queue.Empty:
-                pass
-        self._thread.join()
-        self._pool.shutdown(wait=True, cancel_futures=True)
-        self._stream.synchronize()
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
+            yield self._batch([next(recs) for _ in range(self.batch_size)])  # batch(drop_remainder=True) of a repeated stream
 
 
 def input_fn_builder(config, is_training: bool = True, rank: int = 0, world: int = 1, seed: int = 0,

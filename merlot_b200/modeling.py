@@ -145,9 +145,21 @@ class MerlotModel(object):
     def __init__(self, config, is_training, use_tpu, image, input_ids, mask_input=False, shuffled_idx_img=None,
                  img_mask=None, log_attention_probs=True, *, params: ParamStore, mask_draws: Optional[Dict] = None,
                  mask_override: Optional[Dict] = None, dropout_seed: int = 0, save_for_backward: Optional[bool] = None,
-                 dist=None, export_attention_probs: bool = False):
+                 dist=None, export_attention_probs: bool = False, frame_copies: int = 1):
         """Arguments as model/modeling.py:48-66.  `use_tpu` is accepted and ignored (it only selects one-hot vs gather
-        embedding lookups in the reference, utils/model_utils.py:259-263 -- same values either way)."""
+        embedding lookups in the reference, utils/model_utils.py:259-263 -- same values either way).
+
+        `frame_copies` = c > 1 is the evaluation forward of c copies of every group that share their frames (zero-shot story
+        unshuffling scores two shuffles of each story, downstream/sort_story/get_zero_shot_logits.py:44-56): `image` holds
+        batch_size // c groups of frames, `input_ids` and `shuffled_idx_img` hold batch_size groups, copy d of group s at
+        s*c + d.  The ViT runs once per group of frames; each copy assembles its own viz tokens with its own image indices."""
+        frame_copies = int(frame_copies)
+        if frame_copies < 1:
+            raise ValueError(f"frame_copies must be >= 1, got {frame_copies}")
+        if frame_copies > 1 and (is_training or mask_input or save_for_backward or config.get("num_texts", 1) > 1):
+            raise NotImplementedError("frame_copies > 1 is an evaluation forward: it is not combined with training, "
+                                      "save_for_backward, mask_input or num_texts > 1")
+        self.frame_copies = frame_copies
         self.config = copy.deepcopy(config)
         self.is_training = is_training
         self.use_tpu = use_tpu
@@ -245,9 +257,10 @@ class MerlotModel(object):
         assert w0 % Pp == 0  # :190
         if c3 != 3:
             raise ValueError(f"image must be [N,h,w,3], got {tuple(image.shape)}")
-        nt = self.num_texts
-        if N * nt != self.batch_size * self.num_chunks:
-            raise ValueError(f"image batch {N} x num_texts {nt} != batch_size*num_chunks {self.batch_size * self.num_chunks}")
+        nt, nc = self.num_texts, self.frame_copies
+        if N * nt * nc != self.batch_size * self.num_chunks:
+            raise ValueError(f"image batch {N} x num_texts {nt} x frame_copies {nc} != batch_size*num_chunks "
+                             f"{self.batch_size * self.num_chunks}")
         ncls = cfg.get("num_cls_emb", 2)
         h1, w1 = h0 // Pp, w0 // Pp
         np_ = h1 * w1
@@ -303,24 +316,27 @@ class MerlotModel(object):
         # ---- viz tokens (:95-133) ----
         if shuffled_idx_img is None:
             img_idx = bf.get("img_idx.arange", (N,), torch.int32)
-            img_idx.copy_(torch.arange(ncg, dtype=torch.int32, device=dev).repeat(B // nt))
+            img_idx.copy_(torch.arange(ncg, dtype=torch.int32, device=dev).repeat(B // (nt * nc)))
             self._shuffled = None
         else:
             assert self.num_imgs == 1 and self.num_texts == 1  # :319-320
             img_idx = shuffled_idx_img.reshape(-1).to(torch.int32).contiguous()
-            if img_idx.numel() != N:
-                raise ValueError(f"shuffled_idx_img has {img_idx.numel()} entries, expected B*num_chunks_in_group = {N}")
+            if img_idx.numel() != N * nc:
+                raise ValueError(f"shuffled_idx_img has {img_idx.numel()} entries, expected B*num_chunks_in_group = {N * nc}")
         self._img_idx = img_idx
-        Bi = B // nt  # image groups; with num_texts > 1 every group's tokens are tiled to its nt texts (model/modeling.py:111-119)
+        Bi = B // (nt * nc)  # image groups; with num_texts > 1 every group's tokens are tiled to its nt texts (model/modeling.py:111-119)
         xsum_z = bf.get("viz.xsum", (Bi * Pz, H), torch.float32)
         self.img_trg_h = bf.get("viz.img_trg", (N, H), torch.float32)
-        ops.viz_assemble_fwd(hv, st.P("vision_backbone/img_idx_pe"), img_idx, st.P("vision_backbone/final_pe/pos_embs"),
-                             st.P("vision_backbone/final_pe/cls_emb"), xsum_z, self.img_trg_h, N, h1, w1, ncls, max(sp, 1), H)
         joint_in = bf.get("joint.in", (B * Sj, H), torch.bfloat16)
         mean_z, rstd_z = bf.get("viz.mean", (Bi * Pz,), torch.float32), bf.get("viz.rstd", (Bi * Pz,), torch.float32)
-        for j in range(nt):  # image group g feeds joint rows of texts g*nt + j: row remap (group stride nt*Sj, offset j*Sj)
-            ops.layernorm_fwd(xsum_z, joint_in, st.P("vision_backbone/LayerNorm_final_ln/gamma"),
-                              st.P("vision_backbone/LayerNorm_final_ln/beta"), mean_z, rstd_z, rows=Bi * Pz, remap=(Pz, nt * Sj, j * Sj))
+        for d in range(nc):  # copy d of image group g: its own image indices, joint rows of group g*nc + d
+            idx_d = img_idx if img_idx.numel() == N else img_idx.view(Bi, nc, ncg)[:, d].contiguous()
+            ops.viz_assemble_fwd(hv, st.P("vision_backbone/img_idx_pe"), idx_d, st.P("vision_backbone/final_pe/pos_embs"),
+                                 st.P("vision_backbone/final_pe/cls_emb"), xsum_z, self.img_trg_h, N, h1, w1, ncls, max(sp, 1), H)
+            for j in range(nt):  # image group g feeds joint rows of texts g*nt + j: row remap (group stride nt*Sj, offset j*Sj)
+                ops.layernorm_fwd(xsum_z, joint_in, st.P("vision_backbone/LayerNorm_final_ln/gamma"),
+                                  st.P("vision_backbone/LayerNorm_final_ln/beta"), mean_z, rstd_z, rows=Bi * Pz,
+                                  remap=(Pz, nt * nc * Sj, (d * nt + j) * Sj))
 
         # ---- language-only encoder + masking (:135-139) ----
         ids_bl = self.input_ids.reshape(B, Lj)
