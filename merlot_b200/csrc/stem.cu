@@ -11,7 +11,7 @@
 //                     out, optional ReLU, optional `relu(out + shortcut)` (bottleneck_block :96)
 //   avgpool2          tf.nn.avg_pool2d(ksize 2, strides 2, SAME) (:81,93,159): bottom/right padding not counted
 // The second half of the file holds the gradient of the same pieces (GroupNorm/ReLU/shortcut, avg-pool, col2im, weight
-// standardisation); MerlotModel._hybrid_stem_backward walks the forward tape and calls them.
+// standardisation); HybridStem.backward (stem.py) walks the forward tape and calls them.
 #include "host_common.h"
 #include "ptx.cuh"
 

@@ -24,6 +24,7 @@ import torch
 from . import _lib as L
 from . import ops
 from .params import ParamStore
+from .stem import HybridStem
 
 MASK = 1  # utils/encode/encoder.py:16-22
 PADDING = 0
@@ -61,6 +62,23 @@ class _Buffers:
         elif zero:
             t.zero_()
         return t
+
+
+class _LayerNorm:
+    """LayerNorm `scope` of the rows of x into y (ops.layernorm_fwd), keeping the input and statistics its backward reads.
+    Keyword arguments of forward / backward override the ones given here (rows, remap, dropout)."""
+
+    def __init__(self, store, scope, x, mean, rstd, **kw):
+        self.st, self.scope, self.x, self.mean, self.rstd, self.kw = store, scope, x, mean, rstd, kw
+
+    def forward(self, y, **kw):
+        st, s = self.st, self.scope
+        return ops.layernorm_fwd(self.x, y, st.P(f"{s}/gamma"), st.P(f"{s}/beta"), self.mean, self.rstd, **{**self.kw, **kw})
+
+    def backward(self, dy, dx, **kw):
+        st, s = self.st, self.scope
+        return ops.layernorm_bwd(dy, self.x, self.mean, self.rstd, st.P(f"{s}/gamma"), dx, st.G(f"{s}/gamma"), st.G(f"{s}/beta"),
+                                 **{**self.kw, **kw})
 
 
 def _layer_params(store: ParamStore, scope: str, layers: int):
@@ -291,24 +309,26 @@ class MerlotModel(object):
         img = image if image.dtype == torch.bfloat16 else image.to(torch.bfloat16)
         img = img.contiguous()
         patch = bf.get("vit.patch", (N * np_, H), torch.float32)
+        self._stem = self.d_rc = None  # d_rc: the gradient backward() hands to the hybrid stem
         if not self._resnet_layers:
-            A = bf.get("vit.A", (N * np_, Pp * Pp * 3), torch.bfloat16)
-            ops.patch_im2col(img, A, Pp)
-            ops.gemm(A, st.W(f"{vt}/conv2d/kernel"), b_mn_major=True, bias=st.P(f"{vt}/conv2d/bias"), out=patch)
+            self._patch_A = bf.get("vit.A", (N * np_, Pp * Pp * 3), torch.bfloat16)
+            ops.patch_im2col(img, self._patch_A, Pp)
+            ops.gemm(self._patch_A, st.W(f"{vt}/conv2d/kernel"), b_mn_major=True, bias=st.P(f"{vt}/conv2d/bias"), out=patch)
         else:  # hybrid stem (:206-223): lite_resnet50 -> 1x1 conv_postresnet_proj with bias (not standardised)
             if Pp != 16:
                 raise ValueError("the hybrid ResNet stem needs patch_size 16 (utils/vision_transformer.py:208)")
-            rc, hs, ws_ = self._hybrid_stem(img, N, h0, w0)
+            self._stem = HybridStem(st, bf, self._resnet_layers, self._save)
+            self._rc, hs, ws_ = self._stem.forward(img, N, h0, w0)
             if (hs, ws_) != (h1, w1):
                 raise ValueError(f"stem output {hs}x{ws_} != patch grid {h1}x{w1}")
-            ops.gemm(rc, st.W(f"{vt}/conv_postresnet_proj/kernel"), b_mn_major=True, bias=st.P(f"{vt}/conv_postresnet_proj/bias"),
-                     out=patch)
+            ops.gemm(self._rc, st.W(f"{vt}/conv_postresnet_proj/kernel"), b_mn_major=True,
+                     bias=st.P(f"{vt}/conv_postresnet_proj/bias"), out=patch)
         xsum_v = bf.get("vit.xsum", (Mv, H), torch.float32)
         ops.vit_assemble_fwd(patch, st.P(f"{vt}/pos_embs/pos_embs"), st.P(f"{vt}/pos_embs/cls_emb"), xsum_v, N, h1, w1, ncls, H)
         h0_v = bf.get("vit.h0", (Mv, H), torch.bfloat16)
-        mean_v, rstd_v = bf.get("vit.mean0", (Mv,), torch.float32), bf.get("vit.rstd0", (Mv,), torch.float32)
-        ops.layernorm_fwd(xsum_v, h0_v, st.P(f"{vt}/LayerNorm_ctx_patches_pre_ln/gamma"),
-                          st.P(f"{vt}/LayerNorm_ctx_patches_pre_ln/beta"), mean_v, rstd_v)
+        self._vit_ln = _LayerNorm(st, f"{vt}/LayerNorm_ctx_patches_pre_ln", xsum_v, bf.get("vit.mean0", (Mv,), torch.float32),
+                                  bf.get("vit.rstd0", (Mv,), torch.float32))
+        self._vit_ln.forward(h0_v)
         self._vit = _Stack(st, bf, "vit", vt, cfg.get("num_vision_transformer_hidden_layers", cfg["num_hidden_layers"]), N, Sv,
                            None, h0_v, cfg, p_vit, self._seed, _SITE_VIT, self._save)
         hv = self._vit.forward()
@@ -328,15 +348,14 @@ class MerlotModel(object):
         xsum_z = bf.get("viz.xsum", (Bi * Pz, H), torch.float32)
         self.img_trg_h = bf.get("viz.img_trg", (N, H), torch.float32)
         joint_in = bf.get("joint.in", (B * Sj, H), torch.bfloat16)
-        mean_z, rstd_z = bf.get("viz.mean", (Bi * Pz,), torch.float32), bf.get("viz.rstd", (Bi * Pz,), torch.float32)
+        self._viz_ln = _LayerNorm(st, "vision_backbone/LayerNorm_final_ln", xsum_z, bf.get("viz.mean", (Bi * Pz,), torch.float32),
+                                  bf.get("viz.rstd", (Bi * Pz,), torch.float32), rows=Bi * Pz)
         for d in range(nc):  # copy d of image group g: its own image indices, joint rows of group g*nc + d
             idx_d = img_idx if img_idx.numel() == N else img_idx.view(Bi, nc, ncg)[:, d].contiguous()
             ops.viz_assemble_fwd(hv, st.P("vision_backbone/img_idx_pe"), idx_d, st.P("vision_backbone/final_pe/pos_embs"),
                                  st.P("vision_backbone/final_pe/cls_emb"), xsum_z, self.img_trg_h, N, h1, w1, ncls, max(sp, 1), H)
             for j in range(nt):  # image group g feeds joint rows of texts g*nt + j: row remap (group stride nt*Sj, offset j*Sj)
-                ops.layernorm_fwd(xsum_z, joint_in, st.P("vision_backbone/LayerNorm_final_ln/gamma"),
-                                  st.P("vision_backbone/LayerNorm_final_ln/beta"), mean_z, rstd_z, rows=Bi * Pz,
-                                  remap=(Pz, nt * nc * Sj, (d * nt + j) * Sj))
+                self._viz_ln.forward(joint_in, remap=(Pz, nt * nc * Sj, (d * nt + j) * Sj))
 
         # ---- language-only encoder + masking (:135-139) ----
         ids_bl = self.input_ids.reshape(B, Lj)
@@ -353,7 +372,7 @@ class MerlotModel(object):
         self._ids_j = ids_to_use.contiguous()
 
         # ---- joint encoder (:143-184) ----
-        self._embed_words_into(self._ids_j, "position_embeddings", "emb_j", _SITE_EMB_J, joint_in, remap=(Lj, Sj, Pz))
+        self._emb_j_ln = self._embed_words_into(self._ids_j, "position_embeddings", "emb_j", _SITE_EMB_J, joint_in, remap=(Lj, Sj, Pz))
         valid_j = bf.get("joint.valid", (B * Sj,), torch.uint8)
         ops.joint_valid(self._ids_j, valid_j, B, Pz, Lj)
         c_viz = c_lang = None
@@ -382,188 +401,6 @@ class MerlotModel(object):
         self.encoder_pieces = [{"name": "viz", "start": 0, "end": Pz}, {"name": "lang", "start": Pz, "end": Sj}]
         self._heads = {}
 
-    def _hybrid_stem(self, img, N, h0, w0):
-        """lite_resnet50 (utils/vision_transformer.py:118-170): NHWC bf16 activations as [N*h*w, C] matrices, every conv a K1 GEMM
-        on weight-standardised bf16 kernels (1x1: the activation matrix itself; 3x3: an im2col matrix), GroupNorm32 (+ReLU /
-        +shortcut) and the avg-pool striding as K13 kernels (csrc/stem.cu).  Variables are consumed in the reference's creation
-        order (params.stem_variables).  With save_for_backward every op keeps its own buffers and is recorded on a tape for
-        _hybrid_stem_backward.  Returns ([N*h*w, 4*f_last] bf16, h, w)."""
-        st, bf = self.store, self._bufs
-        vt = "vision_backbone/vision_transformer"
-        save = bool(getattr(self, "_save", False))
-        tape = []
-        site = [0]
-
-        class _Names:  # tf default-name uniquification inside one variable scope
-            def __init__(self, scope):
-                self.scope, self.nc, self.ng = scope, 0, 0
-
-            def conv(self):
-                n = f"{self.scope}/conv2d{'' if self.nc == 0 else '_%d' % self.nc}/kernel"
-                self.nc += 1
-                return n
-
-            def gn(self, name=None):
-                if name is not None:
-                    return f"{self.scope}/GroupNorm_{name}"
-                n = f"{self.scope}/GroupNorm{'' if self.ng == 0 else '_%d' % self.ng}"
-                self.ng += 1
-                return n
-
-        def T(tag, rows, cols):  # training: one buffer per op (the backward pass reads them); inference: reuse by tag and shape
-            site[0] += 1
-            return bf.get(f"stem.{tag}.{site[0]}" if save else f"stem.{tag}", (rows, cols), torch.bfloat16)
-
-        plan = self._ws_plan()
-        plan.standardise()  # :56-60 (fp32 moments, bf16 operand) for every conv kernel of the stem in one launch
-
-        def conv(x, h, w, cin, kname, k, tag, stride=1, sub_half=False):
-            wk = st.P(kname)  # fp32 [k*k*cin, cout]
-            rows, cout = wk.shape
-            assert rows == k * k * cin, (kname, rows, k, cin)
-            kp = (rows + 7) // 8 * 8
-            wstd = plan.wstd[kname]
-            if k == 1:
-                a, ho, wo = x, h, w
-            else:
-                ho, wo = (h + 2 - 3) // stride + 1, (w + 2 - 3) // stride + 1
-                a = bf.get("stem.col", (N * ho * wo, kp), torch.bfloat16)  # recomputed in the backward pass: never per-op
-                ops.im2col3x3(x, N, h, w, cin, stride, a, sub_half=sub_half)
-            y = T(tag, N * ho * wo, cout)
-            ops.gemm(a, wstd, b_mn_major=True, out=y)
-            tape.append(("conv", dict(x=x, h=h, w=w, cin=cin, kname=kname, k=k, stride=stride, sub_half=sub_half, y=y, ho=ho, wo=wo,
-                                      cout=cout, kp=kp)))
-            return y, ho, wo, cout
-
-        def gn(x, hw, c, scope_name, tag, relu=True, shortcut=None):
-            y = T(tag, N * hw, c)
-            stats = bf.get(f"stem.gn_stats.{site[0]}" if save else "stem.gn_stats", (N * 64,), torch.float32)
-            ops.group_norm_fwd(x, st.P(f"{scope_name}/gamma"), st.P(f"{scope_name}/beta"), y, stats, N, hw, c, 32, 1e-4, relu, shortcut)
-            tape.append(("gn", dict(x=x, y=y, scope=scope_name, hw=hw, c=c, relu=relu, shortcut=shortcut, stats=stats)))
-            return y
-
-        def pool(x, h, w, c, tag):
-            ho, wo = (h + 1) // 2, (w + 1) // 2
-            y = T(tag, N * ho * wo, c)
-            ops.avgpool2_same(x, N, h, w, c, y)
-            tape.append(("pool", dict(x=x, h=h, w=w, c=c, y=y)))
-            return y, ho, wo
-
-        nm = _Names(f"{vt}/resnet50lite/stem")
-        x, h, w, c = conv(img, h0, w0, 3, nm.conv(), 3, "s0", stride=2, sub_half=True)  # :138-144 on image - 0.5 (:193)
-        x = gn(x, h * w, c, nm.gn("stem0"), "s0g")
-        x, h, w, c = conv(x, h, w, c, nm.conv(), 3, "s1")
-        x = gn(x, h * w, c, nm.gn("stem1"), "s1g")
-        x, h, w, c = conv(x, h, w, c, nm.conv(), 3, "s2")
-        x = gn(x, h * w, c, nm.gn("stem2"), "s2g")
-        x, h, w = pool(x, h, w, c, "s2p")  # :159
-        for i, blocks in enumerate(self._resnet_layers):
-            nm = _Names(f"{vt}/resnet50lite/block_group{i + 1}")
-            f = 64 * (2 ** i)
-            for b in range(blocks):  # bottleneck_block (:69-96); only the first block of a group projects and strides (:109-113)
-                stride = 2 if (b == 0 and i > 0) else 1
-                shortcut = x
-                if b == 0:
-                    sx, sh, sw = pool(x, h, w, c, f"g{i}sp") if stride > 1 else (x, h, w)
-                    sy, _, _, c4 = conv(sx, sh, sw, c, nm.conv(), 1, f"g{i}sc")
-                    shortcut = gn(sy, sh * sw, c4, nm.gn(), f"g{i}scg", relu=False)
-                y, _, _, c1 = conv(x, h, w, c, nm.conv(), 1, f"g{i}a")
-                y = gn(y, h * w, c1, nm.gn(), f"g{i}ag")
-                y, _, _, c2 = conv(y, h, w, c1, nm.conv(), 3, f"g{i}b")
-                y = gn(y, h * w, c2, nm.gn(), f"g{i}bg")
-                hh, ww = h, w
-                if stride > 1:
-                    y, hh, ww = pool(y, h, w, c2, f"g{i}bp")
-                y, _, _, c3 = conv(y, hh, ww, c2, nm.conv(), 1, f"g{i}c")
-                x = gn(y, hh * ww, c3, nm.gn(), f"g{i}out{b % 2}", relu=True, shortcut=shortcut)  # relu(GN(y) + shortcut) (:95-96)
-                h, w, c = hh, ww, c3
-                assert c3 == 4 * f
-        self._stem_tape = tape if save else None
-        return x, h, w
-
-    def _ws_plan(self):
-        """The stem's conv kernels as one table (ops.WsPlan), cached on the store (the arenas' addresses never change)."""
-        st = self.store
-        names = [n for n in st.entries if "resnet50lite" in n and n.endswith("/kernel")]
-        key = tuple(st.P(n).data_ptr() for n in names)
-        plan = getattr(st, "_ws_plan_cache", None)
-        if plan is None or plan.key != key:
-            plan = ops.WsPlan({n: st.P(n) for n in names}, {n: st.G(n) for n in names}, st.device)
-            st._ws_plan_cache = plan
-        return plan
-
-    def _hybrid_stem_backward(self, d_out, N):
-        """Gradient of _hybrid_stem: walks the tape backwards.  d_out: bf16 gradient of the stem output.  Parameter gradients are
-        ACCUMULATED into the arena (conv kernels through the weight-standardisation backward, GroupNorm gamma/beta directly);
-        activation gradients meet by tensor identity (a block input feeds the first 1x1 and the shortcut)."""
-        st, bf = self.store, self._bufs
-        tape = self._stem_tape
-        trace = getattr(self, "_stem_trace", None)  # tests set this to a list: every op's (dy, dx, d_shortcut) is recorded
-        grads = {tape[-1][1]["y"].data_ptr(): d_out}
-        red = bf.get("stem.gn_red", (N * 64,), torch.float32)
-        ctr = [0]
-        plan = self._ws_plan()  # holds the forward's standardised operands; the wgrad GEMMs accumulate into its gradient arena
-        plan.zero_grads()
-
-        def D(rows, cols):
-            ctr[0] += 1
-            return bf.get(f"stem.d.{ctr[0]}", (rows, cols), torch.bfloat16)
-
-        def acc(t, g):
-            k = t.data_ptr()
-            if k in grads:
-                ops.add_bf16(grads[k], g, grads[k])
-            else:
-                grads[k] = g
-
-        for kind, r in reversed(tape):
-            dy = grads.pop(r["y"].data_ptr(), None)
-            if dy is None:
-                continue
-            if kind == "gn":
-                dx = D(*r["x"].shape)
-                dsc = D(*r["y"].shape) if r["shortcut"] is not None else None
-                ops.group_norm_bwd(dy, r["x"], r["y"] if r["relu"] else None, r["stats"], st.P(f"{r['scope']}/gamma"), dx, dsc,
-                                   st.G(f"{r['scope']}/gamma"), st.G(f"{r['scope']}/beta"), red, N, r["hw"], r["c"], 32, 1e-4, r["relu"])
-                if trace is not None:
-                    trace.append(dict(kind=kind, r=r, dy=dy.clone(), dx=dx.clone(), dsc=None if dsc is None else dsc.clone()))
-                acc(r["x"], dx)
-                if dsc is not None:
-                    acc(r["shortcut"], dsc)
-            elif kind == "pool":
-                dx = D(*r["x"].shape)
-                ops.avgpool2_same_bwd(dy, N, r["h"], r["w"], r["c"], dx)
-                if trace is not None:
-                    trace.append(dict(kind=kind, r=r, dy=dy.clone(), dx=dx.clone()))
-                acc(r["x"], dx)
-            else:  # conv
-                wk = st.P(r["kname"])
-                kp, cout, M = r["kp"], r["cout"], N * r["ho"] * r["wo"]
-                if r["k"] == 1:
-                    a = r["x"]
-                else:
-                    a = bf.get("stem.col", (M, kp), torch.bfloat16)
-                    ops.im2col3x3(r["x"], N, r["h"], r["w"], r["cin"], r["stride"], a, sub_half=r["sub_half"])
-                dws = plan.dws[r["kname"]]
-                ops.gemm(a, dy, a_mn_major=True, b_mn_major=True, out=dws, atomic=True, M=kp, N=cout, K=M)  # d(standardised kernel)
-                if r["sub_half"]:
-                    if trace is not None:
-                        trace.append(dict(kind=kind, r=r, dy=dy.clone(), dx=None))
-                    continue  # the image itself needs no gradient
-                wstd = plan.wstd[r["kname"]]
-                if r["k"] == 1:
-                    dx = D(M, kp)
-                    ops.gemm(dy, wstd, out=dx)  # dx[M, cin] = dy[M, cout] . wstd[cin, cout]^T
-                else:
-                    dcol = bf.get("stem.dcol", (M, kp), torch.bfloat16)
-                    ops.gemm(dy, wstd, out=dcol)
-                    dx = D(N * r["h"] * r["w"], r["cin"])
-                    ops.col2im3x3(dcol, N, r["h"], r["w"], r["cin"], r["stride"], dx)
-                if trace is not None:
-                    trace.append(dict(kind=kind, r=r, dy=dy.clone(), dx=dx.clone()))
-                acc(r["x"], dx)
-        plan.backward()  # weight-standardisation backward of every conv kernel: arena gradients += d(standardise)/dw . dws
-
     def _side_stream(self):
         """Stream for the language-only stack (set MERLOT_NO_SIDE_STREAM=1 to serialise everything on one stream)."""
         st = self.store
@@ -575,7 +412,8 @@ class MerlotModel(object):
 
     # ---------------------------------------------------------------------------------------------------------
     def _embed_words_into(self, ids_2d, norm_scope_name, tag, site, out, remap):
-        """embed_words (:262-297): E[ids] + Pos[0:L] -> LN embed_norm -> dropout -> bf16, written into `out` rows."""
+        """embed_words (:262-297): E[ids] + Pos[0:L] -> LN embed_norm -> dropout -> bf16, written into `out` rows.  Returns the
+        embed_norm, for _embed_bwd."""
         st, bf, cfg = self.store, self._bufs, self.config
         H = self.hidden_size
         R, Lseq = ids_2d.numel(), ids_2d.shape[1]
@@ -583,12 +421,11 @@ class MerlotModel(object):
             raise ValueError(f"sequence length {Lseq} exceeds max_position_embeddings {cfg['max_position_embeddings']}")
         xsum = bf.get(f"{tag}.xsum", (R, H), torch.float32)
         ops.embed_fwd(ids_2d, st.P("word_embeddings/word_embeddings"), st.P(f"{norm_scope_name}/position_embeddings"), xsum, Lseq)
-        mean, rstd = bf.get(f"{tag}.mean", (R,), torch.float32), bf.get(f"{tag}.rstd", (R,), torch.float32)
         p = float(self.dropout_prob or 0.0) if self.is_training else 0.0
-        ops.layernorm_fwd(xsum, out, st.P(f"{norm_scope_name}/LayerNorm_embed_norm/gamma"),
-                          st.P(f"{norm_scope_name}/LayerNorm_embed_norm/beta"), mean, rstd, rows=R, remap=remap,
-                          dropout=(p, self._seed, site))
-        return xsum, mean, rstd
+        ln = _LayerNorm(st, f"{norm_scope_name}/LayerNorm_embed_norm", xsum, bf.get(f"{tag}.mean", (R,), torch.float32),
+                        bf.get(f"{tag}.rstd", (R,), torch.float32), rows=R, remap=remap, dropout=(p, self._seed, site))
+        ln.forward(out)
+        return ln
 
     def embed_words(self, input_ids_2d, norm_scope_name="position_embeddings", reuse=None):
         """Public mirror of :262-297; returns bf16 [B, L, H]."""
@@ -614,7 +451,7 @@ class MerlotModel(object):
         Blo, Llo = ids.shape
         self._ids_lo = ids
         h0 = bf.get("lo.h0", (Blo * Llo, H), torch.bfloat16)
-        self._embed_words_into(ids, "langonly_embeddings", "emb_lo", _SITE_EMB_LO, h0, (0, 0, 0))
+        self._emb_lo_ln = self._embed_words_into(ids, "langonly_embeddings", "emb_lo", _SITE_EMB_LO, h0, (0, 0, 0))
         valid = bf.get("lo.valid", (Blo * Llo,), torch.uint8)
         ops.ids_valid(ids, valid)
         summ = bf.get("lo.attn_summ", (Blo * Llo,), torch.float32, zero=True)
@@ -727,17 +564,16 @@ class MerlotModel(object):
         act = bf.get(f"{tag}.act", (R, Hout), torch.float32)
         ops.gelu_f32(pre, act)
         an = bf.get(f"{tag}.an", (R, Hout), torch.bfloat16)
-        mean, rstd = bf.get(f"{tag}.mean", (R,), torch.float32), bf.get(f"{tag}.rstd", (R,), torch.float32)
-        ops.layernorm_fwd(act, an, st.P(f"{ln_scope}/gamma"), st.P(f"{ln_scope}/beta"), mean, rstd, rows=R)
-        return dict(x=x_bf16, pre=pre, act=act, an=an, mean=mean, rstd=rstd, dense=dense_scope, ln=ln_scope, R=R, Hout=Hout, tag=tag)
+        ln = _LayerNorm(st, ln_scope, act, bf.get(f"{tag}.mean", (R,), torch.float32), bf.get(f"{tag}.rstd", (R,), torch.float32),
+                        rows=R)
+        ln.forward(an)
+        return dict(x=x_bf16, pre=pre, an=an, ln=ln, dense=dense_scope, R=R, Hout=Hout, tag=tag)
 
     def _mlp_ln_bwd(self, t, d_an_f32, need_dx=True):
         """Backward of _mlp_ln: accumulates parameter grads, returns d_x fp32 [R, Hin]."""
-        st, bf = self.store, self._bufs
+        bf = self._bufs
         R, Hout, tag = t["R"], t["Hout"], t["tag"]
-        d_act = bf.get(f"{tag}.d_act", (R, Hout), torch.float32)
-        ops.layernorm_bwd(d_an_f32, t["act"], t["mean"], t["rstd"], st.P(f"{t['ln']}/gamma"), d_act, st.G(f"{t['ln']}/gamma"),
-                          st.G(f"{t['ln']}/beta"), rows=R)
+        d_act = t["ln"].backward(d_an_f32, bf.get(f"{tag}.d_act", (R, Hout), torch.float32))
         d_pre = bf.get(f"{tag}.d_pre", (R, Hout), torch.float32)
         ops.gelu_bwd_f32(d_act, t["pre"], d_pre)
         return self._dense_bwd(tag, t["x"], t["dense"], d_pre, need_dx)
@@ -855,7 +691,7 @@ class MerlotModel(object):
         labels = bf.get("ctr.labels", (n,), torch.int32)
         labels.copy_(torch.arange(n, dtype=torch.int32, device=labels.device) + rank * n)
         nW = n * world
-        outs = {}
+        outs, out2s = {}, {}
         info = dict(lang=lang, viz=viz, all_lang=all_lang, all_viz=all_viz, labels=labels, nW=nW, temp=temp, dirs={})
         for name, x, y in (("lang_to_viz", lang["feat"], all_viz), ("viz_to_lang", viz["feat"], all_lang)):
             logits = bf.get(f"ctr.{name}.logits", (n, nW), torch.float32)
@@ -865,11 +701,11 @@ class MerlotModel(object):
             out2 = bf.get(f"ctr.{name}.out", (2,), torch.float32)
             coeff = bf.get(f"ctr.{name}.coeff", (n,), torch.float32)
             ops.weighted_loss(per, None, None, None, 0, coef / 2.0, out2, coeff)
-            outs[name] = out2[0]
+            outs[name], out2s[name] = out2[0], out2
             info["dirs"][name] = dict(logits=logits, lse=lse, coeff=coeff)
         loss_all = bf.get("ctr.loss_all", (1,), torch.float32)
-        ops.axpby(bf.get("ctr.lang_to_viz.out", (2,), torch.float32)[:1], loss_all, coef / 2.0, 0.0)
-        ops.axpby(bf.get("ctr.viz_to_lang.out", (2,), torch.float32)[:1], loss_all, coef / 2.0, 1.0)
+        ops.axpby(out2s["lang_to_viz"][:1], loss_all, coef / 2.0, 0.0)
+        ops.axpby(out2s["viz_to_lang"][:1], loss_all, coef / 2.0, 1.0)
         outs["loss_all"] = loss_all[0]
         self._heads["ctr"] = info
         return loss_all[0], outs
@@ -966,7 +802,7 @@ class MerlotModel(object):
         w = self._tmp_w
         coef = cfg.get("temporal_coef", 1.0)
         use_vv = cfg.get("image_shuffle_prob", 0) > 0  # :664-665
-        info, heads = {}, {}
+        info, heads, out2s = {}, {}, {}
         for name, xa, xb in (("lang_viz", h_lang, h_viz), ("viz_viz", h_viz, h_viz)):
             hd = self._temporal_head(f"tmp.{name}", f"{name}_temporal", xa, xb)
             R = hd["R"]
@@ -975,12 +811,12 @@ class MerlotModel(object):
             out2 = bf.get(f"tmp.{name}.out", (2,), torch.float32)
             coeff = bf.get(f"tmp.{name}.coeff", (R,), torch.float32)
             ops.weighted_loss(per, corr, w, None, 0, coef, out2, coeff)
-            info[f"{name}_loss"], info[f"{name}_acc"] = out2[0], out2[1]
+            info[f"{name}_loss"], info[f"{name}_acc"], out2s[name] = out2[0], out2[1], out2
             heads[name] = dict(lse=lse, coeff=coeff, in_loss=(name == "lang_viz" or use_vv), **hd)
         tot = bf.get("tmp.loss", (1,), torch.float32)
-        ops.axpby(bf.get("tmp.lang_viz.out", (2,), torch.float32)[:1], tot, 1.0, 0.0)
+        ops.axpby(out2s["lang_viz"][:1], tot, 1.0, 0.0)
         if use_vv:
-            ops.axpby(bf.get("tmp.viz_viz.out", (2,), torch.float32)[:1], tot, 1.0, 1.0)
+            ops.axpby(out2s["viz_viz"][:1], tot, 1.0, 1.0)
         info["loss"] = tot[0]
         loss = bf.get("tmp.loss_scaled", (1,), torch.float32)
         ops.axpby(tot, loss, coef, 0.0)
@@ -1019,7 +855,7 @@ class MerlotModel(object):
         if not self._save:
             raise RuntimeError("MerlotModel was built without save_for_backward (is_training=False)")
         cfg, st, bf, D = self.config, self.store, self._bufs, self._dims
-        H, B, Lj, N = self.hidden_size, self.B, self.L, D["N"]
+        H, B, N = self.hidden_size, self.B, D["N"]
         Sj, Pz, vcl, Sv, Mv, np_, ncls = D["Sj"], D["Pz"], D["vcl"], D["Sv"], D["Mv"], D["np"], D["ncls"]
         vt = "vision_backbone/vision_transformer"
         d_yj = bf.get("bwd.d_yj", (B * Sj, H), torch.bfloat16, zero=True)
@@ -1037,7 +873,6 @@ class MerlotModel(object):
             self._contrastive_bwd(d_lang_trg, d_img_trg)
         if "tmp" in self._heads:
             self._temporal_bwd(d_yj)
-        p_emb = float(self.dropout_prob or 0.0)
         # ---- language-only encoder backward on the side stream: it needs only d_lang_trg (contrastive head) and runs
         # concurrently with the joint-encoder backward below, whose small grids leave a third of the SMs idle ----
         side = self._side_stream()
@@ -1050,24 +885,19 @@ class MerlotModel(object):
                 ops.scatter_add_rows(d_lang_trg, self._pool_idx_lo, d_ylo)
                 d_h0lo = bf.get("bwd.d_h0lo", (Blo * Llo, H), torch.bfloat16)
                 self._lo.backward(d_ylo, d_h0lo)
-                self._embed_bwd("emb_lo", "langonly_embeddings", self._ids_lo, d_h0lo, (0, 0, 0), (p_emb, self._seed, _SITE_EMB_LO),
-                                Blo, Llo)
+                self._embed_bwd("emb_lo", "langonly_embeddings", self._emb_lo_ln, self._ids_lo, d_h0lo)
         # ---- joint encoder ----
         d_jin = bf.get("bwd.d_jin", (B * Sj, H), torch.bfloat16)
         self._joint.backward(d_yj, d_jin)
         # lang piece: embed_norm(position_embeddings) -> word / position tables
-        self._embed_bwd("emb_j", "position_embeddings", self._ids_j, d_jin, (Lj, Sj, Pz), (p_emb, self._seed, _SITE_EMB_J), B, Lj)
+        self._embed_bwd("emb_j", "position_embeddings", self._emb_j_ln, self._ids_j, d_jin)
         # viz piece: final_ln -> K7 backward
         nt = self.num_texts
         Bi = B // nt
         dxz = None
         for j in range(nt):  # the nt texts of an image group all send gradient into the same viz tokens: summed through `dres`
             dxj = bf.get(f"bwd.dxsum_z.{j & 1}", (Bi * Pz, H), torch.float32)
-            ops.layernorm_bwd(d_jin, bf.get("viz.xsum", (Bi * Pz, H), torch.float32), bf.get("viz.mean", (Bi * Pz,), torch.float32),
-                              bf.get("viz.rstd", (Bi * Pz,), torch.float32), st.P("vision_backbone/LayerNorm_final_ln/gamma"), dxj,
-                              st.G("vision_backbone/LayerNorm_final_ln/gamma"), st.G("vision_backbone/LayerNorm_final_ln/beta"),
-                              dres=dxz, rows=Bi * Pz, remap=(Pz, nt * Sj, j * Sj))
-            dxz = dxj
+            dxz = self._viz_ln.backward(d_jin, dxj, dres=dxz, remap=(Pz, nt * Sj, j * Sj))
         d_hv = bf.get("bwd.d_hv", (Mv, H), torch.bfloat16)
         ops.viz_assemble_bwd(dxz, d_img_trg, d_hv, N, D["h1"], D["w1"], ncls, D["sp"], H)
         ops.segment_rowsum_scatter(dxz, N, vcl, self._img_idx, st.G("vision_backbone/img_idx_pe"), H)
@@ -1081,35 +911,30 @@ class MerlotModel(object):
         # ---- ViT ----
         d_h0v = bf.get("bwd.d_h0v", (Mv, H), torch.bfloat16)
         self._vit.backward(d_hv, d_h0v, vit_layer_groups, on_vit_group_done)
-        dxv = bf.get("bwd.dxsum_v", (Mv, H), torch.float32)
-        ops.layernorm_bwd(d_h0v, bf.get("vit.xsum", (Mv, H), torch.float32), bf.get("vit.mean0", (Mv,), torch.float32),
-                          bf.get("vit.rstd0", (Mv,), torch.float32), st.P(f"{vt}/LayerNorm_ctx_patches_pre_ln/gamma"), dxv,
-                          st.G(f"{vt}/LayerNorm_ctx_patches_pre_ln/gamma"), st.G(f"{vt}/LayerNorm_ctx_patches_pre_ln/beta"), rows=Mv)
+        dxv = self._vit_ln.backward(d_h0v, bf.get("bwd.dxsum_v", (Mv, H), torch.float32))
         ops.group_rowsum(dxv, N, Sv, 0, ncls, None, st.G(f"{vt}/pos_embs/cls_emb"), H)
         ops.group_rowsum(dxv, N, Sv, ncls, np_, self._grid_idxmap(D["h1"], D["w1"]), st.G(f"{vt}/pos_embs/pos_embs"), H)
         dpatch = bf.get("bwd.dpatch", (N * np_, H), torch.bfloat16)
         ops.vit_assemble_bwd(dxv, dpatch, N, np_, ncls, H)
         if not self._resnet_layers:
             ops.bias_grad(dpatch, st.G(f"{vt}/conv2d/bias"), rows=N * np_, N=H)
-            ops.gemm(bf.get("vit.A", (N * np_, D["Kp"]), torch.bfloat16), dpatch, a_mn_major=True, b_mn_major=True,
-                     out=st.G(f"{vt}/conv2d/kernel"), atomic=True, M=D["Kp"], N=H, K=N * np_)
+            ops.gemm(self._patch_A, dpatch, a_mn_major=True, b_mn_major=True, out=st.G(f"{vt}/conv2d/kernel"), atomic=True,
+                     M=D["Kp"], N=H, K=N * np_)
         else:  # conv_postresnet_proj (1x1 + bias, not standardised), then the stem's tape
-            rc = self._stem_tape[-1][1]["y"]
-            Cr = rc.shape[1]
+            Cr = self._rc.shape[1]
             ops.bias_grad(dpatch, st.G(f"{vt}/conv_postresnet_proj/bias"), rows=N * np_, N=H)
-            ops.gemm(rc, dpatch, a_mn_major=True, b_mn_major=True, out=st.G(f"{vt}/conv_postresnet_proj/kernel"), atomic=True,
+            ops.gemm(self._rc, dpatch, a_mn_major=True, b_mn_major=True, out=st.G(f"{vt}/conv_postresnet_proj/kernel"), atomic=True,
                      M=Cr, N=H, K=N * np_)
-            d_rc = bf.get("bwd.d_rc", (N * np_, Cr), torch.bfloat16)
-            ops.gemm(dpatch, st.W(f"{vt}/conv_postresnet_proj/kernel"), out=d_rc)  # [M, H] . [Cr, H]^T
-            self._hybrid_stem_backward(d_rc, N)
-    def _embed_bwd(self, tag, norm_scope_name, ids_2d, dy, remap, dropout, groups, Lseq):
+            self.d_rc = bf.get("bwd.d_rc", (N * np_, Cr), torch.bfloat16)
+            ops.gemm(dpatch, st.W(f"{vt}/conv_postresnet_proj/kernel"), out=self.d_rc)  # [M, H] . [Cr, H]^T
+            self._stem.backward(self.d_rc)
+
+    def _embed_bwd(self, tag, norm_scope_name, ln, ids_2d, dy):
+        """Backward of _embed_words_into, whose embed_norm is `ln`."""
         st, bf = self.store, self._bufs
-        H, R = self.hidden_size, ids_2d.numel()
-        dx = bf.get(f"bwd.dxsum.{tag}", (R, H), torch.float32)
-        ops.layernorm_bwd(dy, bf.get(f"{tag}.xsum", (R, H), torch.float32), bf.get(f"{tag}.mean", (R,), torch.float32),
-                          bf.get(f"{tag}.rstd", (R,), torch.float32), st.P(f"{norm_scope_name}/LayerNorm_embed_norm/gamma"), dx,
-                          st.G(f"{norm_scope_name}/LayerNorm_embed_norm/gamma"), st.G(f"{norm_scope_name}/LayerNorm_embed_norm/beta"),
-                          rows=R, remap=remap, dropout=dropout if self.is_training else (0.0, 0, 0))
+        (groups, Lseq), H = ids_2d.shape, self.hidden_size
+        dx = ln.backward(dy, bf.get(f"bwd.dxsum.{tag}", (ids_2d.numel(), H), torch.float32),
+                         dropout=ln.kw["dropout"] if self.is_training else (0.0, 0, 0))
         ops.scatter_add_rows(dx, ids_2d.reshape(-1), st.G("word_embeddings/word_embeddings"))
         ops.group_rowsum(dx, groups, Lseq, 0, Lseq, None, st.G(f"{norm_scope_name}/position_embeddings"), H)
 

@@ -27,6 +27,7 @@ from typing import Dict, List, Optional, Tuple
 import torch
 
 from . import ops
+from .stem import stem_ops
 
 PAD = 64
 TEMPORAL_PAD_N = 8
@@ -126,45 +127,15 @@ def _entries(cfg: dict, task: str = "pretrain") -> List[Entry]:
 
 
 def stem_variables(scope: str, layers, width: int, hidden: int):
-    """Variables of the hybrid ResNet-lite stem in the reference's creation order (utils/vision_transformer.py:69-170,213-223;
-    names per SURVEY.md Appendix A: conv2d, conv2d_1, ... / GroupNorm, GroupNorm_1, ... uniquified inside each variable scope).
-    Yields (name, TF shape) with conv kernels HWIO."""
-    out = []
-
-    class _Scope:
-        def __init__(self, s):
-            self.s, self.nc, self.ng = s, 0, 0
-
-        def conv(self, kh, cin, cout):
-            out.append((f"{self.s}/conv2d{'' if self.nc == 0 else '_%d' % self.nc}/kernel", (kh, kh, cin, cout)))
-            self.nc += 1
-
-        def gn(self, c, name=None):
-            base = f"{self.s}/GroupNorm_{name}" if name is not None else f"{self.s}/GroupNorm{'' if self.ng == 0 else '_%d' % self.ng}"
-            if name is None:
-                self.ng += 1
-            out.append((f"{base}/gamma", (c,)))
-            out.append((f"{base}/beta", (c,)))
-
-    st = _Scope(f"{scope}/resnet50lite/stem")
-    for i, (cin, cout) in enumerate(((3, width // 2), (width // 2, width // 2), (width // 2, width))):
-        st.conv(3, cin, cout)
-        st.gn(cout, f"stem{i}")
-    cin = width
-    for i, blocks in enumerate(layers):
-        f = width * (2 ** i)
-        bg = _Scope(f"{scope}/resnet50lite/block_group{i + 1}")
-        for b in range(blocks):
-            if b == 0:  # projection shortcut is created first (:77-85)
-                bg.conv(1, cin, 4 * f)
-                bg.gn(4 * f)
-            bg.conv(1, cin, f)
-            bg.gn(f)
-            bg.conv(3, f, f)
-            bg.gn(f)
-            bg.conv(1, f, 4 * f)
-            bg.gn(4 * f)
-            cin = 4 * f
+    """Variables of the hybrid ResNet-lite stem in the reference's creation order (stem.stem_ops), then the 1x1
+    conv_postresnet_proj (utils/vision_transformer.py:213-223).  Returns (name, TF shape) pairs with conv kernels HWIO."""
+    out, cin = [], width
+    for op in stem_ops(scope, tuple(layers), width):
+        if op.kind == "conv":
+            out.append((op.name, (op.k, op.k, op.cin, op.cout)))
+            cin = op.cout
+        elif op.kind == "gn":
+            out += [(f"{op.name}/gamma", (op.cout,)), (f"{op.name}/beta", (op.cout,))]
     out.append((f"{scope}/conv_postresnet_proj/kernel", (1, 1, cin, hidden)))
     out.append((f"{scope}/conv_postresnet_proj/bias", (hidden,)))
     return out

@@ -203,6 +203,7 @@ def model_fn_builder(config: NeatConfig, *, store: Optional[ParamStore] = None, 
         store.init_reference(seed=0)
     optimizer, _ = build_optimizer_from_config(loss=None, optimizer_config=config.optimizer, device_config=config.device,
                                                store=store)
+    skip = variables_without_gradient(config.model, store)
 
     def model_fn(features, labels=None, mode="train", params=None):
         is_training = mode == "train"
@@ -216,14 +217,10 @@ def model_fn_builder(config: NeatConfig, *, store: Optional[ParamStore] = None, 
                             (dist.rank if dist is not None else 0), dist=dist, log_attention_probs=log_attention_probs)
         lang_loss, lang_losses = model.mask_loss()
         contr_loss, contr_losses = model.contrastive_loss()
-        skip = []
         if config.model.get("temporal_coef", 1.0) > 0.0:
             temp_loss, temp_losses = model.temporal_loss(features["shuffled_idx_img"], video_src_ids=features["video_src_ids"])
-            if not config.model.get("image_shuffle_prob", 0) > 0:
-                skip = [n for n in store.entries if n.startswith("viz_viz_temporal/")]
         else:
             temp_loss, temp_losses = torch.zeros((), device=store.device), {}
-            skip = [n for n in store.entries if "_temporal/" in n]
         losses = {f"lang/{k}": v for k, v in lang_losses.items()}
         losses.update({f"contr/{k}": v for k, v in contr_losses.items()})
         losses.update({f"temporal/{k}": v for k, v in temp_losses.items()})

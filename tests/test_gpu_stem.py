@@ -85,7 +85,7 @@ def _stem_cfg(tiny_cfg):
     return dict(tiny_cfg, resnet_layers=[1, 2, 1], hidden_dropout_prob=0.0)
 
 
-def test_hybrid_stem_and_model_forward(tiny_cfg):
+def test_hybrid_stem_forward_and_model_forward(tiny_cfg):
     """lite_resnet50 + conv_postresnet_proj inside the MerlotModel forward (is_training=False) against the oracle on the same
     weights (the backward has its own tests below)."""
     from merlot_b200.modeling import MerlotModel
@@ -97,7 +97,7 @@ def test_hybrid_stem_and_model_forward(tiny_cfg):
     m = MerlotModel(cfg, is_training=False, use_tpu=False, image=image.to(DEV), input_ids=ids.to(DEV), mask_input=False,
                     shuffled_idx_img=shuf.to(DEV), params=store)
     N = batch * nc
-    rc, hs, ws = m._hybrid_stem(image.bfloat16().to(DEV).contiguous(), N, 64, 96)
+    rc, hs, ws = m._stem.forward(image.bfloat16().to(DEV).contiguous(), N, 64, 96)
     scope = "vision_backbone/vision_transformer/resnet50lite"
     ref = O.lite_resnet50(image - 0.5, params, scope, cfg["resnet_layers"])
     ref16 = O.lite_resnet50(image - 0.5, params, scope, cfg["resnet_layers"], rnd=O.bf16_round)  # the reference's own dtype policy
@@ -238,20 +238,18 @@ def _stem_model(tiny_cfg, h0, w0, batch=2, nc=2, save=True):
     return cfg, m, params, store, (image, ids, shuf, vid)
 
 
-def test_stem_backward_in_situ(tiny_cfg):
+def test_hybrid_stem_backward_in_situ(tiny_cfg):
     """Every op of the real lite_resnet50 tape (128x192 input: maps 64x96, 32x48, 16x24, 8x12; 4 frames), backward vs autograd
     of that single op on the GPU's own saved input and incoming gradient; plus gradient routing."""
     cfg, m, params, store, (image, ids, shuf, vid) = _stem_model(tiny_cfg, 128, 192)
     N = image.shape[0]
-    tape = m._stem_tape
+    tape = m._stem.tape
     rc = tape[-1][1]["y"]
     g = torch.Generator().manual_seed(3)
     d_rc = (torch.randn(rc.shape, generator=g) * 0.1).bfloat16().to(DEV)
     store.g.zero_()
-    m._stem_trace = []
-    m._hybrid_stem_backward(d_rc.clone(), N)
-    trace = m._stem_trace
-    m._stem_trace = None
+    trace = []
+    m._stem.backward(d_rc.clone(), trace=trace)
     assert len(trace) == len(tape)
     f = lambda t: t.float().cpu()
     worst = {"gn": 0.0, "conv": 0.0, "pool": 0.0, "param": 0.0}
@@ -310,13 +308,13 @@ def test_stem_backward_in_situ(tiny_cfg):
     store.g.zero_()
 
 
-def test_training_step_through_the_stem(tiny_cfg, monkeypatch):
+def test_training_step_through_the_hybrid_stem(tiny_cfg, monkeypatch):
     """Whole pretraining step with the hybrid stem; the oracle's lite_resnet50 is replaced by a LEAF holding the GPU's stem
     output, so the two graphs share their rounding points at the stem boundary: the three losses, every non-stem gradient and the
     gradient handed to the stem are compared at bf16 noise-floor bars (1e-3 losses; gradients 6e-2 worst tensor, 2.5e-2 median, 4e-2 at the stem boundary)."""
     cfg, m, params, store, (image, ids, shuf, vid) = _stem_model(tiny_cfg, 128, 192)
     N = image.shape[0]
-    rc = m._stem_tape[-1][1]["y"]
+    rc = m._stem.tape[-1][1]["y"]
     hs, ws = 128 // 16, 192 // 16
     leaf_rc = rc.float().cpu().reshape(N, hs, ws, rc.shape[1]).clone().requires_grad_(True)
     monkeypatch.setattr(O, "lite_resnet50", lambda x, p, scope, layers, width=64, rnd=O._ident: leaf_rc)
@@ -338,8 +336,7 @@ def test_training_step_through_the_stem(tiny_cfg, monkeypatch):
         if "resnet50lite" in k or v.grad is None or float(v.grad.norm()) < 1e-7:
             continue
         worst[k] = rel(grads[k], v.grad)
-    d_rc = m._bufs.get("bwd.d_rc", (N * hs * ws, rc.shape[1]), torch.bfloat16)
-    e_rc = rel(d_rc, leaf_rc.grad.reshape(N * hs * ws, -1))
+    e_rc = rel(m.d_rc, leaf_rc.grad.reshape(N * hs * ws, -1))
     stem_norm = sum(float(grads[k].norm()) for k in grads if "resnet50lite" in k)
     top = sorted(worst.items(), key=lambda kv: -kv[1])[:4]
     vals = sorted(worst.values())

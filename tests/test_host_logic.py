@@ -280,6 +280,8 @@ def test_hybrid_stem_param_arena(tiny_cfg):
     from merlot_b200.params import stem_variables
     n_stem = sum(int(torch.tensor(s_).prod()) for _, s_ in stem_variables(vt, gold["model"]["resnet_layers"], 64, 768))
     assert n_stem == 11_914_080 + 1024 * 768 + 768  # SURVEY Appendix D: 11.91 M + 0.79 M
+    for layers in ([1, 2, 1], [3, 4, 9]):  # same names, shapes and order: arena offsets and checkpoint layout follow the order
+        assert stem_variables(vt, layers, 64, 768) == list(O.resnet_param_shapes(vt, layers, 64, 768).items()), layers
 
 
 def test_param_arena_roundtrip_and_count(tiny_cfg):

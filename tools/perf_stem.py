@@ -21,12 +21,12 @@ torch.cuda.synchronize()
 img = feats["images"].contiguous()
 N = img.shape[0]
 for _ in range(2):
-    rc, h, w = m._hybrid_stem(img, N, 192, 352)
+    rc, h, w = m._stem.forward(img, N, 192, 352)
 torch.cuda.synchronize()
 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
 e0.record()
 for _ in range(5):
-    rc, h, w = m._hybrid_stem(img, N, 192, 352)
+    rc, h, w = m._stem.forward(img, N, 192, 352)
 e1.record()
 torch.cuda.synchronize()
 ms = e0.elapsed_time(e1) / 5

@@ -1,15 +1,15 @@
-"""CPU check of the hybrid stem's ORCHESTRATION (forward tape + backward walk in merlot_b200/modeling.py) without a GPU: every
-K13 / K1 call is emulated in fp32 torch with the same formulas as the CUDA kernels, and the parameter gradients that come out of
-MerlotModel._hybrid_stem_backward are compared with torch autograd through the oracle's lite_resnet50.  Proves names, shapes, op
+"""CPU check of the hybrid stem's ORCHESTRATION (forward tape + backward walk of merlot_b200/stem.py's HybridStem) without a GPU:
+every K13 / K1 call is emulated in fp32 torch with the same formulas as the CUDA kernels, and the parameter gradients that come out
+of HybridStem.backward are compared with torch autograd through the oracle's lite_resnet50.  Proves names, shapes, op
 order, gradient routing and the closed-form backward formulas -- not the CUDA code itself."""
 import sys
-import types
 
 import torch
 
 sys.path.insert(0, ".")
-from merlot_b200 import modeling, ops  # noqa: E402
+from merlot_b200 import ops  # noqa: E402
 from merlot_b200.params import ParamStore  # noqa: E402
+from merlot_b200.stem import HybridStem  # noqa: E402
 from oracle import merlot_oracle as O  # noqa: E402
 
 LAYERS = [1, 2, 1]
@@ -179,14 +179,13 @@ class Bufs:
         return self.d[k]
 
 
-fake = types.SimpleNamespace(store=st, _bufs=Bufs(), _resnet_layers=LAYERS, _save=True)
-fake._ws_plan = lambda: modeling.MerlotModel._ws_plan(fake)
+stem = HybridStem(st, Bufs(), LAYERS, save=True)
 N = 2
 gen = torch.Generator().manual_seed(1)
 img = torch.rand(N, 64, 96, 3, generator=gen)
-rc, h, w = modeling.MerlotModel._hybrid_stem(fake, img, N, 64, 96)
+rc, h, w = stem.forward(img, N, 64, 96)
 d_out = torch.randn(rc.shape, generator=gen) * 0.1
-modeling.MerlotModel._hybrid_stem_backward(fake, d_out.clone(), N)
+stem.backward(d_out.clone())
 
 leaf = {k: v.clone().requires_grad_(True) for k, v in params.items() if "resnet50lite" in k}
 ref = O.lite_resnet50(img - 0.5, leaf, "vision_backbone/vision_transformer/resnet50lite", LAYERS)
