@@ -68,16 +68,35 @@ static LayerAct carve(const merlot_stack_t* s, char* base) {
   return a;
 }
 
+// Longest sequence every attention kernel of a layer accepts: their token-validity bitmask covers 4096 positions and the
+// host checks of merlot_attention_fwd / _bwd / _colsum keep one 128-row tile of it in reserve (csrc/attention.cu).
+constexpr int kMaxStackSeq = 4096 - 128;
+static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+// The descriptor checks shared by forward and backward, made before anything is enqueued: the dimensions, sequence length,
+// validity / pair mask and dropout probability the attention, GEMM and LayerNorm calls of a layer require, and the 16-byte
+// alignment their vector and TMA accesses need of the input, the arena and the bf16 weights.  The buffers only one direction
+// reads (y; dy, dh_in, scratch) are checked at the top of that direction.
 static int check_stack(const merlot_stack_t* s) {
   MB_REQUIRE(s != nullptr, MERLOT_EINVAL, "stack: null descriptor");
-  MB_REQUIRE(s->B > 0 && s->S > 0 && s->layers > 0, MERLOT_ESHAPE, "stack: bad dims B=%d S=%d layers=%d", s->B, s->S, s->layers);
+  MB_REQUIRE(s->B > 0 && s->S > 0 && s->heads > 0 && s->I > 0 && s->layers > 0, MERLOT_ESHAPE,
+             "stack: bad dims B=%d S=%d heads=%d I=%d layers=%d", s->B, s->S, s->heads, s->I, s->layers);
+  MB_REQUIRE(s->S <= kMaxStackSeq, MERLOT_ESHAPE, "stack: sequence length %d exceeds the attention kernels' %d", s->S,
+             kMaxStackSeq);
   MB_REQUIRE(s->H == s->heads * 64, MERLOT_ESHAPE,
              "stack: hidden_size %d != num_attention_heads %d * 64 (utils/transformer.py:16-19 raises ValueError on the same mismatch)",
              s->H, s->heads);
   MB_REQUIRE(s->H % 8 == 0 && s->I % 8 == 0 && s->H <= 1024, MERLOT_ESHAPE, "stack: H, I must be multiples of 8 and H <= 1024");
   MB_REQUIRE(s->layer_params && s->h_in && s->act_arena && s->final_gamma && s->final_beta, MERLOT_EINVAL, "stack: null pointer");
+  MB_REQUIRE(s->pair_chunk_len >= 0 && s->pair_viz_len >= 0 && (s->pair_chunk_len == 0 || s->valid != nullptr), MERLOT_EINVAL,
+             "stack: pair_chunk_len > 0 (disable_pairwise_lang_attn) needs the token-validity mask and non-negative lengths");
   MB_REQUIRE(s->attention_dropout_p >= 0.f && s->attention_dropout_p < 1.f, MERLOT_EINVAL,
              "stack: attention_probs_dropout_prob must lie in [0, 1) (got %g)", (double)s->attention_dropout_p);
+  MB_REQUIRE(aligned16(s->h_in) && aligned16(s->act_arena), MERLOT_EINVAL, "stack: h_in and act_arena must be 16-byte aligned");
+  for (int l = 0; l < s->layers; ++l) {
+    const merlot_layer_params_t& P = s->layer_params[l];
+    MB_REQUIRE(aligned16(P.w_qkv) && aligned16(P.w_o) && aligned16(P.w_1) && aligned16(P.w_2), MERLOT_EINVAL,
+               "stack: layer %d: bf16 weights must be 16-byte aligned", l);
+  }
   return MERLOT_OK;
 }
 
@@ -153,7 +172,7 @@ extern "C" size_t merlot_stack_scratch_bytes(const merlot_stack_t* s) {
 extern "C" int merlot_stack_forward(const merlot_stack_t* s, void* stream_) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
   RC(check_stack(s));
-  MB_REQUIRE(s->y != nullptr, MERLOT_EINVAL, "stack_forward: y is null");
+  MB_REQUIRE(s->y != nullptr && aligned16(s->y), MERLOT_EINVAL, "stack_forward: y is null or not 16-byte aligned");
   const int M = s->B * s->S, H = s->H, I = s->I;
   const size_t per = layer_act_bytes(s);
   char* arena = reinterpret_cast<char*>(s->act_arena);
@@ -224,6 +243,13 @@ extern "C" int merlot_stack_backward(const merlot_stack_t* s, void* stream_) {
   RC(check_stack(s));
   MB_REQUIRE(s->save_for_backward, MERLOT_EINVAL, "stack_backward: forward was not run with save_for_backward");
   MB_REQUIRE(s->dy && s->scratch && s->d_final_gamma && s->d_final_beta, MERLOT_EINVAL, "stack_backward: null pointer");
+  MB_REQUIRE(aligned16(s->dy) && aligned16(s->dh_in) && aligned16(s->scratch), MERLOT_EINVAL,
+             "stack_backward: dy, dh_in and scratch must be 16-byte aligned");
+  // partial backward (bwd_lo/bwd_hi): the stream gradient is back in dhA after every complete layer (two swaps per layer), so
+  // a call that resumes below the top layer simply continues from dhA
+  const int l_hi = (s->bwd_hi > 0) ? s->bwd_hi : s->layers;
+  const int l_lo = (s->bwd_hi > 0) ? s->bwd_lo : 0;
+  MB_REQUIRE(0 <= l_lo && l_lo < l_hi && l_hi <= s->layers, MERLOT_EINVAL, "stack_backward: bad layer range [%d, %d)", l_lo, l_hi);
   const int M = s->B * s->S, H = s->H, I = s->I;
   const size_t per = layer_act_bytes(s);
   char* arena = reinterpret_cast<char*>(s->act_arena);
@@ -279,11 +305,6 @@ extern "C" int merlot_stack_backward(const merlot_stack_t* s, void* stream_) {
   };
   char* dh = dhA;
   char* dh_other = dhB;
-  // partial backward (bwd_lo/bwd_hi): the stream gradient is back in dhA after every complete layer (two swaps per layer), so
-  // a call that resumes below the top layer simply continues from dhA
-  const int l_hi = (s->bwd_hi > 0) ? s->bwd_hi : s->layers;
-  const int l_lo = (s->bwd_hi > 0) ? s->bwd_lo : 0;
-  MB_REQUIRE(0 <= l_lo && l_lo < l_hi && l_hi <= s->layers, MERLOT_EINVAL, "stack_backward: bad layer range [%d, %d)", l_lo, l_hi);
   if (l_hi == s->layers)
   {  // final LN; its output is the gradient of the last layer's FFN2 output
     LayerAct A = carve(s, arena + per * (s->layers - 1));

@@ -62,11 +62,11 @@ def _keep_tensor(seed: int, site: int, B: int, heads: int, S: int, p: float) -> 
 
 
 def drop_probs(probs: torch.Tensor, seed: int, site: int, p: float) -> torch.Tensor:
-    """probs [B, heads, S, S] * keep * 1/(1-p) under the mask of (seed, site); probs itself when p = 0."""
+    """probs [B, heads, S, S] * keep * 1/(1-p) under the mask of (seed, site), on probs' device; probs itself when p = 0."""
     if p == 0.0:
         return probs
     B, heads, S, _ = probs.shape
-    keep = _keep_tensor(int(seed), int(site), B, heads, S, float(p))
+    keep = _keep_tensor(int(seed), int(site), B, heads, S, float(p)).to(probs.device)
     return probs * (keep.to(probs.dtype) * float(DM.dropout_scale(p)))
 
 

@@ -34,13 +34,11 @@ def test_binding_covers_every_header_symbol():
 
 
 # Header functions no tests/test_gpu_*.py has to call by name.  Pure queries and sizes return host values that the GPU tests
-# use without asserting them one by one (test_attention_bwd_dq_mode_boundary pins the dQ pair); the stack drivers run three
-# times in every whole-model step of test_gpu_model.py, test_gpu_fullsize.py and test_gpu_vcr_train.py.
+# use without asserting them one by one (test_attention_bwd_dq_mode_boundary pins the dQ pair).
 UNTESTED_BY_NAME_OK = {
-    "merlot_abi_version", "merlot_last_error", "merlot_set_sm_reserve",   # queries / process settings
+    "merlot_abi_version", "merlot_last_error",                            # queries
     "merlot_launch_count", "merlot_reset_launch_count",                   # launch counters
     "merlot_gemm_profile_begin", "merlot_gemm_profile_end",               # bench.py's K1 profiler pair
-    "merlot_stack_forward", "merlot_stack_backward",                      # whole transformer stacks
 }
 
 
