@@ -212,6 +212,19 @@ def plan_frames(src_h, src_w, out_size: Sequence[int], scale, u_y, u_x) -> Dict[
     return {"scaled_h": sh, "scaled_w": sw, "offset_y": oy, "offset_x": ox}
 
 
+def plan_frames_eval(src_h, src_w, out_size: Sequence[int]) -> Dict[str, np.ndarray]:
+    """resize_and_pad(do_random_scale=False) (utils/model_utils.py:900-907,918-924) in float32 like the graph: scale by
+    min(Hd/h, Wd/w), truncate the resized sides to int32, no 64-pixel floor, crop origin 0 (pad bottom and right)."""
+    f32 = np.float32
+    Hd, Wd = out_size
+    h, w = np.asarray(src_h).astype(f32), np.asarray(src_w).astype(f32)
+    image_scale = np.minimum(f32(Hd) / h, f32(Wd) / w)
+    sh = (h * image_scale).astype(np.int32)
+    sw = (w * image_scale).astype(np.int32)
+    zero = np.zeros_like(sh)
+    return {"scaled_h": sh, "scaled_w": sw, "offset_y": zero, "offset_x": zero.copy()}
+
+
 # ---------------------------------------------------------------------------------------------------------------------------
 # input_fn_builder (model/dataloader.py:129-278), training input
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -252,6 +265,26 @@ def interleave_records(names: Iterator[str], cycle_length: int, files: Sequence[
         ended_in_a_row = 0
         readers.append(r)
         yield rec
+
+
+def shuffled_records(files: Sequence[str], rng: np.random.Generator, cycle_length: int, buffer_size: int,
+                     stop: Optional[threading.Event] = None):
+    """The training record stream (:153-184): list_files(shuffle=True) -> repeat -> parallel_interleave(cycle_length) ->
+    shuffle(buffer_size).  Every pass over the files is a fresh permutation drawn from `rng`, and so is every pick from
+    the shuffle buffer.  Endless unless `stop` is set."""
+    def names():
+        while True:
+            yield from (files[i] for i in rng.permutation(len(files)))
+
+    buf = []
+    for rec in interleave_records(names(), cycle_length, files, stop):
+        if len(buf) < buffer_size:
+            buf.append(rec)
+            continue
+        i = int(rng.integers(buffer_size))
+        buf[i], rec = rec, buf[i]
+        yield rec
+    yield from buf  # only reached when stopping
 
 
 def stage_frames(frames: Sequence[np.ndarray]):
@@ -366,25 +399,6 @@ class InputPipeline(DevicePipeline):
         self.rng = np.random.default_rng([seed, rank])
         super().__init__(device, num_threads, prefetch)
 
-    # -- record stream: list_files -> repeat -> parallel_interleave(cycle_length) -> shuffle (:153-184) --
-    def _file_names(self):
-        while True:
-            yield from (self.files[i] for i in self.rng.permutation(len(self.files)))
-
-    def _records(self):
-        return interleave_records(self._file_names(), self.cycle_length, self.files, self._stop)
-
-    def _shuffled(self):
-        buf, size = [], self.shuffle_buffer_size
-        for rec in self._records():
-            if len(buf) < size:
-                buf.append(rec)
-                continue
-            i = int(self.rng.integers(size))
-            buf[i], rec = rec, buf[i]
-            yield rec
-        yield from buf  # only reached when stopping
-
     # -- one batch --
     def _batch(self, records):
         b, n = self.batch_size, self.num_chunks
@@ -414,7 +428,7 @@ class InputPipeline(DevicePipeline):
         return feats, info
 
     def _produce(self):
-        recs = self._shuffled()
+        recs = shuffled_records(self.files, self.rng, self.cycle_length, self.shuffle_buffer_size, self._stop)
         while not self._stop.is_set():
             yield self._batch([next(recs) for _ in range(self.batch_size)])  # batch(drop_remainder=True) of a repeated stream
 

@@ -22,7 +22,7 @@ from typing import Dict, Iterable, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from .dataloader import DevicePipeline, decode_jpeg, interleave_records, stage_frames
+from .dataloader import DevicePipeline, decode_jpeg, interleave_records, plan_frames_eval, stage_frames
 from .tfrecord import parse_example
 
 NUM_CHUNKS = 5       # get_zero_shot_logits.py:26-28: five sentences and five frames per story
@@ -196,19 +196,6 @@ def decode_frame(story: Dict, i: int) -> np.ndarray:
         return decode_jpeg(buf)
     except Exception as e:
         raise ValueError(f"story {story['story_id']}: image {i} cannot be decoded ({type(e).__name__}: {e})") from e
-
-
-def plan_frames_eval(src_h, src_w, out_size: Sequence[int]) -> Dict[str, np.ndarray]:
-    """resize_and_pad(do_random_scale=False) (utils/model_utils.py:900-907,918-924) in float32 like the graph: scale by
-    min(Hd/h, Wd/w), truncate the resized sides to int32, no 64-pixel floor, crop origin 0 (pad bottom and right)."""
-    f32 = np.float32
-    Hd, Wd = out_size
-    h, w = np.asarray(src_h).astype(f32), np.asarray(src_w).astype(f32)
-    image_scale = np.minimum(f32(Hd) / h, f32(Wd) / w)
-    sh = (h * image_scale).astype(np.int32)
-    sw = (w * image_scale).astype(np.int32)
-    zero = np.zeros_like(sh)
-    return {"scaled_h": sh, "scaled_w": sw, "offset_y": zero, "offset_x": zero.copy()}
 
 
 def eval_frame_plan(hw: np.ndarray, story_ids: Sequence[int], out_size: Sequence[int]) -> Dict[str, np.ndarray]:

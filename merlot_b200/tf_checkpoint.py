@@ -574,3 +574,15 @@ def latest_checkpoint(directory: str) -> Optional[str]:
         return None
     p = latest if os.path.isabs(latest) else os.path.join(directory, latest)
     return p if os.path.exists(p + ".index") else None
+
+
+def checkpoint_prefixes(directory: str) -> List[str]:
+    """Every checkpoint the state file of `directory` names (all_model_checkpoint_paths, then model_checkpoint_path), once
+    each and resolved like latest_checkpoint, that still has its index file."""
+    latest, every = _read_state(directory)
+    out = []
+    for p in every + ([latest] if latest else []):
+        p = p if os.path.isabs(p) else os.path.join(directory, p)
+        if p not in out and os.path.exists(p + ".index"):
+            out.append(p)
+    return out

@@ -260,8 +260,8 @@ def variables_without_gradient(model_cfg: dict, store: ParamStore):
 
 def main(argv=None):
     """`python -m merlot_b200.train configs/merlot.yaml` (or merlot_vcr.yaml) -- the role of model/train.py:9-26 and
-    downstream/vcr/train.py.  Pretraining reads data.train_file when it matches at least one file (dataloader.input_fn_builder)
-    and otherwise trains on synthetic batches; VCR fine-tuning always trains on synthetic batches.
+    downstream/vcr/train.py.  Both read data.train_file when it matches at least one file (pretraining through
+    dataloader.input_fn_builder, VCR fine-tuning through vcr_input.input_fn_builder) and otherwise train on synthetic batches.
 
     Checkpoints, as the reference's Estimator keeps them (utils/neat_config.py:136-141): when device.output_dir already names
     a latest checkpoint, every rank restores it (parameters, Adam slots, global_step; this takes precedence over
@@ -302,9 +302,11 @@ def main(argv=None):
 
     per_rank = max(1, config.device.get("train_batch_size", 8) // world)
     pipeline = None
-    if make_batch is synthetic_batch and train_files(config.data):
-        pipeline = input_fn_builder(config, is_training=True, rank=rank, world=world, seed=store.global_step if resume else 0,
-                                    batch_size=per_rank)
+    if train_files(config.data):
+        from . import vcr_input
+        build_input = input_fn_builder if make_batch is synthetic_batch else vcr_input.input_fn_builder
+        pipeline = build_input(config, is_training=True, rank=rank, world=world, seed=store.global_step if resume else 0,
+                               batch_size=per_rank)
     elif rank == 0:
         print(f"data.train_file {config.data.get('train_file')!r} matches no file: training on synthetic batches"
               if make_batch is synthetic_batch else "VCR fine-tuning: training on synthetic batches", flush=True)

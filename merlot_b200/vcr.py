@@ -202,7 +202,9 @@ def vcr_model_fn_builder(config, *, store=None, dist=None, seed: int = 0, device
       * mode "train": MerlotModel(is_training=True, mask_input=False), cls_head + cls_loss; metrics loss / accuracy /
         learning_rate; train_op = the head backward, model.backward(d_hidden_state=...), gradient mean over replicas, AdamW;
       * mode "eval": MerlotModel(is_training=False), cls_head_val on the `{downstream.mode}_cls` tower; metrics loss, accuracy,
-        logits and predictions, no train_op.
+        logits and predictions, no train_op;
+      * mode "predict": as "eval" without lm_targets, loss or accuracy (metrics logits and predictions), for unlabelled
+        records: the CE kernel is not run.
     `store=None` builds ParamStore(task="vcr"), applies the reference initialisers and then `model.init_checkpoint` if set
     (restore by name, model/modeling.py:724-740: the towers keep their initial values; a missing checkpoint raises).  The
     dropout seed of a step follows the pretraining rule: seed + step * world + rank."""
@@ -227,7 +229,7 @@ def vcr_model_fn_builder(config, *, store=None, dist=None, seed: int = 0, device
     def model_fn(features, labels=None, mode="train", params=None):
         is_training = mode == "train"
         imgs, ids = features["images"], features["lm_input"]
-        target = (labels or features)["lm_targets"]
+        target = None if mode == "predict" else (labels or features)["lm_targets"]
         if is_training and m_cfg.get("transpose_input", False) and imgs.shape[-1] != 3:
             imgs = imgs.permute(3, 0, 1, 2).contiguous()  # :35-37
         if not is_training:  # [b, 4, L] -> [4b, L] (:39-44)
@@ -239,8 +241,11 @@ def vcr_model_fn_builder(config, *, store=None, dist=None, seed: int = 0, device
                             log_attention_probs=False)
         if not is_training:
             logits = cls_head_val(model, head_from_store(store, eval_mode), eval_mode)
+            metrics = {"logits": logits, "predictions": logits.argmax(-1)}
+            if target is None:
+                return StepSpec(model, (), metrics, None)
             loss, acc = cls_loss(logits, target)
-            metrics = {"loss": loss, "accuracy": acc, "logits": logits, "predictions": logits.argmax(-1)}
+            metrics.update(loss=loss, accuracy=acc)
             return StepSpec(model, (loss,), metrics, None)
         p = float(m_cfg.get("hidden_dropout_prob", 0.0) or 0.0)
         logits = cls_head(model, store, dropout=(p, step_seed))

@@ -1,0 +1,193 @@
+"""`python -m merlot_b200.vcr_validate CONFIG`: VCR validation, the role of downstream/vcr/validate.py.
+
+It follows device.output_dir the way tf.contrib.training.checkpoints_iterator does and evaluates every checkpoint newer than
+the last one it evaluated, oldest first.  It stops after the checkpoint whose global_step reaches optimizer.num_train_steps,
+or once validate.eval_timeout seconds pass without a new checkpoint.  `--checkpoint PREFIX` evaluates one prefix and exits.
+
+Per checkpoint the trainer's restore path (ParamStore.restore_checkpoint, with its name, shape, dtype and checksum checks)
+fills a ParamStore(task="vcr"), and the downstream.mode tower is evaluated through vcr_model_fn_builder's "eval" mode on
+the first validate.eval_samples // device.val_batch_size batches of the evaluation input (vcr_input).  Like the
+reference's `steps=`, the remainder is not evaluated.  A batch can be run in chunks of `--chunk` questions: evaluation has
+no dropout and no term across questions, so the means do not change.  One JSON line per checkpoint, {global_step, avg
+(mean accuracy, the reference's metric name), loss (mean of the per-batch losses), questions}, is appended to
+output_dir/eval/results.jsonl.  `--predictions PATH.npz` (with --checkpoint) also writes, per question, annot_id, img_id,
+log_prob [4], prediction and label: the reference's cls_metric / PREDICT dict.  `--unlabelled` scores records without
+labels: forward and head only, no loss, no accuracy and no results line.
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import re
+import time
+from typing import Callable, Dict, Iterator
+
+import numpy as np
+
+RESULTS_FILE = os.path.join("eval", "results.jsonl")
+
+
+def checkpoint_step(prefix: str) -> int:
+    """The global step in a model.ckpt-<step> prefix (validate.py:48)."""
+    m = re.search(r"-(\d+)$", os.path.basename(prefix))
+    if m is None:
+        raise ValueError(f"{prefix!r} is not a model.ckpt-<global_step> prefix")
+    return int(m.group(1))
+
+
+def follow_checkpoints(directory: str, num_train_steps: int, timeout: float, poll_interval: float = 60.0,
+                       clock: Callable[[], float] = time.monotonic,
+                       sleep: Callable[[float], None] = time.sleep) -> Iterator[str]:
+    """Yield the checkpoint prefixes of `directory` (those its state file lists) as they appear, each one newer than the
+    last yielded, oldest first.  Ends after a checkpoint whose step is >= num_train_steps, or when `timeout` seconds of
+    `clock` pass after the last yield (or the start) without a new checkpoint.  Polls every `poll_interval` seconds."""
+    from .tf_checkpoint import checkpoint_prefixes
+    last = -1
+    deadline = clock() + timeout
+    while True:
+        new = sorted((checkpoint_step(p), p) for p in checkpoint_prefixes(directory) if checkpoint_step(p) > last)
+        if new:
+            for step, prefix in new:
+                yield prefix
+                last = step
+                if step >= num_train_steps:
+                    return
+            deadline = clock() + timeout
+            continue
+        if clock() >= deadline:
+            return
+        sleep(poll_interval)
+
+
+def log_softmax(logits: np.ndarray) -> np.ndarray:
+    """cls_metric's log_prob of fp32 logits [n, 4], computed in float64 and returned as float32."""
+    x = np.asarray(logits, np.float64)
+    x = x - x.max(-1, keepdims=True)
+    return (x - np.log(np.exp(x).sum(-1, keepdims=True))).astype(np.float32)
+
+
+class Validator:
+    """Evaluates checkpoints of a VCR run on the evaluation input of config (data.val_file, downstream.mode)."""
+
+    def __init__(self, config, chunk: int = 0, device="cuda"):
+        from .params import ParamStore
+        from .vcr import vcr_model_fn_builder
+        self.config = config
+        self.batch_size = int(config.device.get("val_batch_size", 64))
+        self.chunk = chunk if chunk > 0 else self.batch_size
+        self.num_batches = int(config.validate.get("eval_samples", 0)) // self.batch_size
+        if self.num_batches < 1:
+            raise ValueError(f"validate.eval_samples {config.validate.get('eval_samples')!r} is less than one batch of "
+                             f"device.val_batch_size {self.batch_size}")
+        self.store = ParamStore(config.model, device=device, optimizer_cfg=config.optimizer, task="vcr")
+        self.model_fn = vcr_model_fn_builder(config, store=self.store, device=device)
+        self.device = device
+
+    def evaluate(self, prefix: str, labelled: bool = True, keep_predictions: bool = False) -> Dict:
+        """Restore `prefix` and evaluate.  Returns {global_step, avg, loss, questions} (avg and loss None when not
+        labelled), plus per-question arrays under 'predictions' when keep_predictions."""
+        import torch
+        from . import vcr_input
+        self.store.restore_checkpoint(prefix)
+        mode = "eval" if labelled else "predict"
+        losses, correct, logits, rows = [], [], [], {"annot_id": [], "img_id": [], "label": []}
+        with torch.no_grad(), vcr_input.input_fn_builder(self.config, is_training=False, batch_size=self.batch_size,
+                                                         device=self.device, labelled=labelled) as pipe:
+            for _, batch in zip(range(self.num_batches), pipe):
+                batch_loss = torch.zeros((), dtype=torch.float32, device=self.device)
+                for a in range(0, self.batch_size, self.chunk):
+                    feats = {k: batch[k][a:a + self.chunk] for k in ("images", "lm_input", "lm_targets")}
+                    spec = self.model_fn(feats, None, mode)
+                    n = feats["lm_targets"].shape[0]
+                    if labelled:  # cls_loss gives chunk means; weigh them by the chunk's share of the batch
+                        batch_loss += spec.metrics["loss"] * (n / self.batch_size)
+                        correct.append(spec.metrics["accuracy"] * n)
+                    if keep_predictions:
+                        logits.append(spec.metrics["logits"].clone())
+                losses.append(batch_loss)
+                if keep_predictions:
+                    rows["annot_id"] += batch["annot_id"]
+                    rows["img_id"] += batch["img_id"]
+                    rows["label"].append(batch["lm_targets"].cpu().numpy())
+        questions = len(losses) * self.batch_size
+        if questions == 0:
+            raise ValueError(f"data.val_file holds no whole batch of {self.batch_size} questions")
+        res = {"global_step": self.store.global_step, "avg": None, "loss": None, "questions": questions}
+        if labelled:
+            res["avg"] = float(torch.stack(correct).sum()) / questions
+            res["loss"] = float(torch.stack(losses).mean())
+        if keep_predictions:
+            lg = torch.cat(logits).float().cpu().numpy()
+            lp = log_softmax(lg)
+            res["predictions"] = {"annot_id": np.array(rows["annot_id"]), "img_id": np.array(rows["img_id"]),
+                                  "log_prob": lp, "prediction": lp.argmax(-1).astype(np.int64),
+                                  "label": np.concatenate(rows["label"]).astype(np.int64)}
+        return res
+
+
+def append_result(output_dir: str, res: Dict) -> str:
+    """Append {global_step, avg, loss, questions} as one JSON line to output_dir/eval/results.jsonl; returns its path."""
+    path = os.path.join(output_dir, RESULTS_FILE)
+    os.makedirs(os.path.dirname(path), exist_ok=True)
+    with open(path, "a", encoding="utf-8") as f:
+        f.write(json.dumps({k: res[k] for k in ("global_step", "avg", "loss", "questions")}) + "\n")
+    return path
+
+
+def write_predictions(path: str, predictions: Dict[str, np.ndarray]) -> None:
+    np.savez(path, **predictions)
+
+
+def main(argv=None, clock: Callable[[], float] = time.monotonic, sleep: Callable[[float], None] = time.sleep):
+    """Returns the result dict of every evaluated checkpoint, in order."""
+    from .config import NeatConfig
+    ap = argparse.ArgumentParser(description="Validate VCR fine-tuning checkpoints (downstream/vcr/validate.py)")
+    ap.add_argument("config_file")
+    ap.add_argument("--checkpoint", help="evaluate this checkpoint prefix once instead of following device.output_dir")
+    ap.add_argument("--predictions", help="write per-question predictions to this .npz (needs --checkpoint)")
+    ap.add_argument("--unlabelled", action="store_true",
+                    help="the records have no labels: predictions only, no loss or accuracy (needs --predictions)")
+    ap.add_argument("--chunk", type=int, default=0, help="questions per forward (default: device.val_batch_size)")
+    ap.add_argument("--poll-interval", type=float, default=60.0, help="seconds between looks at device.output_dir")
+    args = ap.parse_args(argv)
+    if args.predictions and not args.checkpoint:
+        raise ValueError("--predictions writes one checkpoint's predictions: pass --checkpoint PREFIX")
+    if args.predictions and not args.predictions.endswith(".npz"):
+        raise ValueError(f"--predictions {args.predictions!r}: the file must be an .npz")
+    if args.unlabelled and not args.predictions:
+        raise ValueError("--unlabelled computes no metrics: pass --predictions PATH.npz")
+    if args.chunk < 0:
+        raise ValueError(f"--chunk {args.chunk} must be >= 0")
+    config = NeatConfig.from_yaml(args.config_file)
+    if config.downstream.get("task") != "vcr":
+        raise ValueError(f"downstream.task is {config.downstream.get('task')!r}, VCR validation needs 'vcr'")
+    output_dir = str(config.device["output_dir"])
+    if "://" in output_dir:
+        raise ValueError(f"device.output_dir {output_dir!r}: only local directories are supported for checkpoints")
+    import torch
+    if torch.cuda.is_available():
+        torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
+    v = Validator(config, chunk=args.chunk)
+    if args.checkpoint:
+        prefixes = iter([args.checkpoint])
+    else:
+        prefixes = follow_checkpoints(output_dir, int(config.optimizer.get("num_train_steps", 10)),
+                                      float(config.validate.get("eval_timeout", 72000)), args.poll_interval, clock, sleep)
+    results = []
+    for prefix in prefixes:
+        res = v.evaluate(prefix, labelled=not args.unlabelled, keep_predictions=bool(args.predictions))
+        if args.predictions:
+            write_predictions(args.predictions, res.pop("predictions"))
+        if not args.unlabelled:
+            path = append_result(output_dir, res)
+            print(f"{prefix}: global_step {res['global_step']} avg {res['avg']:.4f} loss {res['loss']:.4f} over "
+                  f"{res['questions']} questions -> {path}", flush=True)
+        else:
+            print(f"{prefix}: predictions of {res['questions']} questions -> {args.predictions}", flush=True)
+        results.append(res)
+    return results
+
+
+if __name__ == "__main__":
+    main()
