@@ -18,21 +18,14 @@ from merlot_b200.config import NeatConfig
 from oracle.oracle_np import process_example_np
 from tests import input_oracle as O
 from tests import tfrecord_writer as W
+from tests.gemm_exact_oracle import bf16_ulps
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _ulps(a, b):
-    """Distance in bf16 units of last place between bf16 tensors given as float32 arrays (sign-magnitude order)."""
-    def order(x):
-        bits = (np.ascontiguousarray(x, np.float32).view(np.uint32) >> 16).astype(np.int64)
-        return np.where(bits & 0x8000, -(bits & 0x7FFF), bits)
-    return np.abs(order(a) - order(b))
-
-
 def _check(got, ref, method, transform, what):
-    d = _ulps(got, ref)
+    d = bf16_ulps(got, ref)
     if method == 1 and transform != 2:
         # nearest copies one source value per pixel and the rest of the chain is elementwise: bit-exact
         assert d.max() == 0, f"{what}: {int((d > 0).sum())} elements differ"
@@ -162,7 +155,7 @@ def test_input_pipeline_batch_matches_oracle_and_trains(tmp_path, tiny_cfg):
         for k in ("input_ids", "video_src_ids", "youtube_id", "chunk_num", "mean_time", "is_eoc", "shuffled_idx_img"):
             np.testing.assert_array_equal(feats[k].cpu().numpy(), ref[k], err_msg=k)
         got = feats["images"].float().cpu().numpy()
-        d = _ulps(got, ref["images"])
+        d = bf16_ulps(got, ref["images"])
         assert d.max() <= 1 and (d > 0).mean() <= 0.005, (int(d.max()), float((d > 0).mean()))  # as in the K14 test
         model_fn = model_fn_builder(config, device="cuda")
         spec = model_fn(feats, None, "train", None)

@@ -17,22 +17,15 @@ from merlot_b200.config import NeatConfig
 from oracle import merlot_oracle as MO
 from tests import input_oracle as O
 from tests import story_records as R
+from tests.gemm_exact_oracle import bf16_ulps
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 
 
-def _ulps(a, b):
-    """Distance in bf16 units of last place between bf16 tensors given as float32 arrays (sign-magnitude order)."""
-    def order(x):
-        bits = (np.ascontiguousarray(x, np.float32).view(np.uint32) >> 16).astype(np.int64)
-        return np.where(bits & 0x8000, -(bits & 0x7FFF), bits)
-    return np.abs(order(a) - order(b))
-
-
 def _check_bilinear(got, ref, what):
     # the bar of tests/test_gpu_input.py for bilinear: at most 1 ulp, in at most 0.5% of the elements
-    d = _ulps(got, ref)
+    d = bf16_ulps(got, ref)
     assert d.max() <= 1, f"{what}: max {int(d.max())} ulp"
     assert (d > 0).mean() <= 0.005, f"{what}: {(d > 0).mean():.4f} of the elements differ"
 
