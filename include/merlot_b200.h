@@ -218,6 +218,15 @@ int merlot_softmax_ce_fwd(const float* logits, int ld, const int* labels, int ro
                           float* correct, void* stream);
 int merlot_softmax_ce_bwd(const float* logits, int ld, const int* labels, int rows, int C, const float* lse,
                           const float* coeff, void* dlogits, int dlogits_f32, int ld_d, void* stream);
+/* K16 operands of the contrastive head (model/modeling.py:491-526) on K1 with a three-term bf16 split, x = xh + xl:
+ * ctr_split: fp32 x [rows, C] (row stride ldx) -> bf16 out[s*seg_stride + r*ld + c] = (bit s of lo_mask ? xl : xh), s = 0..2
+ *   (seg_stride = C: the three segments side by side along K; seg_stride = rows*ld: stacked).
+ * ctr_dlogits: dS = scale*coeff[r]*(softmax(logits[r]) - onehot(labels[r])) with the lse of softmax_ce_fwd, as bf16 hi/lo:
+ *   dsh [rows, ld_h >= 3C] row r = [dSh | dSh | dSl];  dsv [3 rows, ld_v >= C] = [dSh ; dSh ; dSl]. */
+int merlot_ctr_split(const float* x, int rows, int C, int ldx, void* out, long long ld, long long seg_stride, int lo_mask,
+                     void* stream);
+int merlot_ctr_dlogits(const float* logits, int ld, const int* labels, int rows, int C, const float* lse,
+                       const float* coeff, float scale, void* dsh, int ld_h, void* dsv, int ld_v, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Transformer stack driver (utils/transformer.py:171-247 `transformer`, pre-LN; forward and explicit backward).

@@ -65,6 +65,26 @@ class NeatConfig(object):
         return cls.from_yaml(args.config_file)
 
 
+def micro_batching(device_config: dict, world: int, default_batch_size: int = 8):
+    """(A, m): every rank runs A micro-batches of m examples per optimizer step.  Without `device.micro_batch_size` this is
+    (1, train_batch_size // world), one batch per step.  With it, m = micro_batch_size and train_batch_size must equal
+    world * A * m for an integer A >= 1, so that the step is the data-parallel step of world * A (virtual) replicas."""
+    tbs = int(device_config.get("train_batch_size", default_batch_size))
+    m = device_config.get("micro_batch_size")
+    if m is None:
+        return 1, max(1, tbs // world)
+    m = int(m)
+    if m < 1 or tbs % (world * m) != 0 or tbs < world * m:
+        raise ValueError(f"train_batch_size {tbs} is not world {world} x A x micro_batch_size {m} for an integer A >= 1")
+    return tbs // (world * m), m
+
+
+def replica_seed(seed: int, step: int, world: int, accum: int, rank: int, micro: int) -> int:
+    """Dropout / masking seed of virtual replica v = rank * accum + micro at optimizer step `step`: seed + step*world*accum + v
+    (with accum = 1, seed + step*world + rank)."""
+    return seed + step * world * accum + rank * accum + micro
+
+
 def patch_embed_variant(model_config: dict) -> dict:
     """Return a copy of a `model:` section with the hybrid ResNet stem switched off (resnet_layers: []), i.e. the
     16x16 patch-embed path of utils/vision_transformer.py:194-205 that BASELINE.json's north star names.

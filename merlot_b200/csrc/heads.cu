@@ -1,6 +1,6 @@
 // Small kernels for the three loss heads (model/modeling.py:491-668): index/label construction (integer, bit-exact),
-// weighted loss reductions with their backward coefficients, and a tiny fp32 matmul for the 32 x (32*world)
-// contrastive logits.  None of these is performance critical (<0.1 % of a step); they exist so that the whole loss path
+// weighted loss reductions with their backward coefficients, and a tiny strided fp32 matmul (the VCR head's logit moves;
+// the contrastive head runs on K16, contrastive.cu).  None of these is performance critical (<0.1 % of a step); they exist so that the whole loss path
 // stays on the device, stream-ordered, with no host round trip.
 #include "host_common.h"
 #include "ptx.cuh"

@@ -37,6 +37,7 @@ from typing import Dict, Iterator, List, Optional, Sequence
 import numpy as np
 import torch
 
+from .config import micro_batching
 from .tfrecord import parse_example, read_records
 
 SHUFFLE_OFFSET = 16  # model/dataloader.py:227
@@ -437,8 +438,9 @@ def input_fn_builder(config, is_training: bool = True, rank: int = 0, world: int
                      batch_size: Optional[int] = None, device=None) -> InputPipeline:
     """model/dataloader.py:129-278 for training: the files of data.train_file (sharded by rank when world > 1), interleaved
     over min(num_threads, files) readers, a shuffle buffer of shuffle_buffer_size records, the parser, batches of
-    `batch_size` (default device.train_batch_size // world) with drop_remainder, and `process_example`.  Returns the
-    running pipeline (an iterator of feature dicts; close() it)."""
+    `batch_size` (default: the micro-batch of config.micro_batching, device.train_batch_size // world without
+    device.micro_batch_size) with drop_remainder, and `process_example`.  Returns the running pipeline (an iterator of
+    feature dicts; close() it)."""
     if not is_training:
         raise NotImplementedError("only the training input is provided (val_file / eval input is not)")
     if config.data.get("unbatch_size", 1) > 1:
@@ -448,5 +450,5 @@ def input_fn_builder(config, is_training: bool = True, rank: int = 0, world: int
         raise ValueError(f"data.train_file {config.data.get('train_file')!r} matches no file")
     files = shard_files(files, rank, world)
     if batch_size is None:
-        batch_size = max(1, config.device.get("train_batch_size", 8) // world)
+        batch_size = micro_batching(config.device, world)[1]
     return InputPipeline(config, files, batch_size, rank=rank, seed=seed, device=device)

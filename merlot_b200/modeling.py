@@ -163,15 +163,26 @@ class MerlotModel(object):
     def __init__(self, config, is_training, use_tpu, image, input_ids, mask_input=False, shuffled_idx_img=None,
                  img_mask=None, log_attention_probs=True, *, params: ParamStore, mask_draws: Optional[Dict] = None,
                  mask_override: Optional[Dict] = None, dropout_seed: int = 0, save_for_backward: Optional[bool] = None,
-                 dist=None, export_attention_probs: bool = False, frame_copies: int = 1):
+                 dist=None, export_attention_probs: bool = False, frame_copies: int = 1, features_only: bool = False):
         """Arguments as model/modeling.py:48-66.  `use_tpu` is accepted and ignored (it only selects one-hot vs gather
         embedding lookups in the reference, utils/model_utils.py:259-263 -- same values either way).
 
         `frame_copies` = c > 1 is the evaluation forward of c copies of every group that share their frames (zero-shot story
         unshuffling scores two shuffles of each story, downstream/sort_story/get_zero_shot_logits.py:44-56): `image` holds
         batch_size // c groups of frames, `input_ids` and `shuffled_idx_img` hold batch_size groups, copy d of group s at
-        s*c + d.  The ViT runs once per group of frames; each copy assembles its own viz tokens with its own image indices."""
+        s*c + d.  The ViT runs once per group of frames; each copy assembles its own viz tokens with its own image indices.
+
+        `features_only` runs what contrastive_features() needs and nothing more: the ViT, the language-only encoder and
+        mask_inputs (with the dropout of is_training), but not the joint encoder, and it allows no backward.  The
+        first pass of a gradient-accumulation step (train.model_fn_builder) computes every micro-batch's features this way."""
         frame_copies = int(frame_copies)
+        if features_only and not mask_input:
+            raise ValueError("features_only needs mask_input=True: the language features come from the language-only encoder")
+        if features_only and save_for_backward:
+            raise ValueError("features_only saves nothing for backward")
+        self.features_only = bool(features_only)
+        if features_only:
+            save_for_backward = False
         if frame_copies < 1:
             raise ValueError(f"frame_copies must be >= 1, got {frame_copies}")
         if frame_copies > 1 and (is_training or mask_input or save_for_backward or config.get("num_texts", 1) > 1):
@@ -217,6 +228,9 @@ class MerlotModel(object):
             cfg["hidden_dropout_prob"] = 0.0
             cfg["attention_probs_dropout_prob"] = 0.0
         self._save = bool(is_training) if save_for_backward is None else bool(save_for_backward)
+        # features_only writes into the training forward's activation arenas (the next training forward overwrites them), so
+        # that a features-only pass takes no memory of its own
+        self._save_arenas = self._save or self.features_only
         self._seed = int(dropout_seed)
         self._bufs = _Buffers(params)
         self._mask_input = mask_input
@@ -317,7 +331,7 @@ class MerlotModel(object):
         else:  # hybrid stem (:206-223): lite_resnet50 -> 1x1 conv_postresnet_proj with bias (not standardised)
             if Pp != 16:
                 raise ValueError("the hybrid ResNet stem needs patch_size 16 (utils/vision_transformer.py:208)")
-            self._stem = HybridStem(st, bf, self._resnet_layers, self._save)
+            self._stem = HybridStem(st, bf, self._resnet_layers, self._save_arenas)
             self._rc, hs, ws_ = self._stem.forward(img, N, h0, w0)
             if (hs, ws_) != (h1, w1):
                 raise ValueError(f"stem output {hs}x{ws_} != patch grid {h1}x{w1}")
@@ -330,7 +344,7 @@ class MerlotModel(object):
                                   bf.get("vit.rstd0", (Mv,), torch.float32))
         self._vit_ln.forward(h0_v)
         self._vit = _Stack(st, bf, "vit", vt, cfg.get("num_vision_transformer_hidden_layers", cfg["num_hidden_layers"]), N, Sv,
-                           None, h0_v, cfg, p_vit, self._seed, _SITE_VIT, self._save)
+                           None, h0_v, cfg, p_vit, self._seed, _SITE_VIT, self._save_arenas)
         hv = self._vit.forward()
 
         # ---- viz tokens (:95-133) ----
@@ -370,6 +384,9 @@ class MerlotModel(object):
         else:
             ids_to_use = ids_bl
         self._ids_j = ids_to_use.contiguous()
+        self._heads = {}
+        if self.features_only:
+            return
 
         # ---- joint encoder (:143-184) ----
         self._emb_j_ln = self._embed_words_into(self._ids_j, "position_embeddings", "emb_j", _SITE_EMB_J, joint_in, remap=(Lj, Sj, Pz))
@@ -399,7 +416,6 @@ class MerlotModel(object):
             self.encoder_info["self_attn_probs"] = probs_j.permute(1, 0, 2, 3)
         self._hidden_f32 = {}
         self.encoder_pieces = [{"name": "viz", "start": 0, "end": Pz}, {"name": "lang", "start": Pz, "end": Sj}]
-        self._heads = {}
 
     def _side_stream(self):
         """Stream for the language-only stack (set MERLOT_NO_SIDE_STREAM=1 to serialise everything on one stream)."""
@@ -460,7 +476,7 @@ class MerlotModel(object):
         if self._export_probs:
             probs_lo = bf.get("lo.probs", (cfg["num_lang_transformer_hidden_layers"], Blo, Llo, Llo), torch.float32)
         self._lo = _Stack(st, bf, "lo", "encoder", cfg["num_lang_transformer_hidden_layers"], Blo, Llo, valid, h0, cfg, p,
-                          self._seed, _SITE_LANGONLY, self._save, colsum=summ, probs=probs_lo)
+                          self._seed, _SITE_LANGONLY, self._save_arenas, colsum=summ, probs=probs_lo)
         y = self._lo.forward()
         nch = self.batch_size * self.num_chunks
         pool_idx = bf.get("lo.pool_idx", (nch,), torch.int32)
@@ -674,65 +690,30 @@ class MerlotModel(object):
         d_inp = self._dense_bwd(t["tag"], t["inp"], f"contrastive/{t['name']}", d_proj)
         return self._mlp_ln_bwd(t["inter"], d_inp) if t["inter"] else d_inp
 
+    def contrastive_features(self):
+        """The l2-normalised lang / viz projections (project_and_norm, :18-44) of this batch, fp32 [n, Cs] each: what
+        contrastive_loss compares.  The tensors are buffers the next model on the same ParamStore overwrites."""
+        lang = self._tower("ctr.lang", self.lang_trg_h, "lang_proj")
+        viz = self._tower("ctr.viz", self.img_trg_h, "viz_proj")
+        return lang, viz
+
     def contrastive_loss(self):
         """contrastive_loss (:491-526).  Multi-GPU: features are all-gathered over the data-parallel group
         (tpu_cross_replica_stack, utils/model_utils.py:673-707) and labels are offset by rank*N (:519)."""
-        cfg, bf = self.config, self._bufs
-        lang = self._tower("ctr.lang", self.lang_trg_h, "lang_proj")
-        viz = self._tower("ctr.viz", self.img_trg_h, "viz_proj")
-        n, Cs = lang["n"], lang["Cs"]
-        world, rank = (self.dist.world, self.dist.rank) if self.dist is not None else (1, 0)
-        if world > 1:
-            all_lang, all_viz = self.dist.all_gather_rows(lang["feat"]), self.dist.all_gather_rows(viz["feat"])
-        else:
-            all_lang, all_viz = lang["feat"], viz["feat"]
-        temp = cfg.get("contrast_temp", 0.05)
-        coef = cfg.get("contrast_coef", 1.0)
-        labels = bf.get("ctr.labels", (n,), torch.int32)
-        labels.copy_(torch.arange(n, dtype=torch.int32, device=labels.device) + rank * n)
-        nW = n * world
-        outs, out2s = {}, {}
-        info = dict(lang=lang, viz=viz, all_lang=all_lang, all_viz=all_viz, labels=labels, nW=nW, temp=temp, dirs={})
-        for name, x, y in (("lang_to_viz", lang["feat"], all_viz), ("viz_to_lang", viz["feat"], all_lang)):
-            logits = bf.get(f"ctr.{name}.logits", (n, nW), torch.float32)
-            ops.small_gemm(x, Cs, 1, y, Cs, 1, logits, n, nW, Cs, alpha=1.0 / temp)
-            per, lse = bf.get(f"ctr.{name}.l", (n,), torch.float32), bf.get(f"ctr.{name}.lse", (n,), torch.float32)
-            ops.softmax_ce_fwd(logits, labels, nW, per, lse, None)
-            out2 = bf.get(f"ctr.{name}.out", (2,), torch.float32)
-            coeff = bf.get(f"ctr.{name}.coeff", (n,), torch.float32)
-            ops.weighted_loss(per, None, None, None, 0, coef / 2.0, out2, coeff)
-            outs[name], out2s[name] = out2[0], out2
-            info["dirs"][name] = dict(logits=logits, lse=lse, coeff=coeff)
-        loss_all = bf.get("ctr.loss_all", (1,), torch.float32)
-        ops.axpby(out2s["lang_to_viz"][:1], loss_all, coef / 2.0, 0.0)
-        ops.axpby(out2s["viz_to_lang"][:1], loss_all, coef / 2.0, 1.0)
-        outs["loss_all"] = loss_all[0]
+        lang, viz = self.contrastive_features()
+        info, outs = contrastive_head(self._bufs, self.config, self.dist, lang["feat"], viz["feat"], lang["n"])
+        info.update(lang=lang, viz=viz)
         self._heads["ctr"] = info
-        return loss_all[0], outs
+        return outs["loss_all"], outs
 
     def _contrastive_bwd(self, d_lang_trg, d_img_trg):
-        bf = self._bufs
         c = self._heads["ctr"]
-        lang, viz, nW, temp = c["lang"], c["viz"], c["nW"], c["temp"]
-        n, Cs = lang["n"], lang["Cs"]
-        world = self.dist.world if self.dist is not None else 1
-        d_feat = {"lang": bf.get("ctr.d_feat.lang", (n, Cs), torch.float32), "viz": bf.get("ctr.d_feat.viz", (n, Cs), torch.float32)}
-        d_all = {"lang": bf.get("ctr.d_all.lang", (nW, Cs), torch.float32), "viz": bf.get("ctr.d_all.viz", (nW, Cs), torch.float32)}
-        for name, xk, yk, y_all in (("lang_to_viz", "lang", "viz", c["all_viz"]), ("viz_to_lang", "viz", "lang", c["all_lang"])):
-            d = c["dirs"][name]
-            dlog = bf.get(f"ctr.{name}.dlogits", (n, nW), torch.float32)
-            ops.softmax_ce_bwd(d["logits"], c["labels"], nW, d["lse"], d["coeff"], dlog)
-            x = c[xk]["feat"]
-            # d_x[i,c] = sum_j dlog[i,j] y_all[j,c] / temp
-            ops.small_gemm(dlog, nW, 1, y_all, 1, Cs, d_feat[xk], n, Cs, nW, alpha=1.0 / temp, beta=0.0)
-            # d_y_all[j,c] = sum_i dlog[i,j] x[i,c] / temp
-            ops.small_gemm(dlog, 1, nW, x, 1, Cs, d_all[yk], nW, Cs, n, alpha=1.0 / temp, beta=0.0)
-        for k in ("lang", "viz"):
-            # gradient of the gather = reduce-scatter(sum) of every rank's d_all (utils/model_utils.py:699-706)
-            mine = self.dist.reduce_scatter_rows(d_all[k]) if world > 1 else d_all[k]
-            ops.axpby(mine, d_feat[k], 1.0, 1.0)
-        dl = self._tower_bwd(lang, d_feat["lang"])
-        dv = self._tower_bwd(viz, d_feat["viz"])
+        d_feat = contrastive_head_bwd(self._bufs, self.dist, c)
+        self._towers_bwd(c["lang"], c["viz"], d_feat["lang"], d_feat["viz"], d_lang_trg, d_img_trg)
+
+    def _towers_bwd(self, lang, viz, d_lang_feat, d_viz_feat, d_lang_trg, d_img_trg):
+        dl = self._tower_bwd(lang, d_lang_feat)
+        dv = self._tower_bwd(viz, d_viz_feat)
         ops.axpby(dl, d_lang_trg, 1.0, 1.0)
         ops.axpby(dv, d_img_trg, 1.0, 1.0)
 
@@ -847,13 +828,23 @@ class MerlotModel(object):
     # ---------------------------------------------------------------------------------------------------------
     # backward of the whole model: call after mask_loss / contrastive_loss / temporal_loss (whichever are in the loss)
     # ---------------------------------------------------------------------------------------------------------
-    def backward(self, on_non_vit_grads_ready=None, vit_layer_groups=None, on_vit_group_done=None, d_hidden_state=None):
+    def backward(self, on_non_vit_grads_ready=None, vit_layer_groups=None, on_vit_group_done=None, d_hidden_state=None,
+                 d_contrastive_features=None):
         """d(lang_loss + contr_loss + temp_loss)/d(params) accumulated into store.g  (model/modeling.py:713 loss,
         utils/optimization.py:176 tf.gradients).  Order: heads -> joint encoder -> language-only encoder -> (callback: every
         gradient outside vision_backbone/vision_transformer is final; data-parallel training starts their all-reduce here)
-        -> ViT."""
+        -> ViT.
+
+        `d_contrastive_features` = (d_lang, d_viz), fp32 [n, Cs] each: the gradient of a contrastive loss computed elsewhere
+        (over the features of several micro-batches, contrastive_head) w.r.t. this batch's contrastive_features().  The
+        projection towers run forward again and backward from it, in place of this model's own contrastive_loss()."""
         if not self._save:
             raise RuntimeError("MerlotModel was built without save_for_backward (is_training=False)")
+        if d_contrastive_features is not None:
+            if "ctr" in self._heads:
+                raise ValueError("d_contrastive_features replaces this model's contrastive_loss(): do not call both")
+            if not self._mask_input:
+                raise ValueError("d_contrastive_features needs mask_input=True (the language features)")
         cfg, st, bf, D = self.config, self.store, self._bufs, self._dims
         H, B, N = self.hidden_size, self.B, D["N"]
         Sj, Pz, vcl, Sv, Mv, np_, ncls = D["Sj"], D["Pz"], D["vcl"], D["Sv"], D["Mv"], D["np"], D["ncls"]
@@ -871,6 +862,13 @@ class MerlotModel(object):
             self._mask_loss_bwd(d_yj)
         if "ctr" in self._heads:
             self._contrastive_bwd(d_lang_trg, d_img_trg)
+        if d_contrastive_features is not None:
+            lang, viz = self.contrastive_features()
+            d_l, d_v = d_contrastive_features
+            shape = (lang["n"], lang["Cs"])
+            if tuple(d_l.shape) != shape or tuple(d_v.shape) != shape or d_l.dtype != torch.float32 or d_v.dtype != torch.float32:
+                raise ValueError(f"d_contrastive_features must be two fp32 {list(shape)} tensors")
+            self._towers_bwd(lang, viz, d_l.contiguous(), d_v.contiguous(), d_lang_trg, d_img_trg)
         if "tmp" in self._heads:
             self._temporal_bwd(d_yj)
         # ---- language-only encoder backward on the side stream: it needs only d_lang_trg (contrastive head) and runs
@@ -946,3 +944,86 @@ class MerlotModel(object):
             j = torch.arange(nw, device=self.store.device)[None]
             d[key] = (i * 64 + j).reshape(-1).to(torch.int32)
         return d[key]
+
+
+def _pad8(k: int) -> int:
+    return (k + 7) // 8 * 8
+
+
+def contrastive_head(bufs: _Buffers, cfg: dict, dist, lang_feat, viz_feat, per_replica: int):
+    """The contrastive loss (:491-526) over rows of l2-normalised features, fp32 [n, Cs]: the rows of this rank, made of
+    n / per_replica (virtual) replicas of `per_replica` rows each.  Features are all-gathered over the data-parallel group
+    (tpu_cross_replica_stack, utils/model_utils.py:673-707), so row i's label is rank*n + i (:519).  Every replica's loss is
+    the mean over its own rows; the backward coefficients are those of the SUM of the replicas' losses, the reported losses
+    are their mean.  Returns (info for contrastive_head_bwd, {'lang_to_viz', 'viz_to_lang', 'loss_all'} 0-d tensors).
+    The products run on K16 (csrc/contrastive.cu): K1 tensor-core GEMMs over a three-term bf16 split of the fp32 features,
+    deterministic, at any n and world."""
+    bf = bufs
+    n, Cs = lang_feat.shape
+    if n % per_replica != 0:
+        raise ValueError(f"{n} contrastive rows are not a whole number of replicas of {per_replica} rows")
+    world, rank = (dist.world, dist.rank) if dist is not None else (1, 0)
+    if world > 1:
+        all_lang, all_viz = dist.all_gather_rows(lang_feat), dist.all_gather_rows(viz_feat)
+    else:
+        all_lang, all_viz = lang_feat, viz_feat
+    temp = cfg.get("contrast_temp", 0.05)
+    coef = cfg.get("contrast_coef", 1.0)
+    labels = bf.get("ctr.labels", (n,), torch.int32)
+    labels.copy_(torch.arange(n, dtype=torch.int32, device=labels.device) + rank * n)
+    nW = n * world
+    outs, out2s = {}, {}
+    feats = {"lang": lang_feat, "viz": viz_feat}
+    if Cs % 8 != 0:
+        raise ValueError(f"contrastive_size {Cs} must be a multiple of 8 (K16's bf16 operand rows)")
+    info = dict(feats=feats, all_lang=all_lang, all_viz=all_viz, labels=labels, nW=nW, temp=temp, dirs={})
+    for name, x, y in (("lang_to_viz", lang_feat, all_viz), ("viz_to_lang", viz_feat, all_lang)):
+        # K16: S = [xh | xh | xl] . [yh | yl | yh]^T / temp, one K1 GEMM over K = 3 Cs
+        xc = bf.get(f"ctr.{name}.xcat", (n, 3 * Cs), torch.bfloat16)
+        yc = bf.get(f"ctr.{name}.ycat", (nW, 3 * Cs), torch.bfloat16)
+        ops.ctr_split(x, xc, 3 * Cs, Cs, 0b100)
+        ops.ctr_split(y, yc, 3 * Cs, Cs, 0b010)
+        logits = bf.get(f"ctr.{name}.logits", (n, _pad8(nW)), torch.float32)[:, :nW]
+        ops.gemm(xc, yc, out=logits, alpha=1.0 / temp, M=n, N=nW, K=3 * Cs)
+        per, lse = bf.get(f"ctr.{name}.l", (n,), torch.float32), bf.get(f"ctr.{name}.lse", (n,), torch.float32)
+        ops.softmax_ce_fwd(logits, labels, nW, per, lse, None)
+        out2 = bf.get(f"ctr.{name}.out", (2,), torch.float32)
+        coeff = bf.get(f"ctr.{name}.coeff", (n,), torch.float32)
+        # out2[0] = mean over all rows = mean of the replicas' losses; coeff[i] = coef / (2 * per_replica)
+        ops.weighted_loss(per, None, None, None, 0, coef / 2.0 * (n // per_replica), out2, coeff)
+        outs[name], out2s[name] = out2[0], out2
+        info["dirs"][name] = dict(logits=logits, lse=lse, coeff=coeff)
+    loss_all = bf.get("ctr.loss_all", (1,), torch.float32)
+    ops.axpby(out2s["lang_to_viz"][:1], loss_all, coef / 2.0, 0.0)
+    ops.axpby(out2s["viz_to_lang"][:1], loss_all, coef / 2.0, 1.0)
+    outs["loss_all"] = loss_all[0]
+    return info, outs
+
+
+def contrastive_head_bwd(bufs: _Buffers, dist, info) -> Dict[str, torch.Tensor]:
+    """Gradient of contrastive_head's loss w.r.t. this rank's feature rows: {'lang', 'viz'} fp32 [n, Cs] buffers."""
+    bf, c = bufs, info
+    nW, temp = c["nW"], c["temp"]
+    n, Cs = c["feats"]["lang"].shape
+    world = dist.world if dist is not None else 1
+    d_feat = {"lang": bf.get("ctr.d_feat.lang", (n, Cs), torch.float32), "viz": bf.get("ctr.d_feat.viz", (n, Cs), torch.float32)}
+    d_all = {"lang": bf.get("ctr.d_all.lang", (nW, Cs), torch.float32), "viz": bf.get("ctr.d_all.viz", (nW, Cs), torch.float32)}
+    for name, xk, yk, y_all in (("lang_to_viz", "lang", "viz", c["all_viz"]), ("viz_to_lang", "viz", "lang", c["all_lang"])):
+        d = c["dirs"][name]
+        # K16: dS = coeff (softmax - onehot) / temp straight into its hi/lo operands, side by side and stacked
+        dsh = bf.get(f"ctr.{name}.dsh", (n, _pad8(3 * nW)), torch.bfloat16)
+        dsv = bf.get(f"ctr.{name}.dsv", (3 * n, _pad8(nW)), torch.bfloat16)
+        ops.ctr_dlogits(d["logits"], c["labels"], nW, d["lse"], d["coeff"], 1.0 / temp, dsh, dsv)
+        ys = bf.get(f"ctr.{name}.ystack", (3 * nW, Cs), torch.bfloat16)
+        xs = bf.get(f"ctr.{name}.xstack", (3 * n, Cs), torch.bfloat16)
+        ops.ctr_split(y_all, ys, Cs, nW * Cs, 0b010)
+        ops.ctr_split(c["feats"][xk], xs, Cs, n * Cs, 0b010)
+        # d_x = [dSh | dSh | dSl] . [yh ; yl ; yh]            (K = 3 nW)
+        ops.gemm(dsh, ys, b_mn_major=True, out=d_feat[xk], M=n, N=Cs, K=3 * nW)
+        # d_y_all = [dSh ; dSh ; dSl]^T . [xh ; xl ; xh]      (K = 3 n)
+        ops.gemm(dsv, xs, a_mn_major=True, b_mn_major=True, out=d_all[yk], M=nW, N=Cs, K=3 * n)
+    for k in ("lang", "viz"):
+        # gradient of the gather = reduce-scatter(sum) of every rank's d_all (utils/model_utils.py:699-706)
+        mine = dist.reduce_scatter_rows(d_all[k]) if world > 1 else d_all[k]
+        ops.axpby(mine, d_feat[k], 1.0, 1.0)
+    return d_feat

@@ -546,6 +546,19 @@ def small_gemm(A, sam, sak, B, sbn, sbk, Cm, M, N, K, alpha=1.0, beta=0.0):
                                   beta, _stream())
 
 
+def ctr_split(x, out, ld, seg_stride, lo_mask):
+    """K16: the fp32 rows of x as three bf16 segments of out (hi, or lo where bit s of lo_mask is set)."""
+    assert x.dtype == torch.float32 and out.dtype == torch.bfloat16 and x.stride(1) == 1
+    L.lib().merlot_ctr_split(x.data_ptr(), x.shape[0], x.shape[1], x.stride(0), out.data_ptr(), ld, seg_stride, lo_mask, _stream())
+
+
+def ctr_dlogits(logits, labels, C, lse, coeff, scale, dsh, dsv):
+    """K16: dS = scale * coeff * (softmax - onehot) as its bf16 hi/lo GEMM operands dsh [rows, >=3C] and dsv [3 rows, >=C]."""
+    assert dsh.dtype == torch.bfloat16 and dsv.dtype == torch.bfloat16
+    L.lib().merlot_ctr_dlogits(logits.data_ptr(), logits.stride(0), labels.data_ptr(), logits.shape[0], C, lse.data_ptr(),
+                               coeff.data_ptr(), scale, dsh.data_ptr(), dsh.stride(0), dsv.data_ptr(), dsv.stride(0), _stream())
+
+
 def axpby(x, y, a=1.0, b=1.0):
     L.lib().merlot_axpby_f32(x.data_ptr(), y.data_ptr(), x.numel(), a, b, _stream())
 

@@ -19,9 +19,9 @@ from typing import Dict, Optional
 
 import torch
 
-from .config import NeatConfig
+from .config import NeatConfig, micro_batching, replica_seed
 from .dataloader import input_fn_builder, train_files
-from .modeling import MerlotModel, START
+from .modeling import MerlotModel, START, _Buffers, contrastive_head, contrastive_head_bwd
 from .optimization import build_optimizer_from_config
 from .params import ParamStore
 
@@ -148,19 +148,26 @@ class StepSpec:
 
 
 def backward_and_apply(model, optimizer, dist: Optional[DataParallel], *, metrics: dict, skip=(), vit_grad_buckets: int = 4,
-                       d_hidden_state=None):
+                       d_hidden_state=None, d_contrastive_features=None, accum: int = 1):
     """The train op of every training step: model.backward (with an external head's gradient `d_hidden_state`, if any, whose
-    parameter gradients are already in store.g), the gradient mean over replicas and AdamW.  With clip_norm > 0 the pre-clip
-    global norm goes into metrics['gradnorms/_overall']."""
+    parameter gradients are already in store.g, and the injected contrastive gradient `d_contrastive_features`), the gradient
+    mean over replicas and AdamW.  With clip_norm > 0 the pre-clip global norm goes into metrics['gradnorms/_overall'].
+    `accum` = A > 1: this is the last of A micro-batches whose gradients store.g already sums, and AdamW applies the mean
+    over the world * A virtual replicas."""
     store = optimizer.store
     world = dist.world if dist is not None else 1
+    grad_scale = 1.0 / (world * accum)
+    bwd = dict(d_hidden_state=d_hidden_state, d_contrastive_features=d_contrastive_features)
     pending = []
     if optimizer.clip_norm > 0.0:  # local clip needs the complete local gradient first: no bucket overlap
-        model.backward(d_hidden_state=d_hidden_state)
+        if accum > 1:
+            raise NotImplementedError("clip_norm > 0 with gradient accumulation: the reference clips every replica's gradient "
+                                      "before the mean, which needs one gradient arena per micro-batch")
+        model.backward(**bwd)
         metrics["gradnorms/_overall"] = optimizer.clip_gradients()
         if world > 1:
             dist.all_reduce_grads(store.g)
-        optimizer.apply_gradients(grad_scale=1.0 / world, skip=skip, zero_grad=True)
+        optimizer.apply_gradients(grad_scale=grad_scale, skip=skip, zero_grad=True)
     elif world > 1:
         # Bucketed, overlapped gradient all-reduce (CrossShardOptimizer's mean, utils/optimization.py:241-245; the 1/world
         # is folded into AdamW).  Bucket 0 = everything outside the ViT, reduced while the ViT backward runs; the ViT is
@@ -177,19 +184,31 @@ def backward_and_apply(model, optimizer, dist: Optional[DataParallel], *, metric
             pending.extend(dist.all_reduce_ranges_async(store.g, store.rest_ranges))
             dist.reserve_sms(True)  # the ViT backward is enqueued (and runs) under the collectives
 
-        model.backward(on_non_vit_grads_ready=on_rest, vit_layer_groups=groups, on_vit_group_done=on_group,
-                       d_hidden_state=d_hidden_state)
+        model.backward(on_non_vit_grads_ready=on_rest, vit_layer_groups=groups, on_vit_group_done=on_group, **bwd)
         dist.reserve_sms(False)
         vit_pending.append(dist.all_reduce_ranges_async(store.g, vit_ranges[-1]))
         dist.wait_all(pending)
-        optimizer.apply_gradients(grad_scale=1.0 / world, skip=skip, zero_grad=True, only=store.rest_ranges, advance=False)
+        optimizer.apply_gradients(grad_scale=grad_scale, skip=skip, zero_grad=True, only=store.rest_ranges, advance=False)
         for k, hs in enumerate(vit_pending):
             dist.wait_all(hs)
-            optimizer.apply_gradients(grad_scale=1.0 / world, skip=skip, zero_grad=True, only=vit_ranges[k],
+            optimizer.apply_gradients(grad_scale=grad_scale, skip=skip, zero_grad=True, only=vit_ranges[k],
                                       advance=(k + 1 == len(vit_pending)))
     else:
-        model.backward(d_hidden_state=d_hidden_state)
-        optimizer.apply_gradients(grad_scale=1.0 / world, skip=skip, zero_grad=True)
+        model.backward(**bwd)
+        optimizer.apply_gradients(grad_scale=grad_scale, skip=skip, zero_grad=True)
+
+
+def accumulate_mean(bufs, acc: dict, metrics: dict, j: int, accum: int):
+    """acc[k] <- the running mean over micro-batches 0..j of accum of every tensor metric (0-d fp32 CUDA tensors, which the
+    next micro-batch's buffers overwrite); other values are copied."""
+    from . import ops
+    for k, v in metrics.items():
+        if not torch.is_tensor(v):
+            acc[k] = v
+            continue
+        t = bufs.get(f"accum.metric.{k}", (1,), torch.float32)
+        ops.axpby(v.float(), t, 1.0 / accum, 1.0 if j else 0.0)
+        acc[k] = t[0]
 
 
 def model_fn_builder(config: NeatConfig, *, store: Optional[ParamStore] = None, dist: Optional[DataParallel] = None,
@@ -197,41 +216,109 @@ def model_fn_builder(config: NeatConfig, *, store: Optional[ParamStore] = None, 
     """model/modeling.py:671-810.  `seed` is the run seed of every random draw of the step (dropout masks, Gumbel noise,
     span lengths, 10/80/10 options, replacement ids): replica r at step t uses seed + t*world + r, so replicas draw
     independently like the reference's per-core tf.random ops and two runs with different seeds differ.
-    `log_attention_probs` defaults to the reference's model_fn (modeling.py:691-709 computes attn/* every step)."""
+    `log_attention_probs` defaults to the reference's model_fn (modeling.py:691-709 computes attn/* every step).
+
+    Gradient accumulation: model_fn([f_0, ..., f_{A-1}]) with A feature dicts of one micro-batch each is the step of the
+    world * A virtual replicas v = rank * A + j, with seed + t*world*A + v (config.replica_seed).  The contrastive loss of
+    each replica is taken against the features of all world * A replicas, exactly, in two passes: model_fn runs a
+    features-only forward of every micro-batch, the contrastive head over all their features and its backward (the
+    contrastive metrics are known on return); train_op then runs, per micro-batch, the training forward again with the same
+    seed and masks, mask_loss, temporal_loss and the backward from the injected contrastive gradient.  Only the last
+    micro-batch's backward runs the bucketed all-reduce; AdamW applies the mean over the world * A replicas.  The lang/,
+    temporal/ and attn/ metrics (means over the rank's micro-batches) and the loss are complete after train_op()."""
     if store is None:
         store = ParamStore(config.model, device=device, optimizer_cfg=config.optimizer)
         store.init_reference(seed=0)
     optimizer, _ = build_optimizer_from_config(loss=None, optimizer_config=config.optimizer, device_config=config.device,
                                                store=store)
     skip = variables_without_gradient(config.model, store)
+    world, rank = (dist.world, dist.rank) if dist is not None else (1, 0)
 
-    def model_fn(features, labels=None, mode="train", params=None):
-        is_training = mode == "train"
+    def build_model(features, dropout_seed, transpose=True, **kw):
         imgs = features["images"]
-        if is_training and config.model.get("transpose_input", False) and imgs.shape[-1] != 3:
+        if transpose and config.model.get("transpose_input", False) and imgs.shape[-1] != 3:
             imgs = imgs.permute(3, 0, 1, 2).contiguous()  # [H,W,3,N] -> [N,H,W,3], modeling.py:683-685
-        model = MerlotModel(config=config.model, is_training=True,  # the reference hard-codes True (:693, SURVEY quirk 3)
-                            image=imgs, input_ids=features["input_ids"], use_tpu=config.device.get("use_tpu", False),
-                            shuffled_idx_img=features.get("shuffled_idx_img", None), mask_input=True, params=store,
-                            dropout_seed=seed + store.global_step * (dist.world if dist is not None else 1) +
-                            (dist.rank if dist is not None else 0), dist=dist, log_attention_probs=log_attention_probs)
-        lang_loss, lang_losses = model.mask_loss()
-        contr_loss, contr_losses = model.contrastive_loss()
+        return MerlotModel(config=config.model, is_training=True,  # the reference hard-codes True (:693, SURVEY quirk 3)
+                           image=imgs, input_ids=features["input_ids"], use_tpu=config.device.get("use_tpu", False),
+                           shuffled_idx_img=features.get("shuffled_idx_img", None), mask_input=True, params=store,
+                           dropout_seed=dropout_seed, dist=dist, **kw)
+
+    def temporal_loss(model, features):
         if config.model.get("temporal_coef", 1.0) > 0.0:
-            temp_loss, temp_losses = model.temporal_loss(features["shuffled_idx_img"], video_src_ids=features["video_src_ids"])
-        else:
-            temp_loss, temp_losses = torch.zeros((), device=store.device), {}
+            return model.temporal_loss(features["shuffled_idx_img"], video_src_ids=features["video_src_ids"])
+        return torch.zeros((), device=store.device), {}
+
+    def metrics_of(model, lang_losses, contr_losses, temp_losses):
         losses = {f"lang/{k}": v for k, v in lang_losses.items()}
         losses.update({f"contr/{k}": v for k, v in contr_losses.items()})
         losses.update({f"temporal/{k}": v for k, v in temp_losses.items()})
         losses["learning_rate"] = optimizer.current_lr()
         if log_attention_probs:  # modeling.py:709  losses.update(model.attention_log)
             losses.update({f"attn/{k}": v for k, v in model.attention_log.items()})
+        return losses
+
+    def model_fn(features, labels=None, mode="train", params=None):
+        if isinstance(features, (list, tuple)):
+            return accumulated_step(list(features))
+        model = build_model(features, seed + store.global_step * world + rank, transpose=mode == "train",
+                            log_attention_probs=log_attention_probs)
+        lang_loss, lang_losses = model.mask_loss()
+        contr_loss, contr_losses = model.contrastive_loss()
+        temp_loss, temp_losses = temporal_loss(model, features)
+        losses = metrics_of(model, lang_losses, contr_losses, temp_losses)
 
         def train_op():
             backward_and_apply(model, optimizer, dist, metrics=losses, skip=skip, vit_grad_buckets=vit_grad_buckets)
 
         return StepSpec(model, (lang_loss, contr_loss, temp_loss), losses, train_op)
+
+    def accumulated_step(micro):
+        A = len(micro)
+        if A < 1:
+            raise ValueError("model_fn needs at least one micro-batch")
+        if optimizer.clip_norm > 0.0 and A > 1:
+            raise NotImplementedError("clip_norm > 0 with gradient accumulation: the reference clips every replica's gradient "
+                                      "before the mean, which needs one gradient arena per micro-batch")
+        bufs = _Buffers(store)
+        seeds = [replica_seed(seed, store.global_step, world, A, rank, j) for j in range(A)]
+        # pass 1: every micro-batch's normalised features into rows [j*n, (j+1)*n) of the step's feature buffers
+        masks, feat = [], None
+        for j, f in enumerate(micro):
+            m1 = build_model(f, seeds[j], features_only=True, log_attention_probs=False)
+            lang, viz = m1.contrastive_features()
+            n, Cs = lang["n"], lang["Cs"]
+            if feat is None:
+                feat = {k: bufs.get(f"accum.feat.{k}", (A * n, Cs), torch.float32) for k in ("lang", "viz")}
+            feat["lang"][j * n:(j + 1) * n].copy_(lang["feat"])
+            feat["viz"][j * n:(j + 1) * n].copy_(viz["feat"])
+            # kept, not redrawn: mask_inputs' attention sums use float atomics, so a second draw may pick other tokens
+            masks.append({k: v.clone() for k, v in m1.lang_mask_info.items()})
+        info, contr_losses = contrastive_head(bufs, config.model, dist, feat["lang"], feat["viz"], n)
+        d_feat = contrastive_head_bwd(bufs, dist, info)
+        metrics = {f"contr/{k}": v for k, v in contr_losses.items()}
+        loss_parts = []
+
+        def train_op():
+            acc = {}
+            for j, f in enumerate(micro):
+                m2 = build_model(f, seeds[j], mask_override=masks[j], log_attention_probs=log_attention_probs)
+                lang_loss, lang_losses = m2.mask_loss()
+                temp_loss, temp_losses = temporal_loss(m2, f)
+                mj = metrics_of(m2, lang_losses, {}, temp_losses)
+                mj.update(_lang=lang_loss, _temp=temp_loss)
+                accumulate_mean(bufs, acc, mj, j, A)
+                dc = (d_feat["lang"][j * n:(j + 1) * n], d_feat["viz"][j * n:(j + 1) * n])
+                if j + 1 < A:
+                    m2.backward(d_contrastive_features=dc)  # store.g accumulates: every gradient writer adds
+                else:
+                    backward_and_apply(m2, optimizer, dist, metrics=metrics, skip=skip, vit_grad_buckets=vit_grad_buckets,
+                                       d_contrastive_features=dc, accum=A)
+            loss_parts[:] = [acc.pop("_lang"), contr_losses["loss_all"], acc.pop("_temp")]
+            metrics.update(acc)
+
+        spec = StepSpec(None, loss_parts, metrics, train_op)
+        spec.mask_info = masks  # lang_mask_info of every micro-batch, as pass 1 drew it
+        return spec
 
     model_fn.store = store
     model_fn.optimizer = optimizer
@@ -268,7 +355,11 @@ def main(argv=None):
     init_checkpoint) and training continues from its global_step to num_train_steps.  model.ckpt-<global_step> is written
     whenever global_step is a multiple of device.iterations_per_loop (default 1000) and after the last step, and every
     checkpoint is kept.  Rank 0 writes; all ranks then meet at a barrier.  The input pipeline's position is not saved: a
-    resumed run seeds it with the restored global_step so that it does not replay the first batches."""
+    resumed run seeds it with the restored global_step so that it does not replay the first batches.
+
+    With device.micro_batch_size every rank draws A = train_batch_size / (world * micro_batch_size) micro-batches per
+    optimizer step and accumulates their gradients (config.micro_batching, model_fn_builder); global_step, the learning-rate
+    schedule and the checkpoints count optimizer steps."""
     config = NeatConfig.from_args("Train MERLOT (H100-native)", argv=argv)
     output_dir = str(config.device["output_dir"])
     if "://" in output_dir:
@@ -300,7 +391,7 @@ def main(argv=None):
         if dist is not None:
             dist.barrier()
 
-    per_rank = max(1, config.device.get("train_batch_size", 8) // world)
+    accum, per_rank = micro_batching(config.device, world)  # A micro-batches of per_rank examples per step and rank
     pipeline = None
     if train_files(config.data):
         from . import vcr_input
@@ -313,10 +404,10 @@ def main(argv=None):
     try:
         for step in range(store.global_step, num_steps):
             if pipeline is not None:
-                feats = next(pipeline)
+                feats = [next(pipeline) for _ in range(accum)]
             else:
-                feats = make_batch(config, per_rank, seed=step + rank * 100003)
-            spec = model_fn(feats, None, "train", None)
+                feats = [make_batch(config, per_rank, seed=step * accum + j + rank * 100003) for j in range(accum)]
+            spec = model_fn(feats[0] if accum == 1 else feats, None, "train", None)
             spec.train_op()
             if step % 10 == 0 and rank == 0:
                 print(f"step {step} loss {spec.loss:.4f} lr {spec.metrics['learning_rate']:.3e}", flush=True)

@@ -207,10 +207,16 @@ def vcr_model_fn_builder(config, *, store=None, dist=None, seed: int = 0, device
         records: the CE kernel is not run.
     `store=None` builds ParamStore(task="vcr"), applies the reference initialisers and then `model.init_checkpoint` if set
     (restore by name, model/modeling.py:724-740: the towers keep their initial values; a missing checkpoint raises).  The
-    dropout seed of a step follows the pretraining rule: seed + step * world + rank."""
+    dropout seed of a step follows the pretraining rule: seed + step * world + rank.
+
+    Gradient accumulation: model_fn([f_0, ..., f_{A-1}]) in training, A feature dicts of one micro-batch each, returns a
+    step whose train_op runs forward, head and backward of every micro-batch in turn (the VCR loss has no term across
+    questions), with dropout seed seed + step*world*A + rank*A + j, then one AdamW step over the mean of the world * A
+    micro-batch gradients.  Its metrics, the means over the rank's micro-batches, are complete after train_op()."""
+    from .config import replica_seed
     from .optimization import build_optimizer_from_config
     from .params import ParamStore
-    from .train import StepSpec, backward_and_apply
+    from .train import StepSpec, accumulate_mean, backward_and_apply
     m_cfg = config.model
     if store is None:
         store = ParamStore(m_cfg, device=device, optimizer_cfg=config.optimizer, task="vcr")
@@ -226,7 +232,46 @@ def vcr_model_fn_builder(config, *, store=None, dist=None, seed: int = 0, device
                                                store=store)
     eval_mode = config.downstream.get("mode", "answer")
 
+    def accumulated_step(micro, labels):
+        A = len(micro)
+        if optimizer.clip_norm > 0.0 and A > 1:
+            raise NotImplementedError("clip_norm > 0 with gradient accumulation: the reference clips every replica's gradient "
+                                      "before the mean, which needs one gradient arena per micro-batch")
+        world, rank = (dist.world, dist.rank) if dist is not None else (1, 0)
+        p = float(m_cfg.get("hidden_dropout_prob", 0.0) or 0.0)
+        metrics = {"learning_rate": optimizer.current_lr()}
+        loss_parts = []
+
+        def train_op():
+            acc = {}
+            for j, f in enumerate(micro):
+                imgs = f["images"]
+                if m_cfg.get("transpose_input", False) and imgs.shape[-1] != 3:
+                    imgs = imgs.permute(3, 0, 1, 2).contiguous()
+                target = (labels[j] if labels else f)["lm_targets"]
+                step_seed = replica_seed(seed, store.global_step, world, A, rank, j)
+                model = MerlotModel(config=m_cfg, is_training=True, use_tpu=config.device.get("use_tpu", False), image=imgs,
+                                    input_ids=f["lm_input"], mask_input=False, params=store, dropout_seed=step_seed, dist=dist,
+                                    log_attention_probs=False)
+                logits = cls_head(model, store, dropout=(p, step_seed))
+                loss, accuracy = cls_loss(logits, target)
+                accumulate_mean(model._bufs, acc, {"loss": loss, "accuracy": accuracy}, j, A)
+                d_hidden = cls_head_backward(model, store, target)
+                if j + 1 < A:
+                    model.backward(d_hidden_state=d_hidden)  # store.g accumulates: every gradient writer adds
+                else:
+                    backward_and_apply(model, optimizer, dist, metrics=metrics, vit_grad_buckets=vit_grad_buckets,
+                                       d_hidden_state=d_hidden, accum=A)
+            metrics.update(acc)
+            loss_parts[:] = [acc["loss"]]
+
+        return StepSpec(None, loss_parts, metrics, train_op)
+
     def model_fn(features, labels=None, mode="train", params=None):
+        if isinstance(features, (list, tuple)):
+            if mode != "train":
+                raise ValueError("a list of micro-batches is a training step (mode 'train')")
+            return accumulated_step(list(features), labels)
         is_training = mode == "train"
         imgs, ids = features["images"], features["lm_input"]
         target = None if mode == "predict" else (labels or features)["lm_targets"]

@@ -27,6 +27,7 @@ import numpy as np
 
 from .dataloader import (DevicePipeline, decode_jpeg, interleave_records, plan_frames, plan_frames_eval, shard_files,
                          shuffled_records, stage_frames, train_files)
+from .config import micro_batching
 from .sort_story import batch_records, val_files
 from .tfrecord import parse_example
 
@@ -213,8 +214,8 @@ class VCREvalPipeline(DevicePipeline):
 def input_fn_builder(config, is_training: bool = True, rank: int = 0, world: int = 1, seed: int = 0,
                      batch_size: Optional[int] = None, device=None, labelled: bool = True):
     """dataloader_joint.input_fn_builder(is_training=True) or dataloader.input_fn_builder(is_training=False).  Training: the
-    files of data.train_file sharded by rank (shard_files), batches of `batch_size` questions (default
-    device.train_batch_size // world).  Evaluation: the files of data.val_file in sorted glob order, the downstream.mode
+    files of data.train_file sharded by rank (shard_files), batches of `batch_size` questions (default: the micro-batch of
+    config.micro_batching, device.train_batch_size // world without device.micro_batch_size).  Evaluation: the files of data.val_file in sorted glob order, the downstream.mode
     input, batches of `batch_size` questions (default device.val_batch_size).  Returns the running pipeline (close() it)."""
     if is_training:
         files = train_files(config.data)
@@ -222,7 +223,7 @@ def input_fn_builder(config, is_training: bool = True, rank: int = 0, world: int
             raise ValueError(f"data.train_file {config.data.get('train_file')!r} matches no file")
         files = shard_files(files, rank, world)
         if batch_size is None:
-            batch_size = max(1, config.device.get("train_batch_size", 64) // world)
+            batch_size = micro_batching(config.device, world, default_batch_size=64)[1]
         return VCRTrainPipeline(config, files, batch_size, rank=rank, seed=seed, device=device)
     files = val_files(config)
     if not files:
