@@ -81,6 +81,97 @@ class _LayerNorm:
                                  **{**self.kw, **kw})
 
 
+class _Dense:
+    """tf.layers.dense `scope` on a small head tensor: bf16 rows x, fp32 accumulate and output (+bias).  Keeps x for its
+    backward; `tag` names the backward's buffers."""
+
+    def __init__(self, store, bufs, tag, scope, x):
+        self.st, self.bf, self.tag, self.scope, self.x = store, bufs, tag, scope, x
+
+    def forward(self, out):
+        st, s = self.st, self.scope
+        return ops.gemm(self.x, st.W(f"{s}/kernel"), b_mn_major=True, bias=st.P(f"{s}/bias"), out=out)
+
+    def backward(self, dy):
+        """Accumulates the kernel and bias gradients of dy fp32 [R, N]; returns d_x fp32 [R, Kin]."""
+        st, bf, s = self.st, self.bf, self.scope
+        (R, N), Kin = dy.shape, self.x.shape[1]
+        ops.bias_grad(dy, st.G(f"{s}/bias"), rows=R, N=N)
+        dyb = bf.get(f"{self.tag}.dyb.{s}", (R, N), torch.bfloat16)
+        ops.cast_f32_to_bf16(dy, dyb)
+        ops.gemm(self.x, dyb, a_mn_major=True, b_mn_major=True, out=st.G(f"{s}/kernel"), atomic=True, M=Kin, N=N, K=R)
+        dx = bf.get(f"{self.tag}.dx.{s}", (R, Kin), torch.float32)
+        return ops.gemm(dyb, st.W(f"{s}/kernel"), out=dx, M=R, N=Kin, K=N)
+
+
+class _MlpLn:
+    """dense + gelu -> layer_norm of bf16 rows x (the heads' repeated pattern, e.g. :28-35, :208-215, :582-589), run at
+    construction: bf16 output `out` [R, Hout]."""
+
+    def __init__(self, store, bufs, tag, x, dense_scope, ln_scope, Hout):
+        R = x.shape[0]
+        self.bf, self.tag = bufs, tag
+        self.dense = _Dense(store, bufs, tag, dense_scope, x)
+        self.pre = self.dense.forward(bufs.get(f"{tag}.pre", (R, Hout), torch.float32))
+        act = ops.gelu_f32(self.pre, bufs.get(f"{tag}.act", (R, Hout), torch.float32))
+        self.out = bufs.get(f"{tag}.an", (R, Hout), torch.bfloat16)
+        self.ln = _LayerNorm(store, ln_scope, act, bufs.get(f"{tag}.mean", (R,), torch.float32),
+                             bufs.get(f"{tag}.rstd", (R,), torch.float32), rows=R)
+        self.ln.forward(self.out)
+
+    def backward(self, d_out):
+        """d_out fp32 [R, Hout] -> parameter gradients accumulated, d_x fp32 [R, Hin] returned."""
+        bf, tag = self.bf, self.tag
+        d_act = self.ln.backward(d_out, bf.get(f"{tag}.d_act", self.pre.shape, torch.float32))
+        d_pre = ops.gelu_bwd_f32(d_act, self.pre, bf.get(f"{tag}.d_pre", self.pre.shape, torch.float32))
+        return self.dense.backward(d_pre)
+
+
+class _SoftmaxCE:
+    """Softmax cross entropy of fp32 logits [R, >= C] against int32 labels (ops.softmax_ce_fwd), reduced by ops.weighted_loss
+    with the caller's weights, nz_labels, denom_mode and scale into `out2` = (loss, accuracy; the accuracy only with
+    accuracy=True).  Keeps what its backward reads; `tag` names its buffers."""
+
+    def __init__(self, bufs, tag, logits, labels, C, weights=None, nz_labels=None, denom_mode=0, scale=1.0, accuracy=False):
+        R = logits.shape[0]
+        self.logits, self.labels, self.C = logits, labels, C
+        per, self.lse = bufs.get(f"{tag}.l", (R,), torch.float32), bufs.get(f"{tag}.lse", (R,), torch.float32)
+        corr = bufs.get(f"{tag}.corr", (R,), torch.float32) if accuracy else None
+        ops.softmax_ce_fwd(logits, labels, C, per, self.lse, corr)
+        self.out2, self.coeff = bufs.get(f"{tag}.out", (2,), torch.float32), bufs.get(f"{tag}.coeff", (R,), torch.float32)
+        ops.weighted_loss(per, corr, weights, nz_labels, denom_mode, scale, self.out2, self.coeff)
+
+    def backward(self, dlogits):
+        ops.softmax_ce_bwd(self.logits, self.labels, self.C, self.lse, self.coeff, dlogits)
+        return dlogits
+
+
+class _Tower:
+    """project_and_norm (:18-44) of fp32 rows x [n, H] under scope 'contrastive', run at construction: l2-normalised fp32
+    features `feat` [n, Cs]."""
+
+    def __init__(self, store, bufs, cfg, tag, x, name):
+        self.n, H = x.shape
+        self.Cs = cfg.get("contrastive_size", H)
+        self.bf, self.tag = bufs, tag
+        xb = ops.cast_f32_to_bf16(x, bufs.get(f"{tag}.xb", (self.n, H), torch.bfloat16))
+        self.inter = None
+        if cfg.get("do_projection", False):
+            self.inter = _MlpLn(store, bufs, f"{tag}.inter", xb, f"contrastive/{name}_intermediate",
+                                f"contrastive/LayerNorm_{name}_ln", self.Cs)
+        self.dense = _Dense(store, bufs, tag, f"contrastive/{name}", self.inter.out if self.inter else xb)
+        proj = self.dense.forward(bufs.get(f"{tag}.proj", (self.n, self.Cs), torch.float32))
+        self.feat = bufs.get(f"{tag}.feat", (self.n, self.Cs), torch.float32)
+        self.inv = bufs.get(f"{tag}.inv", (self.n,), torch.float32)
+        ops.l2norm_fwd(proj, self.feat, self.inv)
+
+    def backward(self, d_feat):
+        d_proj = self.bf.get(f"{self.tag}.d_proj", (self.n, self.Cs), torch.float32)
+        ops.l2norm_bwd(d_feat, self.feat, self.inv, d_proj)
+        d_in = self.dense.backward(d_proj)
+        return self.inter.backward(d_in) if self.inter else d_in
+
+
 def _layer_params(store: ParamStore, scope: str, layers: int):
     key = ("_lp", scope, layers)
     if key in store._bufs:
@@ -384,7 +475,7 @@ class MerlotModel(object):
         else:
             ids_to_use = ids_bl
         self._ids_j = ids_to_use.contiguous()
-        self._heads = {}
+        self._mlm = self._ctr = self._tmp = None  # what mask_loss / contrastive_loss / temporal_loss keep for backward()
         if self.features_only:
             return
 
@@ -567,69 +658,27 @@ class MerlotModel(object):
     # ---------------------------------------------------------------------------------------------------------
     # heads
     # ---------------------------------------------------------------------------------------------------------
-    def _dense_f32(self, x_bf16, scope, out):
-        """tf.layers.dense on a small head tensor: bf16 operands, fp32 accumulate/output (+bias)."""
-        st = self.store
-        return ops.gemm(x_bf16, st.W(f"{scope}/kernel"), b_mn_major=True, bias=st.P(f"{scope}/bias"), out=out)
-
-    def _mlp_ln(self, tag, x_bf16, dense_scope, ln_scope, R, Hout):
-        """dense + gelu -> layer_norm (the repeated head pattern, e.g. :28-35, :208-215, :582-589). Returns bf16 output."""
-        st, bf = self.store, self._bufs
-        pre = bf.get(f"{tag}.pre", (R, Hout), torch.float32)
-        self._dense_f32(x_bf16, dense_scope, pre)
-        act = bf.get(f"{tag}.act", (R, Hout), torch.float32)
-        ops.gelu_f32(pre, act)
-        an = bf.get(f"{tag}.an", (R, Hout), torch.bfloat16)
-        ln = _LayerNorm(st, ln_scope, act, bf.get(f"{tag}.mean", (R,), torch.float32), bf.get(f"{tag}.rstd", (R,), torch.float32),
-                        rows=R)
-        ln.forward(an)
-        return dict(x=x_bf16, pre=pre, an=an, ln=ln, dense=dense_scope, R=R, Hout=Hout, tag=tag)
-
-    def _mlp_ln_bwd(self, t, d_an_f32, need_dx=True):
-        """Backward of _mlp_ln: accumulates parameter grads, returns d_x fp32 [R, Hin]."""
-        bf = self._bufs
-        R, Hout, tag = t["R"], t["Hout"], t["tag"]
-        d_act = t["ln"].backward(d_an_f32, bf.get(f"{tag}.d_act", (R, Hout), torch.float32))
-        d_pre = bf.get(f"{tag}.d_pre", (R, Hout), torch.float32)
-        ops.gelu_bwd_f32(d_act, t["pre"], d_pre)
-        return self._dense_bwd(tag, t["x"], t["dense"], d_pre, need_dx)
-
-    def _dense_bwd(self, tag, x_bf16, scope, dy_f32, need_dx=True):
-        st, bf = self.store, self._bufs
-        R, N = dy_f32.shape
-        Kin = x_bf16.shape[1]
-        ops.bias_grad(dy_f32, st.G(f"{scope}/bias"), rows=R, N=N)
-        dyb = bf.get(f"{tag}.dyb.{scope}", (R, N), torch.bfloat16)
-        ops.cast_f32_to_bf16(dy_f32, dyb)
-        ops.gemm(x_bf16, dyb, a_mn_major=True, b_mn_major=True, out=st.G(f"{scope}/kernel"), atomic=True, M=Kin, N=N, K=R)
-        if not need_dx:
-            return None
-        dx = bf.get(f"{tag}.dx.{scope}", (R, Kin), torch.float32)
-        ops.gemm(dyb, st.W(f"{scope}/kernel"), out=dx, M=R, N=Kin, K=N)
-        return dx
-
     def lm_head(self, hidden_state):
         """lm_head (:205-224) on bf16 rows [R,H]; returns fp32 logits [R, ldV] (columns >= vocab_size are padding)."""
-        return self._lm_head("lm_pub", hidden_state.contiguous())["logits"][:, :self.vocab_size]
+        return self._lm_head("lm_pub", hidden_state.contiguous())[2][:, :self.vocab_size]
 
     def _lm_head(self, tag, pooled):
+        """Returns (the projection's _MlpLn or None, the bf16 rows hn [R, H] the output layer reads, fp32 logits [R, ldV])."""
         cfg, st, bf = self.config, self.store, self._bufs
         R, H, V = pooled.shape[0], self.hidden_size, self.vocab_size
-        t = {}
-        hn = pooled
+        proj = None
         if cfg.get("do_projection", False):
-            t = self._mlp_ln(f"{tag}.proj", pooled, "lm_head/projection", "lm_head/LayerNorm", R, H)
-            hn = t["an"]
-        ldV = (V + 63) // 64 * 64
-        logits = bf.get(f"{tag}.logits", (R, ldV), torch.float32)
+            proj = _MlpLn(st, bf, f"{tag}.proj", pooled, "lm_head/projection", "lm_head/LayerNorm", H)
+        hn = proj.out if proj else pooled
+        logits = bf.get(f"{tag}.logits", (R, (V + 63) // 64 * 64), torch.float32)
         bias = st.P("lm_head/output_bias") if cfg.get("do_bias", False) else None
         ops.gemm(hn, st.W("word_embeddings/word_embeddings"), bias=bias, out=logits, M=R, N=V, K=H)
-        return dict(proj=t, hn=hn, logits=logits, ldV=ldV)
+        return proj, hn, logits
 
     def mask_loss(self):
         """mask_loss (:528-551).  Returns (loss, {'loss','acc'}) as 0-d CUDA tensors."""
         bf = self._bufs
-        B, Lj, V = self.B, self.L, self.vocab_size
+        B, Lj = self.B, self.L
         k = self.lang_mask_info["masked_idx"].shape[1]
         nm = B * k
         rows = bf.get("mlm.rows", (nm,), torch.int32)
@@ -637,85 +686,43 @@ class MerlotModel(object):
         ops.mlm_index(self.input_ids.reshape(B, Lj), self.lang_mask_info["masked_idx"], rows, targets, B, Lj, k, self._dims["Pz"])
         pooled = bf.get("mlm.pooled", (nm, self.hidden_size), torch.bfloat16)
         ops.gather_rows(self._y_j, rows, pooled)
-        hd = self._lm_head("mlm", pooled)
-        per, lse, corr = (bf.get(f"mlm.{n}", (nm,), torch.float32) for n in ("l", "lse", "corr"))
-        ops.softmax_ce_fwd(hd["logits"], targets, V, per, lse, corr)
-        out2 = bf.get("mlm.out", (2,), torch.float32)
-        coeff = bf.get("mlm.coeff", (nm,), torch.float32)
-        ops.weighted_loss(per, corr, None, targets, 1, 1.0, out2, coeff)
-        self._heads["mlm"] = dict(rows=rows, targets=targets, pooled=pooled, lse=lse, coeff=coeff, nm=nm, **hd)
-        return out2[0], {"loss": out2[0], "acc": out2[1]}
+        proj, hn, logits = self._lm_head("mlm", pooled)
+        ce = _SoftmaxCE(bf, "mlm", logits, targets, self.vocab_size, nz_labels=targets, denom_mode=1, accuracy=True)
+        self._mlm = (rows, proj, hn, ce)
+        return ce.out2[0], {"loss": ce.out2[0], "acc": ce.out2[1]}
 
     def _mask_loss_bwd(self, d_yj):
         st, bf = self.store, self._bufs
-        h = self._heads["mlm"]
-        V, H, nm, ldV = self.vocab_size, self.hidden_size, h["nm"], h["ldV"]
-        dlog = bf.get("mlm.dlogits", (nm, ldV), torch.bfloat16)
-        ops.softmax_ce_bwd(h["logits"], h["targets"], V, h["lse"], h["coeff"], dlog)
+        rows, proj, hn, ce = self._mlm
+        V, H = self.vocab_size, self.hidden_size
+        nm, ldV = ce.logits.shape
+        dlog = ce.backward(bf.get("mlm.dlogits", (nm, ldV), torch.bfloat16))
         if self.config.get("do_bias", False):
-            gb = st.G("lm_head/output_bias")
             gb_pad = st.g[st.entries["lm_head/output_bias"].offset:st.entries["lm_head/output_bias"].offset + ldV]
             ops.bias_grad(dlog, gb_pad, rows=nm, N=ldV)
         # tied embedding: dE += dlogits^T hn ; d_hn = dlogits E
-        ops.gemm(dlog, h["hn"], a_mn_major=True, b_mn_major=True, out=st.G("word_embeddings/word_embeddings"), atomic=True,
+        ops.gemm(dlog, hn, a_mn_major=True, b_mn_major=True, out=st.G("word_embeddings/word_embeddings"), atomic=True,
                  M=V, N=H, K=nm)
         d_hn = bf.get("mlm.d_hn", (nm, H), torch.float32, zero=True)  # split-K over the 50370-long contraction
         ops.gemm(dlog, st.W("word_embeddings/word_embeddings"), b_mn_major=True, out=d_hn, atomic=True, M=nm, N=H, K=V)
-        d_pooled = self._mlp_ln_bwd(h["proj"], d_hn) if h["proj"] else d_hn
-        ops.scatter_add_rows(d_pooled, h["rows"], d_yj)
-
-    def _tower(self, tag, x_f32, name):
-        """project_and_norm (:18-44) under scope 'contrastive'."""
-        cfg, bf = self.config, self._bufs
-        n, H = x_f32.shape
-        Cs = cfg.get("contrastive_size", H)
-        xb = bf.get(f"{tag}.xb", (n, H), torch.bfloat16)
-        ops.cast_f32_to_bf16(x_f32, xb)
-        t = {}
-        inp = xb
-        if cfg.get("do_projection", False):
-            t = self._mlp_ln(f"{tag}.inter", xb, f"contrastive/{name}_intermediate", f"contrastive/LayerNorm_{name}_ln", n, Cs)
-            inp = t["an"]
-        proj = bf.get(f"{tag}.proj", (n, Cs), torch.float32)
-        self._dense_f32(inp, f"contrastive/{name}", proj)
-        feat = bf.get(f"{tag}.feat", (n, Cs), torch.float32)
-        inv = bf.get(f"{tag}.inv", (n,), torch.float32)
-        ops.l2norm_fwd(proj, feat, inv)
-        return dict(tag=tag, name=name, xb=xb, inter=t, inp=inp, feat=feat, inv=inv, n=n, Cs=Cs)
-
-    def _tower_bwd(self, t, d_feat):
-        bf = self._bufs
-        d_proj = bf.get(f"{t['tag']}.d_proj", (t["n"], t["Cs"]), torch.float32)
-        ops.l2norm_bwd(d_feat, t["feat"], t["inv"], d_proj)
-        d_inp = self._dense_bwd(t["tag"], t["inp"], f"contrastive/{t['name']}", d_proj)
-        return self._mlp_ln_bwd(t["inter"], d_inp) if t["inter"] else d_inp
+        d_pooled = proj.backward(d_hn) if proj else d_hn
+        ops.scatter_add_rows(d_pooled, rows, d_yj)
 
     def contrastive_features(self):
-        """The l2-normalised lang / viz projections (project_and_norm, :18-44) of this batch, fp32 [n, Cs] each: what
-        contrastive_loss compares.  The tensors are buffers the next model on the same ParamStore overwrites."""
-        lang = self._tower("ctr.lang", self.lang_trg_h, "lang_proj")
-        viz = self._tower("ctr.viz", self.img_trg_h, "viz_proj")
-        return lang, viz
+        """The projection towers (project_and_norm, :18-44) of this batch's lang / viz rows, as two _Tower records whose
+        `feat` fp32 [n, Cs] are the l2-normalised features contrastive_loss compares.  The tensors are buffers the next
+        model on the same ParamStore overwrites."""
+        st, bf, cfg = self.store, self._bufs, self.config
+        return (_Tower(st, bf, cfg, "ctr.lang", self.lang_trg_h, "lang_proj"),
+                _Tower(st, bf, cfg, "ctr.viz", self.img_trg_h, "viz_proj"))
 
     def contrastive_loss(self):
         """contrastive_loss (:491-526).  Multi-GPU: features are all-gathered over the data-parallel group
         (tpu_cross_replica_stack, utils/model_utils.py:673-707) and labels are offset by rank*N (:519)."""
         lang, viz = self.contrastive_features()
-        info, outs = contrastive_head(self._bufs, self.config, self.dist, lang["feat"], viz["feat"], lang["n"])
-        info.update(lang=lang, viz=viz)
-        self._heads["ctr"] = info
+        info, outs = contrastive_head(self._bufs, self.config, self.dist, lang.feat, viz.feat, lang.n)
+        self._ctr = (info, lang, viz)
         return outs["loss_all"], outs
-
-    def _contrastive_bwd(self, d_lang_trg, d_img_trg):
-        c = self._heads["ctr"]
-        d_feat = contrastive_head_bwd(self._bufs, self.dist, c)
-        self._towers_bwd(c["lang"], c["viz"], d_feat["lang"], d_feat["viz"], d_lang_trg, d_img_trg)
-
-    def _towers_bwd(self, lang, viz, d_lang_feat, d_viz_feat, d_lang_trg, d_img_trg):
-        dl = self._tower_bwd(lang, d_lang_feat)
-        dv = self._tower_bwd(viz, d_viz_feat)
-        ops.axpby(dl, d_lang_trg, 1.0, 1.0)
-        ops.axpby(dv, d_img_trg, 1.0, 1.0)
 
     def _temporal_index(self):
         bf, dev = self._bufs, self.store.device
@@ -743,9 +750,10 @@ class MerlotModel(object):
         assert list(xb.shape) == [B, self.num_chunks_in_group, self.hidden_size]
         xa2 = xa.reshape(B * n, H).to(torch.bfloat16).contiguous()
         xb2 = xb.reshape(B * n, H).to(torch.bfloat16).contiguous()
-        return self._temporal_head(f"tmp_pub.{scope_name}", scope_name, xa2, xb2)["logits"][:, :4]
+        return self._temporal_head(f"tmp_pub.{scope_name}", scope_name, xa2, xb2)[2][:, :4]
 
     def _temporal_head(self, tag, scope, xa_bf16, xb_bf16):
+        """Returns (its _MlpLn, its output _Dense, fp32 logits [B*n*n, 8])."""
         st, bf = self.store, self._bufs
         B, n, H = self.B, self.num_chunks_in_group, self.hidden_size
         _, _, idxA, idxB = self._temporal_index()
@@ -753,13 +761,16 @@ class MerlotModel(object):
         hj = bf.get(f"{tag}.hj", (R, 2 * H), torch.bfloat16)
         ops.gather_rows(xa_bf16, idxA, hj[:, :H], H=H)
         ops.gather_rows(xb_bf16, idxB, hj[:, H:], H=H)
-        t = self._mlp_ln(f"{tag}.mlp", hj, f"{scope}/intermediate", f"{scope}/LayerNorm_ln0", R, H)
-        logits = bf.get(f"{tag}.logits", (R, 8), torch.float32)
-        self._dense_f32(t["an"], f"{scope}/logits", logits)
-        return dict(tag=tag, scope=scope, hj=hj, mlp=t, logits=logits, R=R)
+        mlp = _MlpLn(st, bf, f"{tag}.mlp", hj, f"{scope}/intermediate", f"{scope}/LayerNorm_ln0", H)
+        dense = _Dense(st, bf, tag, f"{scope}/logits", mlp.out)
+        return mlp, dense, dense.forward(bf.get(f"{tag}.logits", (R, 8), torch.float32))
 
     def allpairs_temporal_labels(self, video_src_ids, shuffled_idx_img=None):
         """allpairs_temporal_labels (:598-620)."""
+        return self._temporal_labels(video_src_ids, shuffled_idx_img)[0]
+
+    def _temporal_labels(self, video_src_ids, shuffled_idx_img):
+        """(labels int32, pair weights fp32 (:635, :649-652)), [B*n*n] each."""
         bf = self._bufs
         B, n = self.B, self.num_chunks_in_group
         labels = bf.get("tmp.labels", (B * n * n,), torch.int32)
@@ -767,8 +778,7 @@ class MerlotModel(object):
         v = video_src_ids.reshape(B, n).to(torch.int32).contiguous()
         s = (shuffled_idx_img if shuffled_idx_img is not None else torch.zeros_like(v)).reshape(B, n).to(torch.int32).contiguous()
         ops.temporal_labels(v, s, labels, w, B, n)
-        self._tmp_w = w
-        return labels
+        return labels, w
 
     def temporal_loss(self, shuffled_idx_img, video_src_ids):
         """temporal_loss (:622-668)."""
@@ -779,21 +789,16 @@ class MerlotModel(object):
         h_viz = bf.get("tmp.h_viz", (B * n, H), torch.bfloat16)
         ops.gather_rows(self._y_j, idx_l, h_lang)
         ops.gather_rows(self._y_j, idx_v, h_viz)
-        labels = self.allpairs_temporal_labels(video_src_ids, shuffled_idx_img)
-        w = self._tmp_w
+        labels, w = self._temporal_labels(video_src_ids, shuffled_idx_img)
         coef = cfg.get("temporal_coef", 1.0)
         use_vv = cfg.get("image_shuffle_prob", 0) > 0  # :664-665
-        info, heads, out2s = {}, {}, {}
+        info, out2s, in_loss = {}, {}, []
         for name, xa, xb in (("lang_viz", h_lang, h_viz), ("viz_viz", h_viz, h_viz)):
-            hd = self._temporal_head(f"tmp.{name}", f"{name}_temporal", xa, xb)
-            R = hd["R"]
-            per, lse, corr = (bf.get(f"tmp.{name}.{k}", (R,), torch.float32) for k in ("l", "lse", "corr"))
-            ops.softmax_ce_fwd(hd["logits"], labels, 4, per, lse, corr)
-            out2 = bf.get(f"tmp.{name}.out", (2,), torch.float32)
-            coeff = bf.get(f"tmp.{name}.coeff", (R,), torch.float32)
-            ops.weighted_loss(per, corr, w, None, 0, coef, out2, coeff)
-            info[f"{name}_loss"], info[f"{name}_acc"], out2s[name] = out2[0], out2[1], out2
-            heads[name] = dict(lse=lse, coeff=coeff, in_loss=(name == "lang_viz" or use_vv), **hd)
+            mlp, dense, logits = self._temporal_head(f"tmp.{name}", f"{name}_temporal", xa, xb)
+            ce = _SoftmaxCE(bf, f"tmp.{name}", logits, labels, 4, weights=w, scale=coef, accuracy=True)
+            info[f"{name}_loss"], info[f"{name}_acc"], out2s[name] = ce.out2[0], ce.out2[1], ce.out2
+            if name == "lang_viz" or use_vv:
+                in_loss.append((mlp, dense, ce))
         tot = bf.get("tmp.loss", (1,), torch.float32)
         ops.axpby(out2s["lang_viz"][:1], tot, 1.0, 0.0)
         if use_vv:
@@ -801,29 +806,23 @@ class MerlotModel(object):
         info["loss"] = tot[0]
         loss = bf.get("tmp.loss_scaled", (1,), torch.float32)
         ops.axpby(tot, loss, coef, 0.0)
-        self._heads["tmp"] = dict(heads=heads, labels=labels, idx_l=idx_l, idx_v=idx_v)
+        self._tmp = in_loss
         return loss[0], info
 
     def _temporal_bwd(self, d_yj):
-        st, bf = self.store, self._bufs
+        bf = self._bufs
         B, n, H = self.B, self.num_chunks_in_group, self.hidden_size
-        t = self._heads["tmp"]
-        _, _, idxA, idxB = self._temporal_index()
+        idx_l, idx_v, idxA, idxB = self._temporal_index()
         d_hl = bf.get("tmp.d_hl", (B * n, H), torch.float32, zero=True)
         d_hv = bf.get("tmp.d_hv", (B * n, H), torch.float32, zero=True)
-        for name, da, db in (("lang_viz", d_hl, d_hv), ("viz_viz", d_hv, d_hv)):
-            hd = t["heads"][name]
-            if not hd["in_loss"]:
-                continue
-            R, scope, tag = hd["R"], hd["scope"], hd["tag"]
-            dlog = bf.get(f"{tag}.dlogits", (R, 8), torch.float32)
-            ops.softmax_ce_bwd(hd["logits"], t["labels"], 4, hd["lse"], hd["coeff"], dlog)
-            d_an = self._dense_bwd(tag, hd["mlp"]["an"], f"{scope}/logits", dlog)
-            d_hj = self._mlp_ln_bwd(hd["mlp"], d_an)  # fp32 [R, 2H]
+        # lang_viz, then viz_viz when it is in the loss
+        for (mlp, dense, ce), da, db in zip(self._tmp, (d_hl, d_hv), (d_hv, d_hv)):
+            dlog = ce.backward(bf.get(f"{dense.tag}.dlogits", ce.logits.shape, torch.float32))
+            d_hj = mlp.backward(dense.backward(dlog))  # fp32 [R, 2H]
             ops.scatter_add_rows(d_hj[:, :H], idxA, da, H=H)
             ops.scatter_add_rows(d_hj[:, H:], idxB, db, H=H)
-        ops.scatter_add_rows(d_hl, t["idx_l"], d_yj)
-        ops.scatter_add_rows(d_hv, t["idx_v"], d_yj)
+        ops.scatter_add_rows(d_hl, idx_l, d_yj)
+        ops.scatter_add_rows(d_hv, idx_v, d_yj)
 
     # ---------------------------------------------------------------------------------------------------------
     # backward of the whole model: call after mask_loss / contrastive_loss / temporal_loss (whichever are in the loss)
@@ -841,7 +840,7 @@ class MerlotModel(object):
         if not self._save:
             raise RuntimeError("MerlotModel was built without save_for_backward (is_training=False)")
         if d_contrastive_features is not None:
-            if "ctr" in self._heads:
+            if self._ctr is not None:
                 raise ValueError("d_contrastive_features replaces this model's contrastive_loss(): do not call both")
             if not self._mask_input:
                 raise ValueError("d_contrastive_features needs mask_input=True (the language features)")
@@ -858,18 +857,24 @@ class MerlotModel(object):
         d_lang_trg = None
         if self._mask_input:
             d_lang_trg = bf.get("bwd.d_lang_trg", (self.batch_size * self.num_chunks, H), torch.float32, zero=True)
-        if "mlm" in self._heads:
+        if self._mlm is not None:
             self._mask_loss_bwd(d_yj)
-        if "ctr" in self._heads:
-            self._contrastive_bwd(d_lang_trg, d_img_trg)
-        if d_contrastive_features is not None:
-            lang, viz = self.contrastive_features()
-            d_l, d_v = d_contrastive_features
-            shape = (lang["n"], lang["Cs"])
-            if tuple(d_l.shape) != shape or tuple(d_v.shape) != shape or d_l.dtype != torch.float32 or d_v.dtype != torch.float32:
-                raise ValueError(f"d_contrastive_features must be two fp32 {list(shape)} tensors")
-            self._towers_bwd(lang, viz, d_l.contiguous(), d_v.contiguous(), d_lang_trg, d_img_trg)
-        if "tmp" in self._heads:
+        if self._ctr is not None or d_contrastive_features is not None:
+            if self._ctr is not None:
+                info, lang, viz = self._ctr
+                d_feat = contrastive_head_bwd(bf, self.dist, info)
+                d_l, d_v = d_feat["lang"], d_feat["viz"]
+            else:
+                lang, viz = self.contrastive_features()
+                d_l, d_v = d_contrastive_features
+                shape = (lang.n, lang.Cs)
+                if tuple(d_l.shape) != shape or tuple(d_v.shape) != shape or d_l.dtype != torch.float32 or d_v.dtype != torch.float32:
+                    raise ValueError(f"d_contrastive_features must be two fp32 {list(shape)} tensors")
+                d_l, d_v = d_l.contiguous(), d_v.contiguous()
+            dl, dv = lang.backward(d_l), viz.backward(d_v)
+            ops.axpby(dl, d_lang_trg, 1.0, 1.0)
+            ops.axpby(dv, d_img_trg, 1.0, 1.0)
+        if self._tmp is not None:
             self._temporal_bwd(d_yj)
         # ---- language-only encoder backward on the side stream: it needs only d_lang_trg (contrastive head) and runs
         # concurrently with the joint-encoder backward below, whose small grids leave a third of the SMs idle ----
@@ -985,14 +990,10 @@ def contrastive_head(bufs: _Buffers, cfg: dict, dist, lang_feat, viz_feat, per_r
         ops.ctr_split(y, yc, 3 * Cs, Cs, 0b010)
         logits = bf.get(f"ctr.{name}.logits", (n, _pad8(nW)), torch.float32)[:, :nW]
         ops.gemm(xc, yc, out=logits, alpha=1.0 / temp, M=n, N=nW, K=3 * Cs)
-        per, lse = bf.get(f"ctr.{name}.l", (n,), torch.float32), bf.get(f"ctr.{name}.lse", (n,), torch.float32)
-        ops.softmax_ce_fwd(logits, labels, nW, per, lse, None)
-        out2 = bf.get(f"ctr.{name}.out", (2,), torch.float32)
-        coeff = bf.get(f"ctr.{name}.coeff", (n,), torch.float32)
         # out2[0] = mean over all rows = mean of the replicas' losses; coeff[i] = coef / (2 * per_replica)
-        ops.weighted_loss(per, None, None, None, 0, coef / 2.0 * (n // per_replica), out2, coeff)
-        outs[name], out2s[name] = out2[0], out2
-        info["dirs"][name] = dict(logits=logits, lse=lse, coeff=coeff)
+        ce = _SoftmaxCE(bf, f"ctr.{name}", logits, labels, nW, scale=coef / 2.0 * (n // per_replica))
+        outs[name], out2s[name] = ce.out2[0], ce.out2
+        info["dirs"][name] = ce
     loss_all = bf.get("ctr.loss_all", (1,), torch.float32)
     ops.axpby(out2s["lang_to_viz"][:1], loss_all, coef / 2.0, 0.0)
     ops.axpby(out2s["viz_to_lang"][:1], loss_all, coef / 2.0, 1.0)
@@ -1009,11 +1010,11 @@ def contrastive_head_bwd(bufs: _Buffers, dist, info) -> Dict[str, torch.Tensor]:
     d_feat = {"lang": bf.get("ctr.d_feat.lang", (n, Cs), torch.float32), "viz": bf.get("ctr.d_feat.viz", (n, Cs), torch.float32)}
     d_all = {"lang": bf.get("ctr.d_all.lang", (nW, Cs), torch.float32), "viz": bf.get("ctr.d_all.viz", (nW, Cs), torch.float32)}
     for name, xk, yk, y_all in (("lang_to_viz", "lang", "viz", c["all_viz"]), ("viz_to_lang", "viz", "lang", c["all_lang"])):
-        d = c["dirs"][name]
+        ce = c["dirs"][name]
         # K16: dS = coeff (softmax - onehot) / temp straight into its hi/lo operands, side by side and stacked
         dsh = bf.get(f"ctr.{name}.dsh", (n, _pad8(3 * nW)), torch.bfloat16)
         dsv = bf.get(f"ctr.{name}.dsv", (3 * n, _pad8(nW)), torch.bfloat16)
-        ops.ctr_dlogits(d["logits"], c["labels"], nW, d["lse"], d["coeff"], 1.0 / temp, dsh, dsv)
+        ops.ctr_dlogits(ce.logits, c["labels"], nW, ce.lse, ce.coeff, 1.0 / temp, dsh, dsv)
         ys = bf.get(f"ctr.{name}.ystack", (3 * nW, Cs), torch.bfloat16)
         xs = bf.get(f"ctr.{name}.xstack", (3 * n, Cs), torch.bfloat16)
         ops.ctr_split(y_all, ys, Cs, nW * Cs, 0b010)

@@ -286,11 +286,11 @@ def model_fn_builder(config: NeatConfig, *, store: Optional[ParamStore] = None, 
         for j, f in enumerate(micro):
             m1 = build_model(f, seeds[j], features_only=True, log_attention_probs=False)
             lang, viz = m1.contrastive_features()
-            n, Cs = lang["n"], lang["Cs"]
+            n, Cs = lang.n, lang.Cs
             if feat is None:
                 feat = {k: bufs.get(f"accum.feat.{k}", (A * n, Cs), torch.float32) for k in ("lang", "viz")}
-            feat["lang"][j * n:(j + 1) * n].copy_(lang["feat"])
-            feat["viz"][j * n:(j + 1) * n].copy_(viz["feat"])
+            feat["lang"][j * n:(j + 1) * n].copy_(lang.feat)
+            feat["viz"][j * n:(j + 1) * n].copy_(viz.feat)
             # kept, not redrawn: mask_inputs' attention sums use float atomics, so a second draw may pick other tokens
             masks.append({k: v.clone() for k, v in m1.lang_mask_info.items()})
         info, contr_losses = contrastive_head(bufs, config.model, dist, feat["lang"], feat["viz"], n)

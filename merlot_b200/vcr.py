@@ -21,7 +21,7 @@ from typing import Dict
 import torch
 
 from . import ops
-from .modeling import (MerlotModel, _SITE_VCR_ANS_HID, _SITE_VCR_ANS_IN, _SITE_VCR_RAT_HID, _SITE_VCR_RAT_IN)
+from .modeling import (MerlotModel, _SITE_VCR_ANS_HID, _SITE_VCR_ANS_IN, _SITE_VCR_RAT_HID, _SITE_VCR_RAT_IN, _SoftmaxCE)
 from .params import VCR_TOWERS
 
 # (variable scope, input-dropout site, hidden-dropout site); image 2i of a question feeds tower 0, image 2i+1 tower 1 (:79-84)
@@ -92,12 +92,12 @@ def head_from_store(store, mode: str = "answer") -> Dict[str, torch.Tensor]:
             f"{sc}/classifier_mlp1/bias": store.P(f"{sc}/classifier_mlp1/bias")[:1]}
 
 
-def _head_index(model, b: int):
-    """Per tower: int32 [4b] rows of the joint hidden state (row P of every sequence) that the tower reads, question-major
-    (row 4q + c = candidate text c of question q); plus the constant E fp32 [32, 4], E[8c, c] = 1, that moves logits between
-    a tower's padded dense(1) output and the [2b, 4] logits (see cls_head)."""
+def _head_index(model, b: int, Sj: int):
+    """Per tower: int32 [4b] rows of the joint hidden state (row P of every sequence of Sj rows) that the tower reads,
+    question-major (row 4q + c = candidate text c of question q); plus the constant E fp32 [32, 4], E[8c, c] = 1, that moves
+    logits between a tower's padded dense(1) output and the [2b, 4] logits (see cls_head)."""
     bf, dev = model._bufs, model.store.device
-    Sj, P = model._dims["Sj"], model.P
+    P = model.P
     key = ("_vcr_idx", b, Sj, P)
     if key not in bf.d:
         q = torch.arange(b, device=dev)[:, None]
@@ -122,7 +122,7 @@ def cls_head(model, store, dropout=(0.0, 0)) -> torch.Tensor:
     b, H2 = B // 8, H // 2
     p, seed = float(dropout[0]), int(dropout[1])
     bf = model._bufs
-    idx, sel = _head_index(model, b)
+    idx, sel = _head_index(model, b, Sj)
     logits = bf.get("vcr.logits", (2 * b, 8), torch.float32)  # CE reads columns [0, 4)
     saved = []
     for t, (sc, site_in, site_hid) in enumerate(_TOWERS):
@@ -143,8 +143,8 @@ def cls_head(model, store, dropout=(0.0, 0)) -> torch.Tensor:
         # concat + reshape (:124-125): logits[2q + t, c] = sum_k z[q, k] E[k, c] over z viewed as [b, 32] -- an exact
         # strided copy of column 0 (one product by 1.0, the rest by 0.0)
         ops.small_gemm(z, 32, 1, sel, 1, 4, logits[t::2], b, 4, 32)
-        saved.append(dict(x=xd, h=h, gp=gp, z=z))
-    model._heads["vcr"] = dict(logits=logits, towers=saved, b=b, p=p, seed=seed)
+        saved.append((xd, h, gp))
+    model._vcr_cls = (logits, saved, p, seed)  # what cls_head_backward reads
     return logits[:, :4]
 
 
@@ -152,39 +152,32 @@ def cls_head_backward(model, store, target: torch.Tensor) -> torch.Tensor:
     """Gradient of cls_loss(cls_head(...), target) (:133-143 over :77-127).  ACCUMULATES the towers' parameter gradients into
     store.g and returns the bf16 d_hidden_state [B*(P+L), H] for model.backward(d_hidden_state=...): non-zero only at row P of
     each sequence."""
-    hd = model._heads.get("vcr")
-    if hd is None:
+    if getattr(model, "_vcr_cls", None) is None:
         raise RuntimeError("cls_head_backward needs cls_head(model, store, ...) first")
+    logits, saved, p, seed = model._vcr_cls
     y = model.encoder_info["hidden_state"]
     B, Sj, H = y.shape
-    b, H2, p, seed, logits = hd["b"], H // 2, hd["p"], hd["seed"], hd["logits"]
+    b, H2 = logits.shape[0] // 2, H // 2
     bf = model._bufs
-    idx, sel = _head_index(model, b)
-    tgt = target.to(torch.int32).contiguous()
-    n = 2 * b
-    per, lse, coeff = (bf.get(f"vcr.{k}", (n,), torch.float32) for k in ("per", "lse", "coeff"))
-    out2 = bf.get("vcr.out2", (2,), torch.float32)
-    ops.softmax_ce_fwd(logits, tgt, 4, per, lse, None)
-    ops.weighted_loss(per, None, None, None, 0, 1.0, out2, coeff)  # coeff = 1 / img_batch_size (:142)
-    dlog = bf.get("vcr.dlogits", (n, 8), torch.float32)
-    ops.softmax_ce_bwd(logits, tgt, 4, lse, coeff, dlog)
+    idx, sel = _head_index(model, b, Sj)
+    ce = _SoftmaxCE(bf, "vcr", logits, target.to(torch.int32).contiguous(), 4)  # coeff = 1 / img_batch_size (:142)
+    dlog = ce.backward(bf.get("vcr.dlogits", (2 * b, 8), torch.float32))
     d_hidden = bf.get("vcr.d_hidden", (B * Sj, H), torch.bfloat16, zero=True)
-    for t, (sc, site_in, site_hid) in enumerate(_TOWERS):
-        s = hd["towers"][t]
+    for t, ((sc, site_in, site_hid), (x, h, gp)) in enumerate(zip(_TOWERS, saved)):
         # dz[4q + c, 0] = dlogits[2q + t, c], columns 1..7 zero: dz viewed as [b, 32] = dlogits[t::2, :4] E^T
         dz = bf.get(f"vcr.{t}.dz", (4 * b, 8), torch.float32)
         ops.small_gemm(dlog[t::2], 16, 1, sel, 4, 1, dz.view(b, 32), b, 32, 4)
         ops.bias_grad(dz, store.G(f"{sc}/classifier_mlp1/bias"), rows=4 * b, N=8)
         dzb = bf.get(f"vcr.{t}.dzb", (4 * b, 8), torch.bfloat16)
         ops.cast_f32_to_bf16(dz, dzb)
-        ops.gemm(s["h"], dzb, a_mn_major=True, b_mn_major=True, out=store.G(f"{sc}/classifier_mlp1/kernel"), atomic=True,
+        ops.gemm(h, dzb, a_mn_major=True, b_mn_major=True, out=store.G(f"{sc}/classifier_mlp1/kernel"), atomic=True,
                  M=H2, N=8, K=4 * b)
         # d pre = (dz W1^T) * keep/(1-p) * gelu'(pre): the hidden dropout and the GeLU backward in the dgrad epilogue
         dpre = bf.get(f"vcr.{t}.dpre", (4 * b, H2), torch.bfloat16)
-        ops.gemm(dzb, store.W(f"{sc}/classifier_mlp1/kernel"), out=dpre, mul_aux=s["gp"], dropout_p=p, dropout_seed=seed,
+        ops.gemm(dzb, store.W(f"{sc}/classifier_mlp1/kernel"), out=dpre, mul_aux=gp, dropout_p=p, dropout_seed=seed,
                  dropout_site=site_hid, M=4 * b, N=H2, K=8)
         ops.bias_grad(dpre, store.G(f"{sc}/classifier_mlp0/bias"), rows=4 * b, N=H2)
-        ops.gemm(s["x"], dpre, a_mn_major=True, b_mn_major=True, out=store.G(f"{sc}/classifier_mlp0/kernel"), atomic=True,
+        ops.gemm(x, dpre, a_mn_major=True, b_mn_major=True, out=store.G(f"{sc}/classifier_mlp0/kernel"), atomic=True,
                  M=H, N=H2, K=4 * b)
         # d first-token = (dpre W0^T) * keep/(1-p): the input dropout in the dgrad epilogue
         dx = bf.get(f"vcr.{t}.dx", (4 * b, H), torch.float32)

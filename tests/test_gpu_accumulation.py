@@ -104,7 +104,7 @@ def test_accumulated_pretraining_step_is_the_replica_oracle(A):
     assert max(worst.values()) < 4e-2, sorted(worst.items(), key=lambda kv: -kv[1])[:5]
 
 
-def test_features_only_pass_matches_the_training_forward():
+def test_features_only_towers_match_the_training_forward():
     """hidden_dropout_prob 0.1: the first pass (features_only) and the second (the training forward with the first pass's
     masks) compute the same contrastive features under the same seed."""
     from merlot_b200.modeling import MerlotModel
@@ -114,10 +114,10 @@ def test_features_only_pass_matches_the_training_forward():
     kw = dict(is_training=True, use_tpu=False, image=im.to(DEV), input_ids=ids.to(DEV), mask_input=True,
               shuffled_idx_img=sh.to(DEV), params=store, dropout_seed=77)
     m1 = MerlotModel(cfg, features_only=True, **kw)
-    l1, v1 = (t["feat"].clone() for t in m1.contrastive_features())
+    l1, v1 = (t.feat.clone() for t in m1.contrastive_features())
     masks = {k: v.clone() for k, v in m1.lang_mask_info.items()}
     m2 = MerlotModel(cfg, mask_override=masks, **kw)
-    l2, v2 = (t["feat"].clone() for t in m2.contrastive_features())
+    l2, v2 = (t.feat.clone() for t in m2.contrastive_features())
     torch.cuda.synchronize()
     for k in masks:
         assert torch.equal(m2.lang_mask_info[k].reshape(-1), masks[k].reshape(-1))
@@ -126,7 +126,7 @@ def test_features_only_pass_matches_the_training_forward():
     assert torch.equal(l1, l2) and torch.equal(v1, v2)
     # and dropout is on: another seed gives other features
     m3 = MerlotModel(cfg, features_only=True, **dict(kw, dropout_seed=78))
-    assert rel(m3.contrastive_features()[0]["feat"], l1) > 1e-3
+    assert rel(m3.contrastive_features()[0].feat, l1) > 1e-3
     with pytest.raises(RuntimeError, match="save_for_backward"):
         m1.backward()
 

@@ -158,7 +158,7 @@ def _step_parity(cfg, monkeypatch, hw=(64, 96), seed=2 ** 32 + 5):
     ref_logits = V.vcr_cls_head_train(om, leaf, dropout=hook)
     ref_loss, _ = V.vcr_loss(ref_logits, target)
     assert abs(float(spec.metrics["loss"]) - float(ref_loss)) <= 1e-3 * abs(float(ref_loss))
-    gpu_logits = spec.model._heads["vcr"]["logits"][:, :4]
+    gpu_logits = spec.model._vcr_cls[0][:, :4]
     assert rel(gpu_logits, ref_logits) < 1e-2
     assert float(spec.metrics["accuracy"]) == pytest.approx(float((gpu_logits.argmax(-1).cpu() == target.long()).float().mean()),
                                                             abs=1e-6)
@@ -197,11 +197,11 @@ def _step_parity(cfg, monkeypatch, hw=(64, 96), seed=2 ** 32 + 5):
     assert float(store.g.abs().max()) == 0.0 and store.global_step == 1
 
 
-def test_vcr_step_parity_patch_embed(tiny_cfg, monkeypatch):
+def test_vcr_step_parity_patch_embed_saved_head(tiny_cfg, monkeypatch):
     _step_parity(vcr_cfg(tiny_cfg), monkeypatch)
 
 
-def test_vcr_step_parity_through_the_hybrid_stem(tiny_cfg, monkeypatch):
+def test_vcr_step_parity_hybrid_stem_saved_head(tiny_cfg, monkeypatch):
     _step_parity(vcr_cfg(tiny_cfg, resnet_layers=[1, 2, 1]), monkeypatch)
 
 
@@ -234,7 +234,7 @@ def test_train_then_evaluate_on_the_trained_tower(tiny_cfg):
     assert tuple(head["rationale_cls/classifier_mlp1/bias"].shape) == (1,)
 
 
-def test_seeds(tiny_cfg):
+def test_seeds_of_the_saved_head(tiny_cfg):
     """One seed twice: the same logits and loss, gradients within the fp32-atomics spread; another seed: other logits."""
     from merlot_b200 import vcr
     cfg = vcr_cfg(tiny_cfg)
@@ -244,7 +244,7 @@ def test_seeds(tiny_cfg):
         _, store = build(cfg, tower_scale=10.0)
         fn = vcr.vcr_model_fn_builder(neat(cfg), store=store, seed=seed)
         spec = fn({"images": image.to(DEV).bfloat16(), "lm_input": ids.to(DEV), "lm_targets": target.to(DEV)})
-        logits = spec.model._heads["vcr"]["logits"][:, :4].clone()
+        logits = spec.model._vcr_cls[0][:, :4].clone()
         store.g.zero_()
         spec.model.backward(d_hidden_state=vcr.cls_head_backward(spec.model, store, target.to(DEV)))
         out.append((logits, float(spec.metrics["loss"]), store.g.clone()))
