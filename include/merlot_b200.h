@@ -102,10 +102,10 @@ int merlot_gemm_bf16(const merlot_gemm_t* g, void* stream);
  *  fwd   : ctx bf16 [B*S, ld_ctx] <- softmax(.) v
  *  bwd   : needs ctx, d_ctx (bf16 [B*S, ld_ctx]); writes dsum (scratch f32 [B,heads,S]) and dqkv bf16 [B*S, ld_dqkv].
  *          dq_accum is an fp32 workspace of merlot_attention_bwd_workspace_bytes(B,S,heads) bytes with row stride ld_dq (= H):
- *          for sequences of <= 4 key tiles (merlot_attention_bwd_dq_parts(S) > 0) every key tile stores its dQ partial into its
- *          own [B*S, ld_dq] slice (no atomics, bitwise reproducible, no initialisation needed); longer sequences red.add into
- *          ONE slice that MUST be zero on entry and is re-zeroed on exit;
- *          with d_bias_qkv != NULL the same pass adds colsum(dqkv) to it (bias gradient of the q/k/v tf.layers.dense).
+ *          sequences of <= 512 tokens (merlot_attention_bwd_dq_parts(S) > 0) neither read nor write it (dQ is computed per
+ *          64-query tile, with no atomics: dqkv is bitwise reproducible); longer sequences red.add into ONE slice that MUST be
+ *          zero on entry and is re-zeroed on exit;
+ *          with d_bias_qkv != NULL colsum(dqkv) is added to it (bias gradient of the q/k/v tf.layers.dense).
  *  colsum: colsum[b,k] += (1/heads) * sum_q P[b,h,q,k]   (f32 [B,S]; caller zeroes it once per stack).
  *  With dropout_p > 0, P above is the dropped P o Z / (1 - p) wherever it multiplies v or is summed (see the fields below).
  * ------------------------------------------------------------------------------------------------------------ */

@@ -32,9 +32,9 @@ struct AttnDev {
   float* lse;                    // [B, heads, S] natural-log LSE of the masked, scaled scores
   // backward
   float* dsum;                   // [B, heads, S]  D = rowsum(dO * O)
-  float* dq_accum; int ld_dq;    // fp32 [parts][B*S, H]: per-key-tile slices (or one atomically accumulated slice)
-  size_t dq_part_stride;         // elements between slices
-  bf16* dqkv; int ld_dqkv;       // bf16 [B*S, 3H]; this kernel writes the K and V column blocks
+  float* dq_accum; int ld_dq;    // fp32 [B*S, H], atomically accumulated by K3 (sequences of more than 512 tokens)
+  bf16* dqkv; int ld_dqkv;       // bf16 [B*S, 3H]
+  float* d_bias;                 // optional [3H] += column sums of dqkv (the short-sequence kernels add them in their epilogues)
   // K4
   float* colsum;                 // [B, S] += sum_q mean_h P[b,h,q,k]
   float* colsum2;                // optional: queries >= colsum_split accumulate here instead
@@ -102,6 +102,54 @@ __device__ __forceinline__ void quad_sum(float& x) {
   x += __shfl_xor_sync(0xffffffffu, x, 2);
 }
 
+// Attention-probability dropout with queries on the accumulator rows (K2, the dQ kernel): bit 4 jj + 2 i + e of the result is
+// the keep bit of accumulator element s[4 jj + 2 i + e] of this thread in the 64-key tile starting at k0 (ptx.cuh
+// attn_dropout_words: word 2 (q/8 & 1) + (k/8 & 1), with q/8 & 1 = i and k/8 & 1 = jj & 1 here).  drop_row = the query terms.
+__device__ __forceinline__ uint32_t attn_keep_bits_queryrows(const AttnDev& p, uint64_t drop_row, int k0, int lane) {
+  uint32_t z = 0;
+#pragma unroll
+  for (int jp = 0; jp < 4; ++jp) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const uint4 r = attn_dropout_words(p.drop_seed, p.drop_site, drop_row + (uint64_t)((k0 >> 4) + jp) * 8 + 2 * (lane & 3) + e);
+      const uint32_t w[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int kh = 0; kh < 2; ++kh)  // accumulator column group jj = 2 jp + kh
+          z |= ((w[2 * i + kh] >> 16) >= p.drop_thresh16 ? 1u : 0u) << (4 * (2 * jp + kh) + 2 * i + e);
+    }
+  }
+  return z;
+}
+
+// Adds the column sums of a warpgroup's 64 x 64 bf16 output block (this thread's values v[4 jj + 2 i + e], already rounded to
+// bf16 and zero in rows that are not written) to bias[8 jj + 2 (lane % 4) + e]: a sum over the 8 row groups of the warp by
+// shuffles, over the 4 warps through s_red [4][64], then one atomicAdd per column.  Every thread of the (one-warpgroup) CTA
+// calls it.
+__device__ __forceinline__ void bias_colsum_add(float (&v)[32], float* s_red, float* bias, int wq, int lane, int tid) {
+  float c[16];
+#pragma unroll
+  for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      float x = v[4 * jj + e] + v[4 * jj + 2 + e];
+      x += __shfl_xor_sync(0xffffffffu, x, 4);
+      x += __shfl_xor_sync(0xffffffffu, x, 8);
+      x += __shfl_xor_sync(0xffffffffu, x, 16);
+      c[2 * jj + e] = x;
+    }
+  if (lane < 4) {
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      s_red[wq * 64 + 8 * jj + 2 * lane] = c[2 * jj];
+      s_red[wq * 64 + 8 * jj + 2 * lane + 1] = c[2 * jj + 1];
+    }
+  }
+  __syncthreads();
+  if (tid < 64) atomicAdd(bias + tid, ((s_red[tid] + s_red[64 + tid]) + s_red[128 + tid]) + s_red[192 + tid]);
+}
+
 // -----------------------------------------------------------------------------------------------------------------
 // forward.  One CTA per (128-query tile, head, batch); warpgroup w owns queries [64 w, 64 w + 64).  Key tiles of 64 run
 // through a two-buffer TMA ring.  Per key tile:  S = Q K^T (wgmma, smem x smem) -> masked online softmax in registers (key
@@ -131,6 +179,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 2) attn_fwd_kernel(const __grid_c
   const int S = p.S, H = p.H;
   const int tok0 = b * S;
   const int n_kv = (S + FK - 1) / FK;
+  static_assert(FK == 64, "attn_keep_bits_queryrows draws the bits of 64-key tiles");
 
   if (tid == 0) {
     tma_prefetch_desc(&tm_q); tma_prefetch_desc(&tm_kv);
@@ -183,24 +232,9 @@ __global__ void __launch_bounds__(FWD_THREADS, 2) attn_fwd_kernel(const __grid_c
   mbar_wait(bar_q, 0);
   const uint32_t qa = smem_u32(sQ) + wg * 8192;
   for (int j = 0; j < n_kv; ++j) {
-    // keep bits of this key tile, bit x for accumulator element s[x] (x = 4 jj + 2 i + e), drawn while only O is live: with
-    // S live as well the no-mask instance would spill at 128 registers
-    uint32_t zq = 0;
-    if (DROP) {
-#pragma unroll
-      for (int jp = 0; jp < FK / 16; ++jp) {
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const uint4 r = attn_dropout_words(p.drop_seed, p.drop_site, drop_row + (uint64_t)((j * FK >> 4) + jp) * 8 + 2 * (lane & 3) + e);
-          const uint32_t w[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-          for (int i = 0; i < 2; ++i)
-#pragma unroll
-            for (int kh = 0; kh < 2; ++kh)  // word 2 (q/8 & 1) + (k/8 & 1); accumulator column group jj = 2 jp + kh
-              zq |= ((w[2 * i + kh] >> 16) >= p.drop_thresh16 ? 1u : 0u) << (4 * (2 * jp + kh) + 2 * i + e);
-        }
-      }
-    }
+    // keep bits of this key tile, drawn while only O is live: with S live as well the no-mask instance would spill at 128
+    // registers
+    const uint32_t zq = DROP ? attn_keep_bits_queryrows(p, drop_row, j * FK, lane) : 0u;
     mbar_wait(&bar_kv[j & 1], (uint32_t)((j >> 1) & 1));
     const uint32_t ka = smem_u32(sKV + (j & 1) * 16384), va = ka + 8192;
     float s[32];
@@ -294,12 +328,11 @@ __global__ void __launch_bounds__(FWD_THREADS, 2) attn_fwd_kernel(const __grid_c
 //   dS'^T -> bf16 smem; dQ_chunk = dS' K               (wgmma, both operands MN-major; warpgroup w computes head columns
 //                                                       [32 w, 32 w + 32) over all 128 keys) -> fp32 stores of the partial
 // 1/sqrt(d) is applied once per output (dK in the epilogue, dQ in attn_dqkv_finish) instead of once per score.
-// dQ never touches an atomic when the sequence has <= 4 key tiles: every CTA stores its partial for its key tile into its own
-// slice of the [parts][tokens][H] fp32 workspace and attn_dqkv_finish sums the slices (bitwise reproducible); longer
-// sequences red.add into one slice.
+// dQ is red.add-ed into one fp32 slice of the workspace.  K3 serves sequences of more than MAX_DQ_PARTS key tiles; shorter
+// ones take the two short-sequence kernels below.
 // -----------------------------------------------------------------------------------------------------------------
 constexpr int BQ = 64;              // queries per chunk
-constexpr int MAX_DQ_PARTS = 4;     // key tiles per sequence for which dQ goes through per-tile slices instead of atomics
+constexpr int MAX_DQ_PARTS = 4;     // key tiles of 128 up to which the short-sequence kernels run (S <= 512)
 constexpr int BWD_THREADS = 256;
 // K, V (16 KB each), 2 x {Q, dO} chunk (8 KB each), dS^T 16 KB, statistics 2 x 2 x 256 B, query mask, barriers, alignment
 constexpr int BWD_SMEM = 32768 + 32768 + 16384 + 1024 + 512 + 64 + 1024;
@@ -327,7 +360,7 @@ __device__ __forceinline__ uint32_t attn_keep_bits_keyrows(const AttnDev& p, uin
   return z;
 }
 
-template <bool HAS_MASK, bool DQ_ATOMIC, bool DROP>
+template <bool HAS_MASK, bool DROP>
 __global__ void __launch_bounds__(BWD_THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_kv, const __grid_constant__ CUtensorMap tm_q,
                 const __grid_constant__ CUtensorMap tm_do, const AttnDev p) {
@@ -396,7 +429,6 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_kv, const __grid_constant
   float dv[32], dk[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
-  float* dq_base = p.dq_accum + (DQ_ATOMIC ? (size_t)0 : (size_t)kt * p.dq_part_stride);
   uint64_t drop_n16 = 0, drop_bh = 0, drop_key = 0;
   if (DROP) {
     drop_n16 = (uint64_t)((S + 15) >> 4);
@@ -497,15 +529,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_kv, const __grid_constant
     for (int i = 0; i < 2; ++i) {
       const int q = q0 + wq * 16 + (lane >> 2) + 8 * i;
       if (q >= S) continue;
-      float* dst = dq_base + (size_t)(tok0 + q) * p.ld_dq + h * AT_D + wg * 32 + 2 * (lane & 3);
+      float* dst = p.dq_accum + (size_t)(tok0 + q) * p.ld_dq + h * AT_D + wg * 32 + 2 * (lane & 3);
 #pragma unroll
       for (int jj = 0; jj < 4; ++jj) {
         const float v0 = dq[4 * jj + 2 * i], v1 = dq[4 * jj + 2 * i + 1];
-        if (DQ_ATOMIC) {
-          asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst + 8 * jj), "f"(v0), "f"(v1) : "memory");
-        } else {
-          *reinterpret_cast<float2*>(dst + 8 * jj) = make_float2(v0, v1);
-        }
+        asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst + 8 * jj), "f"(v0), "f"(v1) : "memory");
       }
     }
     if (tid < BQ && c + 1 < n_q) stage_stats(c + 1);  // buffer (c + 1) & 1 was last read by chunk c - 1
@@ -563,11 +591,8 @@ __global__ void attn_dsum_kernel(const bf16* __restrict__ o, const bf16* __restr
 
 // dq fp32 accumulator -> bf16 q-block of dqkv (and re-zero the accumulator for the next layer), fused with the column sums
 // of the whole dqkv row block = the gradient of the fused q/k/v bias.  grid = (ceil(3H/256), row slabs), 8 warps, lane = 8 cols.
-// n_parts > 0: dq holds n_parts per-key-tile slices (part_stride elements apart) that are summed here; n_parts == 0: one
-// atomically accumulated slice that is re-zeroed for the next layer.
 __global__ void __launch_bounds__(256) attn_dqkv_finish_kernel(float* __restrict__ dq, int ld_dq, bf16* __restrict__ dqkv, int ld_dqkv,
-                                                               long long rows, int H, float* __restrict__ bias_grad, int n_parts,
-                                                               size_t part_stride, float scale) {
+                                                               long long rows, int H, float* __restrict__ bias_grad, float scale) {
   __shared__ float sred[8][256];
   pdl_launch_dependents();
   pdl_wait();
@@ -580,18 +605,9 @@ __global__ void __launch_bounds__(256) attn_dqkv_finish_kernel(float* __restrict
       bf16* o = dqkv + (size_t)r * ld_dqkv + col;
       if (col < H) {
         float4* src = reinterpret_cast<float4*>(dq + (size_t)r * ld_dq + col);
-        float4 a = src[0], b = src[1];
-        if (n_parts == 0) {
-          src[0] = make_float4(0.f, 0.f, 0.f, 0.f);
-          src[1] = make_float4(0.f, 0.f, 0.f, 0.f);
-        } else {
-          for (int t = 1; t < n_parts; ++t) {  // fixed order: the sum is bitwise reproducible
-            const float4* s2 = reinterpret_cast<const float4*>(dq + (size_t)t * part_stride + (size_t)r * ld_dq + col);
-            const float4 c = s2[0], d = s2[1];
-            a.x += c.x; a.y += c.y; a.z += c.z; a.w += c.w;
-            b.x += d.x; b.y += d.y; b.z += d.z; b.w += d.w;
-          }
-        }
+        const float4 a = src[0], b = src[1];
+        src[0] = make_float4(0.f, 0.f, 0.f, 0.f);
+        src[1] = make_float4(0.f, 0.f, 0.f, 0.f);
         // K3 accumulates dS' K without the 1/sqrt(d) of the scores: applied here, once per output element
         const uint4 pk = make_uint4(pack_bf16x2(a.x * scale, a.y * scale), pack_bf16x2(a.z * scale, a.w * scale),
                                     pack_bf16x2(b.x * scale, b.y * scale), pack_bf16x2(b.z * scale, b.w * scale));
@@ -618,6 +634,379 @@ __global__ void __launch_bounds__(256) attn_dqkv_finish_kernel(float* __restrict
 #pragma unroll
     for (int w = 0; w < 8; ++w) s2 += sred[w][c];
     atomicAdd(bias_grad + blockIdx.x * 256 + c, s2);
+  }
+}
+
+// -----------------------------------------------------------------------------------------------------------------
+// backward for sequences of <= 512 tokens: a dQ kernel (queries on the accumulator rows) launched first, then a dK/dV kernel
+// (keys on the rows).  Both recompute S and dP, which costs 1.4x K3's tensor work, and in return neither needs anything from
+// the other CTAs of its grid: no fp32 dQ workspace, no finish pass, no dsum pass, no atomics except one per bias column.
+// Each CTA is one warpgroup owning a 64-row tile, so a short sequence pads its last tile to 64 rows (not 128 as K3 does),
+// and two or three CTAs share an SM: one CTA's softmax runs under another's wgmma.  The mask, padding-query and dropout rules
+// are K3's, element for element; both orientations draw the same dropout bits (ptx.cuh attn_dropout_words).
+// -----------------------------------------------------------------------------------------------------------------
+constexpr int SB_THREADS = 128;   // one warpgroup
+constexpr int SB_ROWS = 64;       // query rows (dQ kernel) / key rows (dK/dV kernel) per CTA
+constexpr int SB_MASK_WORDS = 16; // validity bits of 512 positions
+// Q, dO, O (8 KB each), 2 x {K, V} chunk (8 KB each), bias column partials [4][64], -lse log2(e) and D [2][64], key mask,
+// barriers, alignment
+constexpr int DQ_SMEM = 3 * 8192 + 2 * 16384 + 1024 + 512 + 64 + 64 + 1024;
+// K, V (8 KB each), 2 x {Q, dO} chunk (8 KB each), bias column partials [2][4][64], statistics [2][2][64], query mask,
+// barriers, alignment
+constexpr int DKV_SMEM = 2 * 8192 + 2 * 16384 + 2048 + 1024 + 64 + 64 + 1024;
+
+// dQ of 64 queries of one (b, h): D = rowsum(dO o O) from the TMA-loaded O and dO tiles (written to dsum for the dK/dV kernel),
+// then 64-key chunks of K and V through a two-buffer TMA ring:
+//   S = Q K^T, dP = dO V^T                     (wgmma, smem x smem)
+//   P = exp2(S sc - lse), dS' = P (dP - D)     (registers; a padding query row sends nothing into dQ)
+//   dQ += dS' K                                (wgmma, A = dS' straight from registers, K MN-major)
+// and dQ x 1/sqrt(d) goes to the q block of dqkv as bf16.
+template <bool HAS_MASK, bool DROP>
+__global__ void __launch_bounds__(SB_THREADS, 3)
+attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
+                   const __grid_constant__ CUtensorMap tm_o, const AttnDev p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sQ = smem;
+  uint8_t* sdO = smem + 8192;
+  uint8_t* sO = smem + 16384;
+  uint8_t* sKV = smem + 24576;  // [2] x { K chunk 8 KB, V chunk 8 KB }: chunk j lives in buffer j & 1
+  float* s_red = reinterpret_cast<float*>(smem + 57344);  // [4][64]
+  float* s_nlse = s_red + 256;                            // [64]  -lse * log2(e)
+  float* s_dsum = s_nlse + SB_ROWS;                       // [64]
+  uint32_t* s_mask = reinterpret_cast<uint32_t*>(s_dsum + SB_ROWS);  // [SB_MASK_WORDS] key validity bits
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_mask + SB_MASK_WORDS);
+  uint64_t *bar_q = bars, *bar_kv = bars + 1 /* [2] */;
+
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int wq = __shfl_sync(0xffffffffu, tid >> 5, 0);
+  const int q0 = blockIdx.x * SB_ROWS, h = blockIdx.y, b = blockIdx.z;
+  pdl_launch_dependents();
+  const int S = p.S, H = p.H, tok0 = b * S;
+  const int n_kv = (S + SB_ROWS - 1) / SB_ROWS;
+
+  if (tid == 0) {
+    tma_prefetch_desc(&tm_qkv); tma_prefetch_desc(&tm_do); tma_prefetch_desc(&tm_o);
+    mbar_init(bar_q, 1); mbar_init(&bar_kv[0], 1); mbar_init(&bar_kv[1], 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();
+  auto load_kv = [&](int j) {
+    uint8_t* buf = sKV + (j & 1) * 16384;
+    mbar_arrive_expect_tx(&bar_kv[j & 1], 16384);
+    tma_load_2d(buf, &tm_qkv, &bar_kv[j & 1], H + h * AT_D, tok0 + j * SB_ROWS);
+    tma_load_2d(buf + 8192, &tm_qkv, &bar_kv[j & 1], 2 * H + h * AT_D, tok0 + j * SB_ROWS);
+  };
+  if (tid == 0) {
+    mbar_arrive_expect_tx(bar_q, 3 * 8192);
+    tma_load_2d(sQ, &tm_qkv, bar_q, h * AT_D, tok0 + q0);
+    tma_load_2d(sdO, &tm_do, bar_q, h * AT_D, tok0 + q0);
+    tma_load_2d(sO, &tm_o, bar_q, h * AT_D, tok0 + q0);
+    load_kv(0);
+    if (n_kv > 1) load_kv(1);
+  }
+  const size_t st0 = ((size_t)b * p.heads + h) * S;
+  if (tid < SB_ROWS) s_nlse[tid] = (q0 + tid < S) ? -p.lse[st0 + q0 + tid] * LOG2E : 0.f;
+  if (HAS_MASK) build_mask(s_mask, p.valid + tok0, n_kv * SB_ROWS, S);
+  mbar_wait(bar_q, 0);
+  // D: 8 lanes per query row, 8 columns each, summed in the order of attn_dsum_kernel (the long-sequence path)
+#pragma unroll
+  for (int it = 0; it < 4; ++it) {
+    const int r = it * 16 + (tid >> 3), sub = tid & 7;
+    const uint4 a = *reinterpret_cast<const uint4*>(sO + sw128_offset(r, sub));
+    const uint4 g = *reinterpret_cast<const uint4*>(sdO + sw128_offset(r, sub));
+    const uint32_t* pa = reinterpret_cast<const uint32_t*>(&a);
+    const uint32_t* pg = reinterpret_cast<const uint32_t*>(&g);
+    float acc = 0.f;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      float2 x = unpack_bf16x2(pa[i]), y = unpack_bf16x2(pg[i]);
+      acc += x.x * y.x + x.y * y.y;
+    }
+    acc += __shfl_xor_sync(0xffffffffu, acc, 1);
+    acc += __shfl_xor_sync(0xffffffffu, acc, 2);
+    acc += __shfl_xor_sync(0xffffffffu, acc, 4);
+    if (sub == 0) {
+      s_dsum[r] = acc;
+      if (q0 + r < S) p.dsum[st0 + q0 + r] = acc;
+    }
+  }
+  __syncthreads();
+
+  // this thread's two query rows (i = 0, 1); gq: the row is in range and valid, so it sends its gradient into q and k
+  float nl[2], dd[2];
+  bool gq[2];
+  int pair_lo[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int r = wq * 16 + (lane >> 2) + 8 * i, q = q0 + r;
+    nl[i] = s_nlse[r];
+    dd[i] = s_dsum[r];
+    const bool vq = (HAS_MASK && q < S) ? (p.valid[tok0 + q] != 0) : true;
+    gq[i] = q < S && vq;
+    pair_lo[i] = (HAS_MASK && vq) ? pair_lo_of(q, p.pair_P, p.pair_chunk) : -1;  // keys this query may see
+  }
+  const float sc2 = p.scale * LOG2E;
+  float dq[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) dq[i] = 0.f;
+  uint64_t drop_row = 0;
+  if (DROP) {
+    const uint64_t n16 = (uint64_t)((S + 15) >> 4);
+    drop_row = ((((uint64_t)b * p.heads + h) * n16 + (uint64_t)((q0 + wq * 16) >> 4)) * 8 + (lane >> 2)) * n16 * 8;
+  }
+  const uint32_t qa = smem_u32(sQ), da = smem_u32(sdO);
+  for (int j = 0; j < n_kv; ++j) {
+    const int k0 = j * SB_ROWS;
+    const uint32_t zq = DROP ? attn_keep_bits_queryrows(p, drop_row, k0, lane) : 0u;
+    mbar_wait(&bar_kv[j & 1], (uint32_t)((j >> 1) & 1));
+    const uint32_t ka = smem_u32(sKV + (j & 1) * 16384), va = ka + 8192;
+    float s[32], dp[32];
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < AT_D / 16; ++k) wgmma_m64n64_ss<0, 0>(s, desc_kmajor(qa, k), desc_kmajor(ka, k), k > 0 ? 1u : 0u);
+#pragma unroll
+    for (int k = 0; k < AT_D / 16; ++k) wgmma_m64n64_ss<0, 0>(dp, desc_kmajor(da, k), desc_kmajor(va, k), k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+    reg_fence(dp);
+    uint32_t iw[2], kw[2];
+#pragma unroll
+    for (int w = 0; w < 2; ++w) {
+      iw[w] = range_word(k0 + 32 * w, S);                           // key in range
+      kw[w] = HAS_MASK ? s_mask[(k0 >> 5) + w] : 0xffffffffu;       // key validity
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      uint32_t aw[2];
+#pragma unroll
+      for (int w = 0; w < 2; ++w)
+        aw[w] = kw[w] & ((HAS_MASK && pair_lo[i] >= 0) ? pair_word(k0 + 32 * w, pair_lo[i], p.pair_P, p.pair_chunk) : 0xffffffffu);
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int x = 4 * jj + 2 * i + e, bit = (8 * jj + 2 * (lane & 3) + e) & 31, w = jj >> 2;
+          float t = s[x] * sc2;
+          t = ((aw[w] >> bit) & 1u) ? t : MASKED_LOG2;
+          float pr = ex2_approx(t + nl[i]);
+          pr = (gq[i] && ((iw[w] >> bit) & 1u)) ? pr : 0.f;
+          if (DROP) {
+            const float zs = ((zq >> x) & 1u) ? p.drop_scale : 0.f;
+            dp[x] = (dp[x] * zs - dd[i]) * pr;
+          } else {
+            dp[x] = (dp[x] - dd[i]) * pr;
+          }
+        }
+      }
+    }
+    // ---- dQ += dS' K (A from registers; K MN-major: rows are keys) ----
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < SB_ROWS / 16; ++kk) {
+      uint32_t a[4];
+      acc_to_afrag(dp, kk, a);
+      wgmma_m64n64_rs<1>(dq, a, desc_mnmajor(ka, kk, 0), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(dq);
+    __syncthreads();  // buffer j & 1 is free
+    if (tid == 0 && j + 2 < n_kv) load_kv(j + 2);
+  }
+  // ---- dQ x 1/sqrt(d) -> bf16 q block; the bias column sums take the rounded values ----
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int q = q0 + wq * 16 + (lane >> 2) + 8 * i;
+    bf16* dst = p.dqkv + (size_t)(tok0 + q) * p.ld_dqkv + h * AT_D + 2 * (lane & 3);
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const uint32_t u = pack_bf16x2(dq[4 * jj + 2 * i] * p.scale, dq[4 * jj + 2 * i + 1] * p.scale);
+      const float2 f = unpack_bf16x2(u);
+      dq[4 * jj + 2 * i] = q < S ? f.x : 0.f;
+      dq[4 * jj + 2 * i + 1] = q < S ? f.y : 0.f;
+      if (q < S) *reinterpret_cast<uint32_t*>(dst + 8 * jj) = u;
+    }
+  }
+  if (p.d_bias) bias_colsum_add(dq, s_red, p.d_bias + h * AT_D, wq, lane, tid);
+}
+
+// dK and dV of 64 keys of one (b, h): K3 without its dQ half.  64-query chunks of Q and dO through a two-buffer TMA ring, with
+// the chunk's -lse log2(e) and D (written by attn_bwd_dq_kernel) staged in smem.  Per chunk:
+//   S^T = K Q^T, dP^T = V dO^T                       (wgmma, smem x smem)
+//   P^T = exp2(S^T sc - lse), dS'^T = P^T (dP^T - D)  (registers)
+//   dV += P^T dO, dK += dS'^T Q                        (wgmma, A straight from registers, dO / Q MN-major)
+template <bool HAS_MASK, bool DROP>
+__global__ void __launch_bounds__(SB_THREADS, 2)
+attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do, const AttnDev p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sK = smem;
+  uint8_t* sV = smem + 8192;
+  uint8_t* sQd = smem + 16384;  // [2] x { Q chunk 8 KB, dO chunk 8 KB }
+  float* s_red = reinterpret_cast<float*>(smem + 49152);  // [2][4][64]
+  float* s_nlse = s_red + 512;                            // [2][64]  -lse * log2(e)
+  float* s_dsum = s_nlse + 2 * BQ;                        // [2][64]
+  uint32_t* s_mask = reinterpret_cast<uint32_t*>(s_dsum + 2 * BQ);  // [SB_MASK_WORDS] query validity bits
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_mask + SB_MASK_WORDS);
+  uint64_t *bar_kv = bars, *bar_q = bars + 1 /* [2] */;
+
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int wq = __shfl_sync(0xffffffffu, tid >> 5, 0);
+  const int k0 = blockIdx.x * SB_ROWS, h = blockIdx.y, b = blockIdx.z;
+  pdl_launch_dependents();
+  const int S = p.S, H = p.H, tok0 = b * S;
+  const int n_q = (S + BQ - 1) / BQ;
+
+  if (tid == 0) {
+    tma_prefetch_desc(&tm_qkv); tma_prefetch_desc(&tm_do);
+    mbar_init(bar_kv, 1); mbar_init(&bar_q[0], 1); mbar_init(&bar_q[1], 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();  // before the first read of dsum: the dQ kernel writes it
+  auto load_q = [&](int c) {
+    uint8_t* buf = sQd + (c & 1) * 16384;
+    mbar_arrive_expect_tx(&bar_q[c & 1], 16384);
+    tma_load_2d(buf, &tm_qkv, &bar_q[c & 1], h * AT_D, tok0 + c * BQ);
+    tma_load_2d(buf + 8192, &tm_do, &bar_q[c & 1], h * AT_D, tok0 + c * BQ);
+  };
+  if (tid == 0) {
+    mbar_arrive_expect_tx(bar_kv, 16384);
+    tma_load_2d(sK, &tm_qkv, bar_kv, H + h * AT_D, tok0 + k0);
+    tma_load_2d(sV, &tm_qkv, bar_kv, 2 * H + h * AT_D, tok0 + k0);
+    load_q(0);
+    if (n_q > 1) load_q(1);
+  }
+  const size_t st0 = ((size_t)b * p.heads + h) * S;
+  auto stage_stats = [&](int c) {  // threads 0..63
+    const int q = c * BQ + tid;
+    s_nlse[(c & 1) * BQ + tid] = (q < S) ? -p.lse[st0 + q] * LOG2E : 0.f;
+    s_dsum[(c & 1) * BQ + tid] = (q < S) ? p.dsum[st0 + q] : 0.f;
+  };
+  if (tid < BQ) stage_stats(0);
+  if (HAS_MASK) build_mask(s_mask, p.valid + tok0, n_q * BQ, S);
+  __syncthreads();
+
+  // this thread's two key rows (i = 0, 1)
+  bool k_in[2], vk[2];
+  int pair_lo[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int kk = k0 + wq * 16 + (lane >> 2) + 8 * i;
+    k_in[i] = kk < S;
+    vk[i] = k_in[i] ? (HAS_MASK ? p.valid[tok0 + kk] != 0 : true) : false;
+    pair_lo[i] = HAS_MASK ? pair_lo_of(kk, p.pair_P, p.pair_chunk) : -1;  // queries this key is seen by
+  }
+  const float sc2 = p.scale * LOG2E;
+  float dv[32], dk[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
+  uint64_t drop_n16 = 0, drop_bh = 0, drop_key = 0;
+  if (DROP) {
+    drop_n16 = (uint64_t)((S + 15) >> 4);
+    drop_bh = ((uint64_t)b * p.heads + h) * drop_n16;
+    drop_key = (uint64_t)((k0 + wq * 16) >> 4) * 8 + (lane >> 2);
+  }
+
+  mbar_wait(bar_kv, 0);
+  const uint32_t ka = smem_u32(sK), va = smem_u32(sV);
+  for (int c = 0; c < n_q; ++c) {
+    const int bb = c & 1, q0 = c * BQ;
+    const uint32_t zk = DROP ? attn_keep_bits_keyrows(p, drop_bh, drop_key, drop_n16, q0, lane) : 0u;
+    mbar_wait(&bar_q[bb], (uint32_t)((c >> 1) & 1));
+    const uint32_t qa = smem_u32(sQd + bb * 16384), da = qa + 8192;
+    float s[32], dp[32];
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < AT_D / 16; ++k) wgmma_m64n64_ss<0, 0>(s, desc_kmajor(ka, k), desc_kmajor(qa, k), k > 0 ? 1u : 0u);
+#pragma unroll
+    for (int k = 0; k < AT_D / 16; ++k) wgmma_m64n64_ss<0, 0>(dp, desc_kmajor(va, k), desc_kmajor(da, k), k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+    reg_fence(dp);
+    const float* nlse = s_nlse + bb * BQ;
+    const float* dsm = s_dsum + bb * BQ;
+    uint32_t iw[2], qw[2];
+#pragma unroll
+    for (int w = 0; w < 2; ++w) {
+      iw[w] = range_word(q0 + 32 * w, S);                                  // query in range
+      qw[w] = HAS_MASK ? s_mask[(q0 >> 5) + w] : 0xffffffffu;              // query validity
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      uint32_t aw[2];
+#pragma unroll
+      for (int w = 0; w < 2; ++w)
+        aw[w] = (HAS_MASK && pair_lo[i] >= 0) ? pair_word(q0 + 32 * w, pair_lo[i], p.pair_P, p.pair_chunk) : 0xffffffffu;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int x = 4 * jj + 2 * i + e, col = 8 * jj + 2 * (lane & 3) + e, bit = col & 31, w = jj >> 2;
+          float t = s[x] * sc2;
+          t = (vk[i] && ((aw[w] >> bit) & 1u)) ? t : MASKED_LOG2;
+          t = ((qw[w] >> bit) & 1u) ? t : 0.f;  // padding query: uniform row (zero scores)
+          float pr = ex2_approx(t + nlse[col]);
+          pr = (k_in[i] && ((iw[w] >> bit) & 1u)) ? pr : 0.f;
+          const float gq = ((qw[w] >> bit) & 1u) ? pr : 0.f;  // a padding query keeps P for dV, sends nothing into k
+          if (DROP) {
+            const float zs = ((zk >> x) & 1u) ? p.drop_scale : 0.f;
+            s[x] = pr * zs;
+            dp[x] = (dp[x] * zs - dsm[col]) * gq;
+          } else {
+            s[x] = pr;
+            dp[x] = (dp[x] - dsm[col]) * gq;
+          }
+        }
+      }
+    }
+    // ---- dV += P^T dO, dK += dS'^T Q (A from registers; dO / Q MN-major: rows are queries) ----
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BQ / 16; ++kk) {
+      uint32_t a[4];
+      acc_to_afrag(s, kk, a);
+      wgmma_m64n64_rs<1>(dv, a, desc_mnmajor(da, kk, 0), 1u);
+    }
+#pragma unroll
+    for (int kk = 0; kk < BQ / 16; ++kk) {
+      uint32_t a[4];
+      acc_to_afrag(dp, kk, a);
+      wgmma_m64n64_rs<1>(dk, a, desc_mnmajor(qa, kk, 0), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(dv);
+    reg_fence(dk);
+    if (tid < BQ && c + 1 < n_q) stage_stats(c + 1);  // buffer (c + 1) & 1 was last read by chunk c - 1
+    __syncthreads();  // Q/dO buffer bb is free
+    if (tid == 0 && c + 2 < n_q) load_q(c + 2);
+  }
+  // ---- dK (x 1/sqrt(d)), dV of this key tile; the bias column sums take the rounded values ----
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int key = k0 + wq * 16 + (lane >> 2) + 8 * i;
+    bf16* dst = p.dqkv + (size_t)(tok0 + key) * p.ld_dqkv + h * AT_D + 2 * (lane & 3);
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const int x = 4 * jj + 2 * i;
+      const uint32_t uk = pack_bf16x2(dk[x] * p.scale, dk[x + 1] * p.scale), uv = pack_bf16x2(dv[x], dv[x + 1]);
+      const float2 fk = unpack_bf16x2(uk), fv = unpack_bf16x2(uv);
+      dk[x] = key < S ? fk.x : 0.f; dk[x + 1] = key < S ? fk.y : 0.f;
+      dv[x] = key < S ? fv.x : 0.f; dv[x + 1] = key < S ? fv.y : 0.f;
+      if (key < S) {
+        *reinterpret_cast<uint32_t*>(dst + H + 8 * jj) = uk;
+        *reinterpret_cast<uint32_t*>(dst + 2 * H + 8 * jj) = uv;
+      }
+    }
+  }
+  if (p.d_bias) {
+    bias_colsum_add(dk, s_red, p.d_bias + H + h * AT_D, wq, lane, tid);
+    bias_colsum_add(dv, s_red + 256, p.d_bias + 2 * H + h * AT_D, wq, lane, tid);
   }
 }
 
@@ -820,6 +1209,8 @@ extern "C" int merlot_attention_fwd(const merlot_attn_t* a, void* stream_) {
   return MERLOT_OK;
 }
 
+// > 0 (S <= 512): the short-sequence kernels run and the workspace is left alone; its size and this count stay as they were so
+// that callers sizing scratch from them keep working
 extern "C" int merlot_attention_bwd_dq_parts(int S) {
   const int n_kv = ceil_div(S, AT_N);
   return n_kv <= MAX_DQ_PARTS ? n_kv : 0;
@@ -843,8 +1234,41 @@ extern "C" int merlot_attention_bwd(const merlot_attn_t* a, void* stream_) {
   AttnDev p; fill_dev(a, &p);
   const int H = p.H;
   const long long tokens = (long long)a->B * a->S;
-  const int parts = merlot_attention_bwd_dq_parts(a->S);
-  p.dq_part_stride = (size_t)tokens * a->ld_dq;
+  CUtensorMap tq, tdo;
+  rc = make_tmap_bf16_2d(&tq, a->qkv, (uint64_t)a->ld_qkv, (uint64_t)tokens, (uint64_t)a->ld_qkv, 64, BQ);
+  if (rc) return rc;
+  rc = make_tmap_bf16_2d(&tdo, a->d_ctx, (uint64_t)a->ld_ctx, (uint64_t)tokens, (uint64_t)a->ld_ctx, 64, BQ);
+  if (rc) return rc;
+  if (merlot_attention_bwd_dq_parts(a->S) > 0) {  // short sequences: the dQ kernel, then the dK/dV kernel; dq_accum is not used
+    static_assert(SB_ROWS == BQ, "one 64-row tensor map serves both short-sequence kernels");
+    static_assert(MAX_DQ_PARTS * AT_N <= SB_MASK_WORDS * 32, "the short-sequence kernels' validity masks hold 512 positions");
+    CUtensorMap to;
+    rc = make_tmap_bf16_2d(&to, a->ctx, (uint64_t)a->ld_ctx, (uint64_t)tokens, (uint64_t)a->ld_ctx, 64, SB_ROWS);
+    if (rc) return rc;
+    p.d_bias = a->d_bias_qkv;
+    // [HAS_MASK][DROP]
+    static void (*const kdq[2][2])(CUtensorMap, CUtensorMap, CUtensorMap, AttnDev) = {
+        {attn_bwd_dq_kernel<false, false>, attn_bwd_dq_kernel<false, true>},
+        {attn_bwd_dq_kernel<true, false>, attn_bwd_dq_kernel<true, true>}};
+    static void (*const kdkv[2][2])(CUtensorMap, CUtensorMap, AttnDev) = {
+        {attn_bwd_dkdv_kernel<false, false>, attn_bwd_dkdv_kernel<false, true>},
+        {attn_bwd_dkdv_kernel<true, false>, attn_bwd_dkdv_kernel<true, true>}};
+    static bool attr_short = false;
+    if (!attr_short) {
+      for (int i = 0; i < 4; ++i) {
+        MB_CHECK_CUDA(cudaFuncSetAttribute(kdq[i >> 1][i & 1], cudaFuncAttributeMaxDynamicSharedMemorySize, DQ_SMEM));
+        MB_CHECK_CUDA(cudaFuncSetAttribute(kdkv[i >> 1][i & 1], cudaFuncAttributeMaxDynamicSharedMemorySize, DKV_SMEM));
+      }
+      attr_short = true;
+    }
+    const int m = a->valid != nullptr, d = a->dropout_p > 0.f;
+    dim3 grid(ceil_div(a->S, SB_ROWS), a->heads, a->B);
+    MB_CHECK_CUDA(launch_pdl(kdq[m][d], grid, dim3(SB_THREADS), DQ_SMEM, stream, tq, tdo, to, p));
+    MB_CHECK_LAUNCH();
+    MB_CHECK_CUDA(launch_pdl(kdkv[m][d], grid, dim3(SB_THREADS), DKV_SMEM, stream, tq, tdo, p));
+    MB_CHECK_LAUNCH();
+    return MERLOT_OK;
+  }
   {  // D = rowsum(dO * O)
     const long long threads = tokens * a->heads * 8;
     MB_CHECK_CUDA(launch_pdl(attn_dsum_kernel, dim3((unsigned)ceil_div_ll(threads, 256)), dim3(256), 0, stream,
@@ -852,34 +1276,27 @@ extern "C" int merlot_attention_bwd(const merlot_attn_t* a, void* stream_) {
                              a->B, a->S, a->heads));
     MB_CHECK_LAUNCH();
   }
-  CUtensorMap tkv, tq, tdo;
-  rc = make_tmap_bf16_2d(&tkv, a->qkv, (uint64_t)a->ld_qkv, (uint64_t)tokens, (uint64_t)a->ld_qkv, 64, 128);
+  CUtensorMap tkv;
+  rc = make_tmap_bf16_2d(&tkv, a->qkv, (uint64_t)a->ld_qkv, (uint64_t)tokens, (uint64_t)a->ld_qkv, 64, AT_N);
   if (rc) return rc;
-  rc = make_tmap_bf16_2d(&tq, a->qkv, (uint64_t)a->ld_qkv, (uint64_t)tokens, (uint64_t)a->ld_qkv, 64, BQ);
-  if (rc) return rc;
-  rc = make_tmap_bf16_2d(&tdo, a->d_ctx, (uint64_t)a->ld_ctx, (uint64_t)tokens, (uint64_t)a->ld_ctx, 64, BQ);
-  if (rc) return rc;
-  // [HAS_MASK][DQ_ATOMIC][DROP]
-  static void (*const kerns[2][2][2])(CUtensorMap, CUtensorMap, CUtensorMap, AttnDev) = {
-      {{attn_bwd_kernel<false, false, false>, attn_bwd_kernel<false, false, true>},
-       {attn_bwd_kernel<false, true, false>, attn_bwd_kernel<false, true, true>}},
-      {{attn_bwd_kernel<true, false, false>, attn_bwd_kernel<true, false, true>},
-       {attn_bwd_kernel<true, true, false>, attn_bwd_kernel<true, true, true>}}};
+  // [HAS_MASK][DROP]
+  static void (*const kerns[2][2])(CUtensorMap, CUtensorMap, CUtensorMap, AttnDev) = {
+      {attn_bwd_kernel<false, false>, attn_bwd_kernel<false, true>},
+      {attn_bwd_kernel<true, false>, attn_bwd_kernel<true, true>}};
   static bool attr = false;
   if (!attr) {
-    for (int i = 0; i < 8; ++i)
-      MB_CHECK_CUDA(cudaFuncSetAttribute(kerns[i >> 2][(i >> 1) & 1][i & 1], cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
+    for (int i = 0; i < 4; ++i)
+      MB_CHECK_CUDA(cudaFuncSetAttribute(kerns[i >> 1][i & 1], cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
     attr = true;
   }
   dim3 grid(ceil_div(a->S, AT_N), a->heads, a->B);
-  MB_CHECK_CUDA(launch_pdl(kerns[a->valid != nullptr][parts == 0][a->dropout_p > 0.f], grid, dim3(BWD_THREADS), BWD_SMEM, stream, tkv,
-                           tq, tdo, p));
+  MB_CHECK_CUDA(launch_pdl(kerns[a->valid != nullptr][a->dropout_p > 0.f], grid, dim3(BWD_THREADS), BWD_SMEM, stream, tkv, tq, tdo, p));
   MB_CHECK_LAUNCH();
   {
     long long slabs = ceil_div_ll(tokens, 64);
     if (slabs > 128) slabs = 128;
     MB_CHECK_CUDA(launch_pdl(attn_dqkv_finish_kernel, dim3(ceil_div(3 * H, 256), (unsigned)slabs), dim3(256), 0, stream, a->dq_accum,
-                             a->ld_dq, p.dqkv, a->ld_dqkv, tokens, H, a->d_bias_qkv, parts, p.dq_part_stride, a->scale));
+                             a->ld_dq, p.dqkv, a->ld_dqkv, tokens, H, a->d_bias_qkv, a->scale));
     MB_CHECK_LAUNCH();
   }
   return MERLOT_OK;
