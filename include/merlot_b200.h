@@ -322,11 +322,14 @@ int merlot_ids_valid(const int* ids, void* valid_u8, long long n, void* stream);
  * lr_t = lr * schedule * sqrt(1-beta2^t)/(1-beta1^t) is computed by the host (optimization.py:352-358).
  * ------------------------------------------------------------------------------------------------------------ */
 typedef struct merlot_adamw {
-  float* p; float* g; void* m; void* v;   /* fp32 master, fp32 grad, bf16 m, packed bf16 v */
+  float* p; float* g; void* m; void* v;   /* fp32 master, fp32 grad, moments as moments_f32 says */
   void* p_bf16;                           /* optional bf16 compute copy of p */
   long long n;
   float beta1, one_minus_beta1, beta2, one_minus_beta2, epsilon, lr_t, weight_decay, grad_scale;
   int zero_grad;
+  /* 0: bf16 m and sign-packed bf16 v (use_bfloat16_adam: True, :371-383); 1: fp32 m and v (use_bfloat16_adam: False, the
+   * reference's default, :305).  Any other value is MERLOT_EINVAL. */
+  int moments_f32;
 } merlot_adamw_t;
 int merlot_adamw_step(const merlot_adamw_t* d, void* stream);
 /* tf.clip_by_global_norm over the flat gradient arena (utils/optimization.py:233-237); scratch_f64 = one device double;

@@ -4,10 +4,13 @@
 //   g2 = g*g + 1e-30;  m' = b1*m + (1-b1)*g;  v' = b2*v + (1-b2)*g2;  u = m'/(sqrt(v')+eps);  u += wd*p (wd>0);
 //   p' = p - lr_t*u;   m' -> bf16 (RNE);  v' -> e=bf16(v'), stored as +e if |e-v'| <= |e*1.00390625-v'| else -e.
 // g is first scaled by grad_scale (= 1/world_size: CrossShardOptimizer's mean, :241-245).
+// With use_bfloat16_adam off (the reference's default, :305) m and v are plain fp32 and skip the bf16 rounding and the
+// sign packing: adamw_kernel<true>.
 // Also emits the bf16 compute copy of the new parameter (bfloat16_getter, utils/model_utils.py:572-602) and can zero
-// the gradient for the next step.  HBM traffic: 20 B/param (+2 bf16 copy, +4 grad zeroing).
+// the gradient for the next step.  HBM traffic: 20 B/param with bf16 moments, 28 B/param with fp32 moments (+2 bf16 copy,
+// +4 grad zeroing: 26 and 34 B).
 // Explicit round-to-nearest intrinsics keep the op-by-op fp32 rounding of the reference (no FMA contraction), so the
-// stored bf16 moments are bit-exact against the oracle.
+// stored moments, bf16 or fp32, are bit-exact against the oracle.
 #include "host_common.h"
 #include "ptx.cuh"
 
@@ -40,23 +43,57 @@ __device__ __forceinline__ void adam_elem(float& p, float g, bf16& mb, bf16& vb,
   vb = (err0 <= err1) ? e : __float2bfloat16_rn(-ef);
 }
 
+// fp32 moments: the same operations in the same order as adam_elem, without the bf16 storage of m and v.
+__device__ __forceinline__ void adam_elem_f32(float& p, float g, float& m, float& v, const AdamDev& a) {
+  g = __fmul_rn(g, a.grad_scale);
+  const float g2 = __fadd_rn(__fmul_rn(g, g), 1e-30f);
+  m = __fadd_rn(__fmul_rn(a.b1, m), __fmul_rn(a.omb1, g));
+  v = __fadd_rn(__fmul_rn(a.b2, v), __fmul_rn(a.omb2, g2));
+  float u = __fdiv_rn(m, __fadd_rn(__fsqrt_rn(v), a.eps));
+  if (a.wd > 0.f) u = __fadd_rn(u, __fmul_rn(a.wd, p));
+  p = __fsub_rn(p, __fmul_rn(a.lr_t, u));
+}
+
+// F32M: a.m / a.v hold fp32 moments (8 elements = two float4 each) instead of bf16 m and packed bf16 v (one uint4 each).
+template <bool F32M>
 __global__ void __launch_bounds__(256) adamw_kernel(const AdamDev a) {
   const long long i8 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * 8;
   if (i8 >= a.n) return;
   if (i8 + 8 <= a.n) {
+    float* mf = reinterpret_cast<float*>(a.m);
+    float* vf = reinterpret_cast<float*>(a.v);
     float4 p0 = *reinterpret_cast<float4*>(a.p + i8), p1 = *reinterpret_cast<float4*>(a.p + i8 + 4);
     float4 g0 = *reinterpret_cast<float4*>(a.g + i8), g1 = *reinterpret_cast<float4*>(a.g + i8 + 4);
-    uint4 mu = *reinterpret_cast<uint4*>(a.m + i8), vu = *reinterpret_cast<uint4*>(a.v + i8);
+    alignas(16) float mm[8], vv[8];  // F32M: fp32 m and v
+    uint4 mu, vu;                    // !F32M: bf16 m, packed bf16 v
+    if constexpr (F32M) {
+      reinterpret_cast<float4*>(mm)[0] = *reinterpret_cast<float4*>(mf + i8);
+      reinterpret_cast<float4*>(mm)[1] = *reinterpret_cast<float4*>(mf + i8 + 4);
+      reinterpret_cast<float4*>(vv)[0] = *reinterpret_cast<float4*>(vf + i8);
+      reinterpret_cast<float4*>(vv)[1] = *reinterpret_cast<float4*>(vf + i8 + 4);
+    } else {
+      mu = *reinterpret_cast<uint4*>(a.m + i8); vu = *reinterpret_cast<uint4*>(a.v + i8);
+    }
     float pv[8] = {p0.x, p0.y, p0.z, p0.w, p1.x, p1.y, p1.z, p1.w};
     const float gv[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-    bf16* mm = reinterpret_cast<bf16*>(&mu);
-    bf16* vv = reinterpret_cast<bf16*>(&vu);
+    bf16* mb = reinterpret_cast<bf16*>(&mu);
+    bf16* vb = reinterpret_cast<bf16*>(&vu);
 #pragma unroll
-    for (int k = 0; k < 8; ++k) adam_elem(pv[k], gv[k], mm[k], vv[k], a);
+    for (int k = 0; k < 8; ++k) {
+      if constexpr (F32M) adam_elem_f32(pv[k], gv[k], mm[k], vv[k], a);
+      else adam_elem(pv[k], gv[k], mb[k], vb[k], a);
+    }
     *reinterpret_cast<float4*>(a.p + i8) = make_float4(pv[0], pv[1], pv[2], pv[3]);
     *reinterpret_cast<float4*>(a.p + i8 + 4) = make_float4(pv[4], pv[5], pv[6], pv[7]);
-    *reinterpret_cast<uint4*>(a.m + i8) = mu;
-    *reinterpret_cast<uint4*>(a.v + i8) = vu;
+    if constexpr (F32M) {
+      *reinterpret_cast<float4*>(mf + i8) = reinterpret_cast<float4*>(mm)[0];
+      *reinterpret_cast<float4*>(mf + i8 + 4) = reinterpret_cast<float4*>(mm)[1];
+      *reinterpret_cast<float4*>(vf + i8) = reinterpret_cast<float4*>(vv)[0];
+      *reinterpret_cast<float4*>(vf + i8 + 4) = reinterpret_cast<float4*>(vv)[1];
+    } else {
+      *reinterpret_cast<uint4*>(a.m + i8) = mu;
+      *reinterpret_cast<uint4*>(a.v + i8) = vu;
+    }
     if (a.p_bf16)
       *reinterpret_cast<uint4*>(a.p_bf16 + i8) =
           make_uint4(pack_bf16x2(pv[0], pv[1]), pack_bf16x2(pv[2], pv[3]), pack_bf16x2(pv[4], pv[5]), pack_bf16x2(pv[6], pv[7]));
@@ -67,9 +104,17 @@ __global__ void __launch_bounds__(256) adamw_kernel(const AdamDev a) {
   } else {
     for (long long i = i8; i < a.n; ++i) {
       float pv = a.p[i];
-      bf16 mm = a.m[i], vv = a.v[i];
-      adam_elem(pv, a.g[i], mm, vv, a);
-      a.p[i] = pv; a.m[i] = mm; a.v[i] = vv;
+      if constexpr (F32M) {
+        float* mf = reinterpret_cast<float*>(a.m);
+        float* vf = reinterpret_cast<float*>(a.v);
+        float mm = mf[i], vv = vf[i];
+        adam_elem_f32(pv, a.g[i], mm, vv, a);
+        a.p[i] = pv; mf[i] = mm; vf[i] = vv;
+      } else {
+        bf16 mm = a.m[i], vv = a.v[i];
+        adam_elem(pv, a.g[i], mm, vv, a);
+        a.p[i] = pv; a.m[i] = mm; a.v[i] = vv;
+      }
       if (a.p_bf16) a.p_bf16[i] = __float2bfloat16_rn(pv);
       if (a.zero_grad) a.g[i] = 0.f;
     }
@@ -138,6 +183,7 @@ extern "C" int merlot_clip_by_global_norm(float* g, long long n, float clip_norm
 extern "C" int merlot_adamw_step(const merlot_adamw_t* d, void* stream_) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
   MB_REQUIRE(d && d->p && d->g && d->m && d->v, MERLOT_EINVAL, "adamw_step: null pointer");
+  MB_REQUIRE(d->moments_f32 == 0 || d->moments_f32 == 1, MERLOT_EINVAL, "adamw_step: moments_f32 must be 0 (packed bf16) or 1 (fp32)");
   MB_REQUIRE(((uintptr_t)d->p % 16) == 0 && ((uintptr_t)d->g % 16) == 0 && ((uintptr_t)d->m % 16) == 0 &&
                  ((uintptr_t)d->v % 16) == 0 && (!d->p_bf16 || ((uintptr_t)d->p_bf16 % 16) == 0),
              MERLOT_ESHAPE, "adamw_step: buffers must be 16-byte aligned (pad each group to a multiple of 8 elements)");
@@ -146,7 +192,11 @@ extern "C" int merlot_adamw_step(const merlot_adamw_t* d, void* stream_) {
   a.p = d->p; a.g = d->g; a.m = (bf16*)d->m; a.v = (bf16*)d->v; a.p_bf16 = (bf16*)d->p_bf16; a.n = d->n;
   a.b1 = d->beta1; a.omb1 = d->one_minus_beta1; a.b2 = d->beta2; a.omb2 = d->one_minus_beta2;
   a.eps = d->epsilon; a.lr_t = d->lr_t; a.wd = d->weight_decay; a.grad_scale = d->grad_scale; a.zero_grad = d->zero_grad;
-  adamw_kernel<<<(unsigned)ceil_div_ll(ceil_div_ll(d->n, 8), 256), 256, 0, st>>>(a);
+  const unsigned grid = (unsigned)ceil_div_ll(ceil_div_ll(d->n, 8), 256);
+  if (d->moments_f32)
+    adamw_kernel<true><<<grid, 256, 0, st>>>(a);
+  else
+    adamw_kernel<false><<<grid, 256, 0, st>>>(a);
   MB_CHECK_LAUNCH();
   return MERLOT_OK;
 }

@@ -590,10 +590,14 @@ def mask_inputs(ids, attn_summ, draws, masked_ids, masked_idx, valid_out, num_to
 
 
 def adamw_step(p, g, m, v, p_bf16, n, beta1, omb1, beta2, omb2, eps, lr_t, wd, grad_scale, zero_grad):
+    """K10 on n elements.  m and v are both float32 (use_bfloat16_adam: False) or both bfloat16 (bf16 m, sign-packed v)."""
+    if m.dtype != v.dtype or m.dtype not in (torch.float32, torch.bfloat16):
+        raise L.MerlotError(L.MERLOT_EINVAL, f"adamw_step: m and v must be both float32 or both bfloat16, got {m.dtype} and {v.dtype}")
     d = L.merlot_adamw_t()
     d.p, d.g, d.m, d.v, d.p_bf16, d.n = p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), _ptr(p_bf16), n
     d.beta1, d.one_minus_beta1, d.beta2, d.one_minus_beta2 = beta1, omb1, beta2, omb2
     d.epsilon, d.lr_t, d.weight_decay, d.grad_scale, d.zero_grad = eps, lr_t, wd, grad_scale, int(zero_grad)
+    d.moments_f32 = int(m.dtype == torch.float32)
     L.lib().merlot_adamw_step(C.byref(d), _stream())
 
 

@@ -35,8 +35,12 @@ class AdamOptimizer:
                  clip_norm=1.0, adafactor=False, **kwargs):
         if adafactor:
             raise ValueError("Adafactor not supported rn")  # optimization.py:178-179
-        if not use_bfloat16_adam:
-            raise NotImplementedError("use_bfloat16_adam: False (fp32 Adam moments) is not provided; every shipped config sets True")
+        # The moments' storage was fixed when the ParamStore was built: fp32 for use_bfloat16_adam False (the reference's
+        # default), bf16 m and sign-packed bf16 v for True (utils/optimization.py:371-411).
+        want_dt = torch.bfloat16 if use_bfloat16_adam else torch.float32
+        if store.moment_dtype != want_dt:
+            raise ValueError(f"ParamStore keeps {store.moment_dtype} Adam moments but this config sets use_bfloat16_adam: "
+                             f"{bool(use_bfloat16_adam)}; build ParamStore(cfg, optimizer_cfg=...) from the same config")
         self.clip_norm = float(clip_norm or 0.0)
         self.store = store
         self.learning_rate = learning_rate

@@ -1,8 +1,9 @@
 """Parameter arena: every trainable variable of the reference (SURVEY.md Appendix A) in ONE flat fp32 master buffer, with
-matching flat buffers for the fp32 gradients (the NCCL all-reduce bucket), the bf16 Adam first moment, the sign-packed
-bf16 second moment (utils/optimization.py:371-383) and the bf16 compute copy (bfloat16_getter,
-utils/model_utils.py:572-602).  Layout in HBM: [hyper-parameter group 0 | group 1 | ...], each variable padded to 64
-elements so every slice is 256-byte (fp32) / 128-byte (bf16) aligned and usable as a TMA base.
+matching flat buffers for the fp32 gradients (the NCCL all-reduce bucket), the Adam moments -- bf16 first moment and
+sign-packed bf16 second moment with use_bfloat16_adam (utils/optimization.py:371-383), fp32 both without it, the
+reference's default (:305) -- and the bf16 compute copy (bfloat16_getter, utils/model_utils.py:572-602).  Layout in HBM:
+[hyper-parameter group 0 | group 1 | ...], each variable padded to 64 elements so every slice is 256-byte (fp32) / 128-byte
+(bf16) aligned and usable as a TMA base.
 
 Storage differs from the TF variables in three places (converted by load_tf_dict / to_tf_dict):
   * query/key/value kernels [H,H] x3 are fused into `.../qkv/kernel` [H,3H] (and biases into [3H]);
@@ -169,7 +170,9 @@ def hyper_for(tf_name: str, optimizer_cfg: dict) -> Tuple[float, float, float, f
 
 
 class ParamStore:
-    """Flat arenas + named views.  `optimizer_cfg` fixes the hyper-parameter grouping (needed only for training)."""
+    """Flat arenas + named views.  `optimizer_cfg` fixes the hyper-parameter grouping (needed only for training) and the
+    Adam moments' storage: fp32 unless it sets use_bfloat16_adam (the reference's default is False); without an
+    optimizer_cfg the moments are bf16."""
 
     def __init__(self, model_cfg: dict, device="cuda", optimizer_cfg: Optional[dict] = None, with_optimizer_state=True,
                  task: str = "pretrain"):
@@ -218,9 +221,11 @@ class ParamStore:
         self.p = torch.zeros(off, dtype=torch.float32, device=self.device)
         self.g = torch.zeros(off, dtype=torch.float32, device=self.device)
         self.pb = torch.zeros(off, dtype=torch.bfloat16, device=self.device)
+        use_bf16_adam = optimizer_cfg is None or bool(optimizer_cfg.get("use_bfloat16_adam", False))
+        self.moment_dtype = torch.bfloat16 if use_bf16_adam else torch.float32
         if with_optimizer_state:
-            self.m = torch.zeros(off, dtype=torch.bfloat16, device=self.device)
-            self.v = torch.zeros(off, dtype=torch.bfloat16, device=self.device)
+            self.m = torch.zeros(off, dtype=self.moment_dtype, device=self.device)
+            self.v = torch.zeros(off, dtype=self.moment_dtype, device=self.device)
         self.global_step = 0
 
     def vit_buckets(self, n_groups: int = 4):
@@ -355,23 +360,25 @@ class ParamStore:
 
     def _checkpoint_tensors(self, skip):
         """(name, TF dtype, device view) of every variable of a checkpoint of this store, in data-file order: global_step,
-        the fp32 parameters, then the bf16 slots (every offset stays a multiple of its element size)."""
+        the fp32 parameters, then the slots -- bf16 or fp32 as the moments are stored (every offset stays a multiple of
+        its element size)."""
         from .tf_checkpoint import DT_BFLOAT16, DT_FLOAT
         if not hasattr(self, "m"):
             raise ValueError("checkpoints hold the optimizer state: build the ParamStore with with_optimizer_state=True")
         slots = {e.name for e in self.slot_entries(skip)}
         views = self.tf_views(self.p)
         out = [(nm, DT_FLOAT, t) for _, nm, t in views]
+        slot_dt = DT_FLOAT if self.moment_dtype == torch.float32 else DT_BFLOAT16
         for suffix, buf in (("adam_m", self.m), ("adam_v", self.v)):
-            out += [(f"{nm}/{suffix}", DT_BFLOAT16, t) for e, nm, t in self.tf_views(buf) if e.name in slots]
+            out += [(f"{nm}/{suffix}", slot_dt, t) for e, nm, t in self.tf_views(buf) if e.name in slots]
         return out
 
     def save_checkpoint(self, prefix: str, skip=()) -> Dict[str, float]:
         """Write the training state as the TensorFlow V2 checkpoint `prefix` (model.ckpt-<step> of the reference's Estimator):
-        every variable under its reference name (as to_tf_dict maps it), the bf16 `adam_m` / sign-packed `adam_v` slots of
-        slot_entries(skip) bit for bit, and `global_step` (int64).  The data file is gathered on the device, checksummed
-        there by one K15 launch, copied to pinned host memory at once and written by tf_checkpoint.write_bundle.  Extra
-        device memory: one buffer of the data file's size.  Returns the seconds each phase took and the bytes written."""
+        every variable under its reference name (as to_tf_dict maps it), the `adam_m` / `adam_v` slots of slot_entries(skip)
+        bit for bit (bf16 and sign-packed bf16, or fp32 both, as the store keeps them), and `global_step` (int64).  The
+        data file is gathered on the device, checksummed there by one K15 launch, copied to pinned host memory at once and
+        written by tf_checkpoint.write_bundle.  Extra device memory: one buffer of the data file's size.  Returns the seconds each phase took and the bytes written."""
         import time
         from .tf_checkpoint import DT_INT64, write_bundle
         t0 = time.perf_counter()
@@ -406,7 +413,8 @@ class ParamStore:
         Padding columns and padding elements restore as zero; slots of variables outside slot_entries(skip) restore as zero.
         (load_checkpoint is the other operation: init_checkpoint's restore-by-name of model variables.)"""
         import numpy as np
-        from .tf_checkpoint import DT_INT64, CheckpointFormatError, _index, mask_crc
+        from .tf_checkpoint import DT_BFLOAT16, DT_FLOAT, DT_INT64, CheckpointFormatError, _index, mask_crc
+        slot_flag = {DT_BFLOAT16: True, DT_FLOAT: False}  # slot dtype -> the use_bfloat16_adam that writes it
         header, entries = _index(prefix, True)
         want = [("global_step", DT_INT64, None)] + self._checkpoint_tensors(skip)
         missing = [nm for nm, _, _ in want if nm not in entries]
@@ -417,8 +425,11 @@ class ParamStore:
             e = entries[nm]
             shape = [] if t is None else list(t.shape)
             if int(e["dtype"]) != dt or [int(d) for d in e["shape"]] != shape:
-                raise CheckpointFormatError(f"{nm}: checkpoint has dtype {e['dtype']} shape {e['shape']}, the store needs "
-                                            f"dtype {dt} shape {shape}")
+                msg = f"{nm}: checkpoint has dtype {e['dtype']} shape {e['shape']}, the store needs dtype {dt} shape {shape}"
+                if nm.endswith(("/adam_m", "/adam_v")) and int(e["dtype"]) != dt and int(e["dtype"]) in slot_flag:
+                    msg += (f"; the checkpoint was written with use_bfloat16_adam: {slot_flag[int(e['dtype'])]}, this store "
+                            f"keeps its moments for use_bfloat16_adam: {slot_flag[dt]} (slots are not converted)")
+                raise CheckpointFormatError(msg)
             if e["slices"]:
                 raise NotImplementedError(f"{nm}: partitioned (sliced) variables are not supported")
         if header["num_shards"] != 1 or any(int(e["shard_id"]) for e in entries.values()):
