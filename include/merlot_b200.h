@@ -335,6 +335,10 @@ int merlot_adamw_step(const merlot_adamw_t* d, void* stream);
 /* tf.clip_by_global_norm over the flat gradient arena (utils/optimization.py:233-237); scratch_f64 = one device double;
  * norm_out (optional device float) receives the pre-clip global norm (the reference's gradnorms/_overall metric). */
 int merlot_clip_by_global_norm(float* g, long long n, float clip_norm, double* scratch_f64, float* norm_out, void* stream);
+/* One micro-batch of a clipped accumulated step: acc += g * clip_norm / max(norm, clip_norm) with norm = ||g|| (summed in
+ * fp64), then g = 0, in one fused pass after the norm pass.  acc and g are distinct, 16-byte aligned arenas of n floats;
+ * scratch_f64 = one device double; norm_out (optional device float) receives the pre-clip norm. */
+int merlot_clip_accumulate(float* acc, float* g, long long n, float clip_norm, double* scratch_f64, float* norm_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Loss-head glue (model/modeling.py:491-668): integer index/label construction and weighted reductions, on device.

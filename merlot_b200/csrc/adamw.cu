@@ -161,9 +161,52 @@ __global__ void __launch_bounds__(256) clip_scale_kernel(float* __restrict__ g, 
   }
 }
 
+// Gradient accumulation with a per-micro-batch clip: acc += s * g and g = 0 in one pass, s = clip_norm / max(norm, clip_norm)
+// from the norm sumsq_kernel left in *sumsq.  20 B/element with the norm pass (g read twice, acc read and written, g written).
+// s * g and the add round separately (no FMA), so s == 1 adds g exactly as the unclipped accumulation would.
+__global__ void __launch_bounds__(256) clip_accumulate_kernel(float* __restrict__ acc, float* __restrict__ g, long long n,
+                                                              const double* __restrict__ sumsq, float clip_norm,
+                                                              float* __restrict__ norm_out) {
+  const float norm = (float)sqrt(*sumsq);
+  if (blockIdx.x == 0 && threadIdx.x == 0 && norm_out) *norm_out = norm;
+  const float scale = clip_norm / fmaxf(norm, clip_norm);
+  for (long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * 4; i < n; i += (long long)gridDim.x * blockDim.x * 4) {
+    if (i + 4 <= n) {
+      float4 a = *reinterpret_cast<float4*>(acc + i);
+      const float4 v = *reinterpret_cast<const float4*>(g + i);
+      a.x = __fadd_rn(a.x, __fmul_rn(scale, v.x)); a.y = __fadd_rn(a.y, __fmul_rn(scale, v.y));
+      a.z = __fadd_rn(a.z, __fmul_rn(scale, v.z)); a.w = __fadd_rn(a.w, __fmul_rn(scale, v.w));
+      *reinterpret_cast<float4*>(acc + i) = a;
+      *reinterpret_cast<float4*>(g + i) = make_float4(0.f, 0.f, 0.f, 0.f);
+    } else {
+      for (long long j = i; j < n; ++j) {
+        acc[j] = __fadd_rn(acc[j], __fmul_rn(scale, g[j]));
+        g[j] = 0.f;
+      }
+    }
+  }
+}
+
 }  // namespace mb
 
 using namespace mb;
+
+extern "C" int merlot_clip_accumulate(float* acc, float* g, long long n, float clip_norm, double* scratch_f64, float* norm_out,
+                                      void* stream_) {
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
+  MB_REQUIRE(acc && g && scratch_f64, MERLOT_EINVAL, "clip_accumulate: null pointer");
+  MB_REQUIRE(acc != g, MERLOT_EINVAL, "clip_accumulate: acc and g must be different arenas");
+  MB_REQUIRE(clip_norm > 0.f && ((uintptr_t)g % 16) == 0 && ((uintptr_t)acc % 16) == 0, MERLOT_EINVAL,
+             "clip_accumulate: clip_norm must be > 0 and acc, g 16-byte aligned");
+  if (n <= 0) return MERLOT_OK;
+  MB_CHECK_CUDA(cudaMemsetAsync(scratch_f64, 0, sizeof(double), st));
+  const int grid = device_sms() * 8;
+  sumsq_kernel<<<grid, 256, 0, st>>>(g, n, scratch_f64);
+  MB_CHECK_LAUNCH();
+  clip_accumulate_kernel<<<grid, 256, 0, st>>>(acc, g, n, scratch_f64, clip_norm, norm_out);
+  MB_CHECK_LAUNCH();
+  return MERLOT_OK;
+}
 
 extern "C" int merlot_clip_by_global_norm(float* g, long long n, float clip_norm, double* scratch_f64, float* norm_out, void* stream_) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);

@@ -603,3 +603,13 @@ def adamw_step(p, g, m, v, p_bf16, n, beta1, omb1, beta2, omb2, eps, lr_t, wd, g
 
 def clip_by_global_norm(g, clip_norm, scratch_f64, norm_out):
     L.lib().merlot_clip_by_global_norm(g.data_ptr(), g.numel(), clip_norm, scratch_f64.data_ptr(), _ptr(norm_out), _stream())
+
+
+def clip_accumulate(acc, g, clip_norm, scratch_f64, norm_out):
+    """acc += g * clip_norm / max(||g||, clip_norm), then g = 0 (norm_out <- ||g||, on the device)."""
+    _require_cuda(acc, g, scratch_f64, norm_out)
+    if acc.numel() != g.numel() or acc.dtype != torch.float32 or g.dtype != torch.float32:
+        raise L.MerlotError(L.MERLOT_EINVAL, f"clip_accumulate: acc and g must be float32 of one length, got {acc.dtype} "
+                                             f"[{acc.numel()}] and {g.dtype} [{g.numel()}]")
+    L.lib().merlot_clip_accumulate(acc.data_ptr(), g.data_ptr(), g.numel(), clip_norm, scratch_f64.data_ptr(), _ptr(norm_out),
+                                   _stream())

@@ -59,12 +59,13 @@ class AdamOptimizer:
             raise ValueError("every parameter group has learning_rate 0: nothing would be trained")
         self._frozen = [(off, off + cnt) for h, off, cnt in store.groups if h[0] == 0]
 
-    def zero_frozen_grads(self):
+    def zero_frozen_grads(self, g: Optional[torch.Tensor] = None):
         """Variables with learning_rate 0 are removed from tvars before tf.gradients / clipping in the reference
         (utils/optimization.py:149-156): their accumulated gradients are discarded here so they neither enter the global norm
-        nor grow step after step."""
+        nor grow step after step.  `g`: the gradient arena (default store.g)."""
+        g = self.store.g if g is None else g
         for a, b in self._frozen:
-            self.store.g[a:b].zero_()
+            g[a:b].zero_()
 
     def scalars(self, hyper, step):
         lr, wd, b1, b2, eps = hyper
@@ -77,15 +78,18 @@ class AdamOptimizer:
         return dict(beta1=float(b1), omb1=float(np.float32(1.0) - b1), beta2=float(b2), omb2=float(np.float32(1.0) - b2),
                     eps=float(np.float32(eps)), lr_t=float(lr_t), wd=float(np.float32(wd)), lr=float(np.float32(lr) * scale))
 
-    def apply_gradients(self, grad_scale: float = 1.0, skip: Iterable[str] = (), zero_grad=True, only=None, advance=True):
+    def apply_gradients(self, grad_scale: float = 1.0, skip: Iterable[str] = (), zero_grad=True, only=None, advance=True,
+                        grads: Optional[torch.Tensor] = None):
         """One optimizer step on every parameter that received a gradient; `skip` lists parameters whose gradient is
         None in the reference (optimization.py:343-344 leaves those untouched).  `only` = [(a, b), ...] restricts the update
         to those arena ranges (data-parallel training updates the already all-reduced part while the rest is in flight);
-        pass advance=False for all but the last partial call of a step."""
+        pass advance=False for all but the last partial call of a step.  `grads` is the gradient arena to apply, in store.g's
+        layout (default store.g; a clipped accumulated step applies store.grad_accumulator())."""
         st = self.store
+        g = st.g if grads is None else grads
         step = st.global_step
         if zero_grad:
-            self.zero_frozen_grads()
+            self.zero_frozen_grads(g)
         skip_ranges = sorted((st.entries[n].offset, st.entries[n].offset + st.entries[n].padded) for n in skip)
         if only is not None:  # complement of `only` is skipped in this call
             cur, extra = 0, []
@@ -113,11 +117,11 @@ class AdamOptimizer:
             if cur < off + cnt:
                 segs.append((cur, off + cnt))
             for a, b in segs:
-                ops.adamw_step(st.p[a:b], st.g[a:b], st.m[a:b], st.v[a:b], st.pb[a:b], b - a, s["beta1"], s["omb1"], s["beta2"],
+                ops.adamw_step(st.p[a:b], g[a:b], st.m[a:b], st.v[a:b], st.pb[a:b], b - a, s["beta1"], s["omb1"], s["beta2"],
                                s["omb2"], s["eps"], s["lr_t"], s["wd"], grad_scale, zero_grad)
         if zero_grad and zero_ranges and advance:
             for a, b in zero_ranges:
-                st.g[a:b].zero_()
+                g[a:b].zero_()
         if advance:
             st.global_step += 1  # :251-253
 
@@ -128,11 +132,27 @@ class AdamOptimizer:
             return None
         st = self.store
         self.zero_frozen_grads()
+        self._clip_buffers()
+        ops.clip_by_global_norm(st.g, self.clip_norm, st._clip_scratch, st._clip_norm)
+        return st._clip_norm[0]
+
+    def clip_accumulate(self):
+        """One micro-batch of a step over A > 1 micro-batches with clip_norm > 0.  The reference clips every replica's own
+        gradient before CrossShardOptimizer averages them (utils/optimization.py:233-245), so each micro-batch is clipped
+        alone: the learning-rate-0 variables' gradients in store.g are zeroed, then store.grad_accumulator() += clipped
+        store.g and store.g = 0 (one K10c call).  Returns the micro-batch's pre-clip norm (0-d CUDA tensor, overwritten by
+        the next call)."""
+        st = self.store
+        self.zero_frozen_grads()
+        self._clip_buffers()
+        ops.clip_accumulate(st.grad_accumulator(), st.g, self.clip_norm, st._clip_scratch, st._clip_norm)
+        return st._clip_norm[0]
+
+    def _clip_buffers(self):
+        st = self.store
         if not hasattr(st, "_clip_scratch"):
             st._clip_scratch = torch.zeros(1, dtype=torch.float64, device=st.device)
             st._clip_norm = torch.zeros(1, dtype=torch.float32, device=st.device)
-        ops.clip_by_global_norm(st.g, self.clip_norm, st._clip_scratch, st._clip_norm)
-        return st._clip_norm[0]
 
     def current_lr(self):
         return float(np.float32(self.learning_rate) * learning_rate_scale(self.store.global_step, self.num_train_steps,

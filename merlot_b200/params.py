@@ -226,7 +226,17 @@ class ParamStore:
         if with_optimizer_state:
             self.m = torch.zeros(off, dtype=self.moment_dtype, device=self.device)
             self.v = torch.zeros(off, dtype=self.moment_dtype, device=self.device)
+        self.g_acc: Optional[torch.Tensor] = None  # grad_accumulator(): allocated by the first clipped accumulated step
         self.global_step = 0
+
+    def grad_accumulator(self) -> torch.Tensor:
+        """The second fp32 gradient arena, in g's layout, of a step with clip_norm > 0 over A > 1 micro-batches: it sums the
+        micro-batches' clipped gradients (optimization.AdamOptimizer.clip_accumulate), and the all-reduce and AdamW read it.
+        The backward pass keeps writing g, so no captured gradient pointer moves.  Allocated at first use (4 B per
+        parameter); zero between steps."""
+        if self.g_acc is None:
+            self.g_acc = torch.zeros_like(self.g)
+        return self.g_acc
 
     def vit_buckets(self, n_groups: int = 4):
         """Gradient buckets of the ViT for the data-parallel all-reduce, in BACKWARD order.  Returns (layer_groups, ranges):

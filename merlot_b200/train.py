@@ -151,23 +151,27 @@ def backward_and_apply(model, optimizer, dist: Optional[DataParallel], *, metric
                        d_hidden_state=None, d_contrastive_features=None, accum: int = 1):
     """The train op of every training step: model.backward (with an external head's gradient `d_hidden_state`, if any, whose
     parameter gradients are already in store.g, and the injected contrastive gradient `d_contrastive_features`), the gradient
-    mean over replicas and AdamW.  With clip_norm > 0 the pre-clip global norm goes into metrics['gradnorms/_overall'].
-    `accum` = A > 1: this is the last of A micro-batches whose gradients store.g already sums, and AdamW applies the mean
-    over the world * A virtual replicas."""
+    mean over replicas and AdamW.  With clip_norm > 0 the pre-clip global norm goes into metrics['gradnorms/_overall'] and is
+    returned (None without clipping).
+    `accum` = A > 1: this is the last of A micro-batches, whose earlier backward passes ran through backward_micro_batch,
+    and AdamW applies the mean over the world * A virtual replicas.  With clip_norm > 0 every micro-batch's gradient is
+    clipped alone (the reference's per-replica clip) into store.grad_accumulator(), which is then all-reduced and applied."""
     store = optimizer.store
     world = dist.world if dist is not None else 1
     grad_scale = 1.0 / (world * accum)
     bwd = dict(d_hidden_state=d_hidden_state, d_contrastive_features=d_contrastive_features)
     pending = []
     if optimizer.clip_norm > 0.0:  # local clip needs the complete local gradient first: no bucket overlap
-        if accum > 1:
-            raise NotImplementedError("clip_norm > 0 with gradient accumulation: the reference clips every replica's gradient "
-                                      "before the mean, which needs one gradient arena per micro-batch")
         model.backward(**bwd)
-        metrics["gradnorms/_overall"] = optimizer.clip_gradients()
+        if accum > 1:
+            norm, grads = optimizer.clip_accumulate(), store.grad_accumulator()
+        else:
+            norm, grads = optimizer.clip_gradients(), store.g
+        metrics["gradnorms/_overall"] = norm
         if world > 1:
-            dist.all_reduce_grads(store.g)
-        optimizer.apply_gradients(grad_scale=grad_scale, skip=skip, zero_grad=True)
+            dist.all_reduce_grads(grads)
+        optimizer.apply_gradients(grad_scale=grad_scale, skip=skip, zero_grad=True, grads=grads)
+        return norm
     elif world > 1:
         # Bucketed, overlapped gradient all-reduce (CrossShardOptimizer's mean, utils/optimization.py:241-245; the 1/world
         # is folded into AdamW).  Bucket 0 = everything outside the ViT, reduced while the ViT backward runs; the ViT is
@@ -196,6 +200,15 @@ def backward_and_apply(model, optimizer, dist: Optional[DataParallel], *, metric
     else:
         model.backward(**bwd)
         optimizer.apply_gradients(grad_scale=grad_scale, skip=skip, zero_grad=True)
+    return None
+
+
+def backward_micro_batch(model, optimizer, *, d_hidden_state=None, d_contrastive_features=None):
+    """model.backward of a micro-batch before the step's last.  Without clipping store.g accumulates (every gradient writer
+    adds).  With clip_norm > 0 the micro-batch's gradient, complete in store.g, is clipped into store.grad_accumulator() and
+    store.g is zeroed for the next micro-batch; returns its pre-clip norm (None without clipping)."""
+    model.backward(d_hidden_state=d_hidden_state, d_contrastive_features=d_contrastive_features)
+    return optimizer.clip_accumulate() if optimizer.clip_norm > 0.0 else None
 
 
 def accumulate_mean(bufs, acc: dict, metrics: dict, j: int, accum: int):
@@ -276,9 +289,6 @@ def model_fn_builder(config: NeatConfig, *, store: Optional[ParamStore] = None, 
         A = len(micro)
         if A < 1:
             raise ValueError("model_fn needs at least one micro-batch")
-        if optimizer.clip_norm > 0.0 and A > 1:
-            raise NotImplementedError("clip_norm > 0 with gradient accumulation: the reference clips every replica's gradient "
-                                      "before the mean, which needs one gradient arena per micro-batch")
         bufs = _Buffers(store)
         seeds = [replica_seed(seed, store.global_step, world, A, rank, j) for j in range(A)]
         # pass 1: every micro-batch's normalised features into rows [j*n, (j+1)*n) of the step's feature buffers
@@ -309,10 +319,12 @@ def model_fn_builder(config: NeatConfig, *, store: Optional[ParamStore] = None, 
                 accumulate_mean(bufs, acc, mj, j, A)
                 dc = (d_feat["lang"][j * n:(j + 1) * n], d_feat["viz"][j * n:(j + 1) * n])
                 if j + 1 < A:
-                    m2.backward(d_contrastive_features=dc)  # store.g accumulates: every gradient writer adds
+                    norm = backward_micro_batch(m2, optimizer, d_contrastive_features=dc)
                 else:
-                    backward_and_apply(m2, optimizer, dist, metrics=metrics, skip=skip, vit_grad_buckets=vit_grad_buckets,
-                                       d_contrastive_features=dc, accum=A)
+                    norm = backward_and_apply(m2, optimizer, dist, metrics=metrics, skip=skip,
+                                              vit_grad_buckets=vit_grad_buckets, d_contrastive_features=dc, accum=A)
+                if norm is not None and A > 1:
+                    accumulate_mean(bufs, acc, {"gradnorms/_overall": norm}, j, A)
             loss_parts[:] = [acc.pop("_lang"), contr_losses["loss_all"], acc.pop("_temp")]
             metrics.update(acc)
 

@@ -209,7 +209,7 @@ def vcr_model_fn_builder(config, *, store=None, dist=None, seed: int = 0, device
     from .config import replica_seed
     from .optimization import build_optimizer_from_config
     from .params import ParamStore
-    from .train import StepSpec, accumulate_mean, backward_and_apply
+    from .train import StepSpec, accumulate_mean, backward_and_apply, backward_micro_batch
     m_cfg = config.model
     if store is None:
         store = ParamStore(m_cfg, device=device, optimizer_cfg=config.optimizer, task="vcr")
@@ -227,9 +227,6 @@ def vcr_model_fn_builder(config, *, store=None, dist=None, seed: int = 0, device
 
     def accumulated_step(micro, labels):
         A = len(micro)
-        if optimizer.clip_norm > 0.0 and A > 1:
-            raise NotImplementedError("clip_norm > 0 with gradient accumulation: the reference clips every replica's gradient "
-                                      "before the mean, which needs one gradient arena per micro-batch")
         world, rank = (dist.world, dist.rank) if dist is not None else (1, 0)
         p = float(m_cfg.get("hidden_dropout_prob", 0.0) or 0.0)
         metrics = {"learning_rate": optimizer.current_lr()}
@@ -251,10 +248,12 @@ def vcr_model_fn_builder(config, *, store=None, dist=None, seed: int = 0, device
                 accumulate_mean(model._bufs, acc, {"loss": loss, "accuracy": accuracy}, j, A)
                 d_hidden = cls_head_backward(model, store, target)
                 if j + 1 < A:
-                    model.backward(d_hidden_state=d_hidden)  # store.g accumulates: every gradient writer adds
+                    norm = backward_micro_batch(model, optimizer, d_hidden_state=d_hidden)
                 else:
-                    backward_and_apply(model, optimizer, dist, metrics=metrics, vit_grad_buckets=vit_grad_buckets,
-                                       d_hidden_state=d_hidden, accum=A)
+                    norm = backward_and_apply(model, optimizer, dist, metrics=metrics, vit_grad_buckets=vit_grad_buckets,
+                                              d_hidden_state=d_hidden, accum=A)
+                if norm is not None and A > 1:
+                    accumulate_mean(model._bufs, acc, {"gradnorms/_overall": norm}, j, A)
             metrics.update(acc)
             loss_parts[:] = [acc["loss"]]
 
