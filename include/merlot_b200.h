@@ -345,6 +345,12 @@ int merlot_clip_accumulate(float* acc, float* g, long long n, float clip_norm, d
  * ------------------------------------------------------------------------------------------------------------ */
 /* is_valid of the joint sequence: viz part all true (modeling.py:106-107), lang part ids != 0 (:148) */
 int merlot_joint_valid(const int* ids, void* valid_u8, int B, int P, int L, void* stream);
+/* is_valid of the joint sequence with several images per text and an image mask (modeling.py:106-122,152): row b holds
+ * ni images of `span` viz tokens, then L language tokens.  img_mask_u8 [B / nt, ni] (NULL = all valid) is tiled to the nt
+ * texts of each image group and over each image's tokens: valid[b, t] = img_mask[b / nt, t / span] != 0 for t < ni * span;
+ * valid[b, ni * span + l] = ids[b, l] != 0.  nt must divide B. */
+int merlot_joint_valid_img(const int* ids, const void* img_mask_u8, void* valid_u8, int B, int nt, int ni, int span, int L,
+                           void* stream);
 /* rows of the masked positions in the joint sequence and their targets (modeling.py:533-536) */
 int merlot_mlm_index(const int* ids, const int* masked_idx, int* rows, int* targets, int B, int L, int k, int P, void* stream);
 /* allpairs_temporal_labels (modeling.py:598-620) + the 0.01/1.0 pair weights (:635,649-650) */

@@ -16,6 +16,21 @@ __global__ void joint_valid_kernel(const int* __restrict__ ids, uint8_t* __restr
   valid[i] = t < P ? 1 : (ids[(size_t)b * L + (t - P)] != 0);
 }
 
+// The same with an image mask (model/modeling.py:106-122,152): row b's vision part is ni images of `span` tokens each, and
+// token t < ni*span is valid iff img_mask[b / nt, t / span] != 0 (the mask is tiled to the nt texts of an image group, then
+// over each image's tokens); img_mask == null means every image is valid.  valid[b, ni*span + l] = ids[b, l] != 0.
+__global__ void joint_valid_img_kernel(const int* __restrict__ ids, const uint8_t* __restrict__ img_mask, uint8_t* __restrict__ valid,
+                                       int B, int nt, int ni, int span, int L) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int P = ni * span, Sj = P + L;
+  if (i >= (long long)B * Sj) return;
+  const int b = (int)(i / Sj), t = (int)(i % Sj);
+  if (t < P)
+    valid[i] = img_mask ? (img_mask[(size_t)(b / nt) * ni + t / span] != 0) : 1;
+  else
+    valid[i] = ids[(size_t)b * L + (t - P)] != 0;
+}
+
 // rows[b*k+m] = b*Sj + P + masked_idx[b,m]  (modeling.py:534 in joint-sequence coordinates); targets = input_ids there (:536)
 __global__ void mlm_index_kernel(const int* __restrict__ ids, const int* __restrict__ masked_idx, int* __restrict__ rows,
                                  int* __restrict__ targets, int B, int L, int k, int P) {
@@ -106,6 +121,19 @@ extern "C" int merlot_joint_valid(const int* ids, void* valid, int B, int P, int
   MB_REQUIRE(ids && valid, MERLOT_EINVAL, "joint_valid: null pointer");
   const long long n = (long long)B * (P + L);
   joint_valid_kernel<<<(unsigned)ceil_div_ll(n, 256), 256, 0, st>>>(ids, reinterpret_cast<uint8_t*>(valid), B, P, L);
+  MB_CHECK_LAUNCH();
+  return MERLOT_OK;
+}
+
+extern "C" int merlot_joint_valid_img(const int* ids, const void* img_mask, void* valid, int B, int nt, int ni, int span, int L,
+                                      void* stream_) {
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
+  MB_REQUIRE(ids && valid, MERLOT_EINVAL, "joint_valid_img: null pointer");
+  MB_REQUIRE(B > 0 && nt > 0 && B % nt == 0 && ni > 0 && span > 0 && L >= 0, MERLOT_ESHAPE,
+             "joint_valid_img: needs B > 0, nt > 0 dividing B, ni > 0, span > 0, L >= 0");
+  const long long n = (long long)B * ((long long)ni * span + L);
+  joint_valid_img_kernel<<<(unsigned)ceil_div_ll(n, 256), 256, 0, st>>>(ids, reinterpret_cast<const uint8_t*>(img_mask),
+                                                                      reinterpret_cast<uint8_t*>(valid), B, nt, ni, span, L);
   MB_CHECK_LAUNCH();
   return MERLOT_OK;
 }

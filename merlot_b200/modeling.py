@@ -250,6 +250,51 @@ class _Stack:
         return dh_in
 
 
+def check_num_imgs(cfg, batch_size, num_chunks, B, n_images, img_mask=None, mask_input=False, shuffled_idx_img=None,
+                   frame_copies=1):
+    """The several-images-per-text input of model/modeling.py:106-122 (`num_imgs` = ni, `img_mask`), checked on the host.
+    B is the joint encoder's batch (MerlotModel.B).  Returns ni.  With ni > 1 the reshapes at :112 and :121 hold only for
+    num_chunks == 1, and then `image` holds (batch_size // num_texts) * ni images, image group g = images g*ni .. g*ni+ni-1
+    for texts g*nt .. g*nt+nt-1.  `img_mask` is any bool or integer tensor of B // num_texts * ni entries (:109); non-zero
+    means valid.  Raises ValueError on shapes the reference cannot reshape, NotImplementedError on combinations
+    the reference cannot run or that no program of it uses."""
+    ni, nt = int(cfg.get("num_imgs", 1)), int(cfg.get("num_texts", 1))
+    if ni < 1:
+        raise ValueError(f"num_imgs must be >= 1, got {ni}")
+    new_path = ni > 1 or img_mask is not None
+    if not new_path:
+        return ni
+    if ni > 1 and shuffled_idx_img is not None:
+        raise NotImplementedError("num_imgs > 1 with shuffled_idx_img: the reference asserts num_imgs == 1 there "
+                                  "(model/modeling.py:319)")
+    if mask_input:
+        raise NotImplementedError("num_imgs > 1 / img_mask with mask_input=True: the pretraining heads index viz tokens through "
+                                  "P (one image per chunk) and model_fn never passes an img_mask")
+    if cfg.get("disable_pairwise_lang_attn", False):
+        raise NotImplementedError("num_imgs > 1 / img_mask with disable_pairwise_lang_attn: the reference builds a P + L segment "
+                                  "mask (model/modeling.py:162) for a P * num_imgs + L sequence")
+    if frame_copies > 1:
+        raise NotImplementedError("num_imgs > 1 / img_mask with frame_copies > 1 (the zero-shot story forward) is not provided")
+    max_vpe = int(cfg.get("max_vision_pos_embeddings", 1024))
+    if ni > max_vpe:
+        raise ValueError(f"num_imgs {ni} exceeds max_vision_pos_embeddings {max_vpe} (model/modeling.py:305-311)")
+    if ni > 1:
+        if num_chunks != 1:
+            raise ValueError(f"num_imgs {ni} > 1 needs num_chunks == 1 (the reshapes at model/modeling.py:112,121), "
+                             f"got num_chunks {num_chunks}")
+        if batch_size % nt != 0 or n_images != (batch_size // nt) * ni:
+            raise ValueError(f"image batch {n_images} != (batch_size {batch_size} // num_texts {nt}) x num_imgs {ni}"
+                             + ("" if batch_size % nt == 0 else " (batch_size is not a multiple of num_texts)"))
+    if img_mask is not None:
+        if img_mask.dtype.is_floating_point or img_mask.dtype.is_complex:
+            raise ValueError(f"img_mask must be a bool or integer tensor, got {img_mask.dtype}")
+        want = B // nt * ni
+        if B % nt != 0 or img_mask.numel() != want:
+            raise ValueError(f"img_mask has {img_mask.numel()} entries (shape {tuple(img_mask.shape)}); it must reshape to "
+                             f"[B // num_texts, num_imgs] = [{want // ni}, {ni}] (model/modeling.py:109)")
+    return ni
+
+
 class MerlotModel(object):
     def __init__(self, config, is_training, use_tpu, image, input_ids, mask_input=False, shuffled_idx_img=None,
                  img_mask=None, log_attention_probs=True, *, params: ParamStore, mask_draws: Optional[Dict] = None,
@@ -262,6 +307,10 @@ class MerlotModel(object):
         unshuffling scores two shuffles of each story, downstream/sort_story/get_zero_shot_logits.py:44-56): `image` holds
         batch_size // c groups of frames, `input_ids` and `shuffled_idx_img` hold batch_size groups, copy d of group s at
         s*c + d.  The ViT runs once per group of frames; each copy assembles its own viz tokens with its own image indices.
+
+        `num_imgs` = ni > 1 in the config and `img_mask` (model/modeling.py:106-122) put several images before every text:
+        `image` holds (batch_size // num_texts) * ni images, the joint sequence P * ni viz tokens then L language tokens, and
+        an image masked in `img_mask` [B // num_texts, ni] drops out of the joint attention (check_num_imgs has the rules).
 
         `features_only` runs what contrastive_features() needs and nothing more: the ViT, the language-only encoder and
         mask_inputs (with the dropout of is_training), but not the joint encoder, and it allows no backward.  The
@@ -290,8 +339,6 @@ class MerlotModel(object):
             raise L.MerlotError(L.MERLOT_EINVAL, "MerlotModel needs CUDA tensors: merlot_b200 has no CPU fallback")
         if not cfg.get("use_bfloat16", False):
             raise NotImplementedError("use_bfloat16: False (fp32 activations) is not provided; every shipped config sets True")
-        if cfg.get("num_imgs", 1) != 1 or img_mask is not None:
-            raise NotImplementedError("num_imgs > 1 / img_mask (model/modeling.py:106-122) not provided (no shipped config uses them)")
         if cfg.get("num_texts", 1) > 1 and (mask_input or shuffled_idx_img is not None):
             raise NotImplementedError("num_texts > 1 (VCR, model/modeling.py:111-119) is a finetuning/inference path: mask_input and "
                                       "shuffled_idx_img are not combined with it in the reference either (:319-320)")
@@ -312,7 +359,8 @@ class MerlotModel(object):
             self.num_chunks_in_group = cfg.get("num_chunks_in_group", self.num_chunks)
             assert self.num_chunks % self.num_chunks_in_group == 0  # :82
         self.input_ids = self.input_ids.to(torch.int32).contiguous()
-        self.num_imgs = cfg.get("num_imgs", 1)
+        self.num_imgs = check_num_imgs(cfg, self.batch_size, self.num_chunks, self.B, image.shape[0] if image.dim() == 4 else None,
+                                       img_mask, mask_input, shuffled_idx_img, frame_copies)
         self.num_texts = cfg.get("num_texts", 1)
         self.img_batch_size = self.batch_size // self.num_texts
         if not is_training:  # :88-90
@@ -329,7 +377,7 @@ class MerlotModel(object):
         # PREDICT-mode outputs of model_fn (model/modeling.py:762-770): encoder_info / lang_transformer_info['self_attn_probs']
         # = head-mean probabilities [B, layers, S, S].  Materialised only on request (60 MB per joint layer at configs[1]).
         self._export_probs = bool(export_attention_probs)
-        self._forward(image, shuffled_idx_img, mask_draws, mask_override)
+        self._forward(image, shuffled_idx_img, img_mask, mask_draws, mask_override)
 
     # ---- shapes (:226-260) ----
     @property
@@ -369,7 +417,7 @@ class MerlotModel(object):
         return self.store.P("word_embeddings/word_embeddings")
 
     # ---------------------------------------------------------------------------------------------------------
-    def _forward(self, image, shuffled_idx_img, mask_draws, mask_override):
+    def _forward(self, image, shuffled_idx_img, img_mask, mask_draws, mask_override):
         cfg, st, bf = self.config, self.store, self._bufs
         H = self.hidden_size
         dev = st.device
@@ -380,8 +428,8 @@ class MerlotModel(object):
         assert w0 % Pp == 0  # :190
         if c3 != 3:
             raise ValueError(f"image must be [N,h,w,3], got {tuple(image.shape)}")
-        nt, nc = self.num_texts, self.frame_copies
-        if N * nt * nc != self.batch_size * self.num_chunks:
+        nt, nc, ni = self.num_texts, self.frame_copies, self.num_imgs
+        if ni == 1 and N * nt * nc != self.batch_size * self.num_chunks:  # ni > 1: check_num_imgs
             raise ValueError(f"image batch {N} x num_texts {nt} x frame_copies {nc} != batch_size*num_chunks "
                              f"{self.batch_size * self.num_chunks}")
         ncls = cfg.get("num_cls_emb", 2)
@@ -393,7 +441,7 @@ class MerlotModel(object):
         h2, w2 = (h1 // sp, w1 // sp) if sp > 1 else (h1, w1)
         self.vision_transformer_info = {"num_h": h2, "num_w": w2}
         vcl, ncg, B, Lj = self.viz_chunk_length, self.num_chunks_in_group, self.B, self.L
-        Pz = self.P
+        Pz = self.P * ni  # the ni images of a text side by side (model/modeling.py:121)
         Sj = Pz + Lj
         self._dims = dict(N=N, h1=h1, w1=w1, np=np_, ncls=ncls, Sv=Sv, Mv=Mv, sp=max(sp, 1), h2=h2, w2=w2, vcl=vcl, Pz=Pz,
                           Sj=Sj, Kp=Pp * Pp * 3)
@@ -441,7 +489,7 @@ class MerlotModel(object):
         # ---- viz tokens (:95-133) ----
         if shuffled_idx_img is None:
             img_idx = bf.get("img_idx.arange", (N,), torch.int32)
-            img_idx.copy_(torch.arange(ncg, dtype=torch.int32, device=dev).repeat(B // (nt * nc)))
+            img_idx.copy_(torch.arange(ncg * ni, dtype=torch.int32, device=dev).repeat(B // (nt * nc)))  # :312-315
             self._shuffled = None
         else:
             assert self.num_imgs == 1 and self.num_texts == 1  # :319-320
@@ -482,7 +530,14 @@ class MerlotModel(object):
         # ---- joint encoder (:143-184) ----
         self._emb_j_ln = self._embed_words_into(self._ids_j, "position_embeddings", "emb_j", _SITE_EMB_J, joint_in, remap=(Lj, Sj, Pz))
         valid_j = bf.get("joint.valid", (B * Sj,), torch.uint8)
-        ops.joint_valid(self._ids_j, valid_j, B, Pz, Lj)
+        if ni > 1 or img_mask is not None:  # :106-122: image i of row b valid iff img_mask[b // nt, i], over its P tokens
+            mask_u8 = None
+            if img_mask is not None:
+                mask_u8 = bf.get("joint.img_mask", (B // nt, ni), torch.uint8)
+                mask_u8.copy_(img_mask.reshape(B // nt, ni) != 0)
+            ops.joint_valid_img(self._ids_j, mask_u8, valid_j, B, nt, ni, self.P, Lj)
+        else:
+            ops.joint_valid(self._ids_j, valid_j, B, Pz, Lj)
         c_viz = c_lang = None
         if self._log_attention_probs:  # split column sums of the joint attention maps for attention_log (:186-203)
             c_viz = bf.get("joint.c_viz", (B * Sj,), torch.float32, zero=True)

@@ -527,6 +527,11 @@ def joint_valid(ids, valid, B, P, Lseq):
     L.lib().merlot_joint_valid(ids.data_ptr(), valid.data_ptr(), B, P, Lseq, _stream())
 
 
+def joint_valid_img(ids, img_mask, valid, B, nt, ni, span, Lseq):
+    """img_mask: uint8 [B // nt, ni] on the device, or None (every image valid)."""
+    L.lib().merlot_joint_valid_img(ids.data_ptr(), _ptr(img_mask), valid.data_ptr(), B, nt, ni, span, Lseq, _stream())
+
+
 def mlm_index(ids, masked_idx, rows, targets, B, Lseq, k, P):
     L.lib().merlot_mlm_index(ids.data_ptr(), masked_idx.data_ptr(), rows.data_ptr(), targets.data_ptr(), B, Lseq, k, P, _stream())
 

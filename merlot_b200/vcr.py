@@ -45,11 +45,12 @@ def cls_head_val(model, head: Dict[str, torch.Tensor], mode: str = "answer") -> 
     """downstream/vcr/modeling.py:57-77 on model.encoder_hidden_states['lang'] -> fp32 logits [img_batch_size, 4]."""
     y = model.encoder_info["hidden_state"]  # bf16 [B, P+L, H]; encoder_hidden_states['lang'][:, 0] is its row P (cast to fp32 there)
     B, Sj, H = y.shape
+    lang0 = model.encoder_pieces[1]["start"]  # P * num_imgs: the language piece follows every image's viz tokens
     if B % 4 != 0:
         raise ValueError(f"VCR heads score 4 candidates per image: batch {B} is not a multiple of 4")
     dev = y.device
     first = torch.empty((B, H), dtype=torch.bfloat16, device=dev)
-    idx = (torch.arange(B, device=dev, dtype=torch.int32) * Sj + model.P).contiguous()
+    idx = (torch.arange(B, device=dev, dtype=torch.int32) * Sj + lang0).contiguous()
     ops.gather_rows(y.reshape(B * Sj, H), idx, first)  # hidden_state[:, 0, :] of the language piece
     k0 = head[f"{mode}_cls/classifier_mlp0/kernel"].to(torch.bfloat16).contiguous()
     pre = ops.gemm(first, k0, b_mn_major=True, bias=head[f"{mode}_cls/classifier_mlp0/bias"].float().contiguous(), out_dtype=torch.float32)
@@ -93,11 +94,12 @@ def head_from_store(store, mode: str = "answer") -> Dict[str, torch.Tensor]:
 
 
 def _head_index(model, b: int, Sj: int):
-    """Per tower: int32 [4b] rows of the joint hidden state (row P of every sequence of Sj rows) that the tower reads,
+    """Per tower: int32 [4b] rows of the joint hidden state (the first language row, P * num_imgs, of every sequence of Sj
+    rows) that the tower reads,
     question-major (row 4q + c = candidate text c of question q); plus the constant E fp32 [32, 4], E[8c, c] = 1, that moves
     logits between a tower's padded dense(1) output and the [2b, 4] logits (see cls_head)."""
     bf, dev = model._bufs, model.store.device
-    P = model.P
+    P = model.encoder_pieces[1]["start"]  # P * num_imgs
     key = ("_vcr_idx", b, Sj, P)
     if key not in bf.d:
         q = torch.arange(b, device=dev)[:, None]
