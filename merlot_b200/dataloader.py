@@ -29,10 +29,11 @@ import glob
 import io
 import itertools
 import math
+import os
 import queue
 import threading
 from concurrent.futures import ThreadPoolExecutor
-from typing import Dict, Iterator, List, Optional, Sequence
+from typing import Callable, Dict, Iterator, List, Optional, Sequence
 
 import numpy as np
 import torch
@@ -245,11 +246,22 @@ def shard_files(files: Sequence[str], rank: int, world: int) -> List[str]:
     return list(files)
 
 
-def interleave_records(names: Iterator[str], cycle_length: int, files: Sequence[str], stop: Optional[threading.Event] = None):
+def interleave_records(names: Iterator[str], cycle_length: int, files: Sequence[str], stop: Optional[threading.Event] = None,
+                       keep: Optional[Callable[[int], bool]] = None):
     """parallel_interleave(cycle_length, block_length=1) of TFRecord files: one record from each of `cycle_length` open files in
     turn, a file that ends replaced by the next of `names`.  Ends when `names` (finite for evaluation) and every open file are
-    exhausted or `stop` is set; raises ValueError when no file of `files` yields a record."""
-    readers = collections.deque(read_records(n) for n in itertools.islice(names, cycle_length))
+    exhausted or `stop` is set; raises ValueError when no file of `files` yields a record.
+
+    With `keep`, keep(i) is asked for the i-th record of the stream before its data is read; a record it declines is skipped
+    by read_records' header-only path and comes out as None, so the positions of the others do not move."""
+    if keep is None:
+        open_file = read_records
+    else:
+        position = [0]  # of the record the next yield carries: a reader asks keep() only when it has found one
+
+        def open_file(name):
+            return read_records(name, keep=lambda: keep(position[0]))
+    readers = collections.deque(open_file(n) for n in itertools.islice(names, cycle_length))
     ended_in_a_row = 0
     while readers and not (stop is not None and stop.is_set()):
         r = readers.popleft()
@@ -261,11 +273,26 @@ def interleave_records(names: Iterator[str], cycle_length: int, files: Sequence[
                 raise ValueError(f"no records in {list(files)}")
             name = next(names, None)
             if name is not None:
-                readers.append(read_records(name))
+                readers.append(open_file(name))
             continue
         ended_in_a_row = 0
         readers.append(r)
+        if keep is not None:
+            position[0] += 1
         yield rec
+
+
+DEFAULT_NUM_THREADS = 64  # data.num_threads when the config leaves it out
+
+
+def eval_decode_threads(data_cfg) -> int:
+    """Decode threads of one evaluation process: data.num_threads when the config sets it; otherwise the default 64 split
+    over the LOCAL_WORLD_SIZE processes of this host (at least 1), so N ranks on one host run as many decoders in all as
+    one process does.  The interleave's cycle_length keeps reading data.num_threads (or 64) on every rank: it fixes the
+    record order, which must not depend on the number of ranks."""
+    if "num_threads" in data_cfg:
+        return int(data_cfg["num_threads"])
+    return max(1, DEFAULT_NUM_THREADS // int(os.environ.get("LOCAL_WORLD_SIZE", "1")))
 
 
 def shuffled_records(files: Sequence[str], rng: np.random.Generator, cycle_length: int, buffer_size: int,

@@ -22,7 +22,8 @@ from typing import Dict, Iterable, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from .dataloader import DevicePipeline, decode_jpeg, interleave_records, plan_frames_eval, stage_frames
+from .dataloader import (DEFAULT_NUM_THREADS, DevicePipeline, decode_jpeg, eval_decode_threads, interleave_records,
+                         plan_frames_eval, stage_frames)
 from .tfrecord import parse_example
 
 NUM_CHUNKS = 5       # get_zero_shot_logits.py:26-28: five sentences and five frames per story
@@ -224,6 +225,23 @@ def batch_records(records: Iterable, batch_size: int, tail: List):
     tail.extend(batch)
 
 
+def eval_batches(files: Sequence[str], cycle_length: int, batch_size: int, tail: List, stop=None, rank: int = 0,
+                 world: int = 1):
+    """The evaluation record stream -- `files` in order, interleave_records over cycle_length readers, batch_records with
+    drop_remainder -- as rank `rank` of `world` sees it: the global batches k with k % world == rank, in order.  The set of
+    batches and their composition do not depend on `world`.  Every rank walks the whole stream to find the batch boundaries,
+    but reads another rank's records by their headers only (read_records' skip path): their data is never checksummed,
+    parsed or decoded here.  A last partial batch goes to `tail` (None in place of another rank's records), so len(tail) is
+    the global count of dropped records on every rank."""
+    if world == 1:
+        yield from batch_records(interleave_records(iter(files), cycle_length, files, stop), batch_size, tail)
+        return
+    recs = interleave_records(iter(files), cycle_length, files, stop, keep=lambda i: (i // batch_size) % world == rank)
+    for k, records in enumerate(batch_records(recs, batch_size, tail)):
+        if k % world == rank:
+            yield records
+
+
 def val_files(config) -> List[str]:
     """data.val_file: comma-separated globs, each sorted (list_files(shuffle=False))."""
     if "val_file_expanded" in config.data:
@@ -236,16 +254,19 @@ class StoryPipeline(DevicePipeline):
     """Iterator of evaluation batches {images [b*5, H, W, 3] bf16, sentences [b, 5, 32] int32 (both on `device`), story_id
     [b] and permutation_identity_encode [b] (int64 NumPy)} over the records of `files` in deterministic order: the files in
     the given order, interleaved over min(num_threads, files) readers, no shuffle, no repeat.  A last partial batch is not
-    returned; after the iteration ends `dropped` is the number of records it held."""
+    returned; after the iteration ends `dropped` is the number of records it held.  As rank `rank` of `world` evaluation
+    processes it returns the batches k with k % world == rank (eval_batches); `dropped` stays the global count."""
 
-    def __init__(self, config, files: Sequence[str], batch_size: int, device=None, prefetch: int = 2):
+    def __init__(self, config, files: Sequence[str], batch_size: int, device=None, prefetch: int = 2, rank: int = 0,
+                 world: int = 1):
         self.files = list(files)
         self.batch_size = batch_size
+        self.rank, self.world = rank, world
         self.out_size = tuple(config.model["image_size"])
-        num_threads = config.data.get("num_threads", 64)
+        num_threads = config.data.get("num_threads", DEFAULT_NUM_THREADS)
         self.cycle_length = min(num_threads, len(self.files))
         self.dropped = None
-        super().__init__(device, num_threads, prefetch)
+        super().__init__(device, eval_decode_threads(config.data), prefetch)
 
     def _batch(self, records):
         from . import ops
@@ -264,15 +285,15 @@ class StoryPipeline(DevicePipeline):
 
     def _produce(self):
         tail = []
-        recs = interleave_records(iter(self.files), self.cycle_length, self.files, self._stop)
-        for records in batch_records(recs, self.batch_size, tail):
+        for records in eval_batches(self.files, self.cycle_length, self.batch_size, tail, self._stop, self.rank, self.world):
             yield self._batch(records)
         self.dropped = len(tail)
 
 
-def input_fn_builder(config, batch_size: Optional[int] = None, device=None) -> StoryPipeline:
+def input_fn_builder(config, batch_size: Optional[int] = None, device=None, rank: int = 0, world: int = 1) -> StoryPipeline:
     """dataloader.py:111-170 with is_training=False: the story records of data.val_file, batches of `batch_size` (default
-    device.val_batch_size, 16 if unset) with drop_remainder.  Returns the running pipeline (an iterator; close() it)."""
+    device.val_batch_size, 16 if unset) with drop_remainder; rank `rank` of `world` gets the batches k with
+    k % world == rank.  Returns the running pipeline (an iterator; close() it)."""
     if config.model.get("num_chunks_in_group", NUM_CHUNKS) != NUM_CHUNKS:  # get_zero_shot_logits.py:28
         raise ValueError(f"zero-shot story unshuffling needs model.num_chunks_in_group == {NUM_CHUNKS}, "
                          f"got {config.model.get('num_chunks_in_group')}")
@@ -281,7 +302,7 @@ def input_fn_builder(config, batch_size: Optional[int] = None, device=None) -> S
         raise ValueError(f"data.val_file {config.data.get('val_file')!r} matches no file")
     if batch_size is None:
         batch_size = config.device.get("val_batch_size", 16)
-    return StoryPipeline(config, files, batch_size, device=device)
+    return StoryPipeline(config, files, batch_size, device=device, rank=rank, world=world)
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -364,13 +385,36 @@ def _story_rows(pred: Dict):
                "sentences": sents[i], "lang_viz_probs": probs["lang_viz_probs"][i], "viz_viz_probs": probs["viz_viz_probs"][i]}
 
 
+def gather_story_rows(config, prefix: str, group, seed: int = 1234) -> Tuple[List[List[Dict]], int]:
+    """Every rank of `group` restores `prefix` (restore_for_zero_shot) and runs zero_shot_predict on its batches
+    (input_fn_builder with the group's rank and world).  Returns, on every rank, the _story_rows of every batch in global
+    batch order and the number of records dropped.  A failure on any rank raises RankFailure on every rank."""
+    import torch
+
+    def own():
+        store = restore_for_zero_shot(config, prefix)
+        rows = []
+        with torch.no_grad(), input_fn_builder(config, rank=group.rank, world=group.world) as pipe:
+            for batch in pipe:
+                rows.append(list(_story_rows(zero_shot_predict(config, store, batch, seed=seed))))
+            return rows, pipe.dropped
+    from .eval_ranks import in_batch_order
+    per_rank = group.run_and_gather(own)
+    return in_batch_order([rows for rows, _ in per_rank]), per_rank[0][1]
+
+
 def main(argv=None) -> Dict:
     """`python -m merlot_b200.sort_story <yaml> [--out logits_val.h5|.npz]`: the story records of $SORTSTORY_PATH (or
     data.val_file when it is unset), the latest checkpoint of device.output_dir restored by name, one group per story
     written to --out, then the number of stories scored and dropped and score_permutations.py's three metrics.  Returns
-    the metrics."""
+    the metrics.
+
+    Under torchrun with WORLD_SIZE > 1 every rank scores its share of the batches (eval_batches) from the checkpoint rank 0
+    chose, and rank 0 writes the stories in the order one process writes them, prints and scores; every rank returns the
+    metrics."""
     import torch
     from .config import NeatConfig
+    from .eval_ranks import eval_group
     from .tf_checkpoint import latest_checkpoint
     ap = argparse.ArgumentParser(description="Zero-shot story unshuffling: temporal probabilities of every story and scores")
     ap.add_argument("config_file")
@@ -394,23 +438,32 @@ def main(argv=None) -> Dict:
     files = val_files(config)
     if not files:
         raise ValueError(f"SORTSTORY_PATH / data.val_file {config.data.get('val_file')!r} matches no file")
-    prefix = latest_checkpoint(str(config.device["output_dir"]))
-    if not prefix:
-        raise ValueError(f"device.output_dir {config.device['output_dir']!r} holds no checkpoint")
-    store = restore_for_zero_shot(config, prefix)
-    with input_fn_builder(config) as pipe:
-        def rows():
-            with torch.no_grad():
-                for batch in pipe:
-                    yield from _story_rows(zero_shot_predict(config, store, batch, seed=args.seed))
-        n = write(args.out, rows())
-        dropped = pipe.dropped
-    print(f"restored {prefix}; scored {n} stories, dropped {dropped} (the last partial batch of "
-          f"{config.device.get('val_batch_size', 16)}); wrote {args.out}", flush=True)
-    res = score_file(args.out)
-    print("Spearman:", res["spearman"], "Absolute Distance:", res["absolute_distance"], "Pairwise:", res["pairwise"],
-          sep="\n", flush=True)
-    return res
+    with eval_group() as group:
+        # rank 0 picks the checkpoint, so a checkpoint written meanwhile cannot split the ranks
+        prefix = group.broadcast(latest_checkpoint(str(config.device["output_dir"])) if group.rank == 0 else None)
+        if not prefix:
+            raise ValueError(f"device.output_dir {config.device['output_dir']!r} holds no checkpoint")
+        if group.world == 1:
+            store = restore_for_zero_shot(config, prefix)
+            with input_fn_builder(config) as pipe:
+                def rows():
+                    with torch.no_grad():
+                        for batch in pipe:
+                            yield from _story_rows(zero_shot_predict(config, store, batch, seed=args.seed))
+                n = write(args.out, rows())
+                dropped = pipe.dropped
+        else:
+            batches, dropped = gather_story_rows(config, prefix, group, seed=args.seed)
+            n = group.on_rank0(lambda: write(args.out, (row for rows in batches for row in rows)))
+
+        def report():
+            print(f"restored {prefix}; scored {n} stories, dropped {dropped} (the last partial batch of "
+                  f"{config.device.get('val_batch_size', 16)}); wrote {args.out}", flush=True)
+            res = score_file(args.out)
+            print("Spearman:", res["spearman"], "Absolute Distance:", res["absolute_distance"], "Pairwise:", res["pairwise"],
+                  sep="\n", flush=True)
+            return res
+        return group.broadcast(group.on_rank0(report))
 
 
 if __name__ == "__main__":

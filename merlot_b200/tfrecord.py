@@ -10,8 +10,9 @@ The varint, CRC-32C and protobuf field walkers are those of the checkpoint reade
 """
 from __future__ import annotations
 
+import os
 import struct
-from typing import Dict, Iterator, List, Union
+from typing import Callable, Dict, Iterator, List, Optional, Union
 
 import numpy as np
 
@@ -24,9 +25,14 @@ class RecordFormatError(ValueError):
     pass
 
 
-def read_records(path: str) -> Iterator[bytes]:
-    """The serialized records of one TFRecord file (uncompressed), in file order."""
+def read_records(path: str, keep: Optional[Callable[[], bool]] = None) -> Iterator[Optional[bytes]]:
+    """The serialized records of one TFRecord file (uncompressed), in file order.
+
+    With `keep`, it is asked before each record's data is read.  A record it declines has its 12-byte header read and its
+    length checksum verified, then its data and data checksum are skipped by seeking: they are never read or checksummed,
+    and None is yielded in the record's place.  A skipped record that runs past the end of the file still raises."""
     with open(path, "rb") as f:
+        size = os.fstat(f.fileno()).st_size if keep is not None else 0
         while True:
             head = f.read(12)
             if not head:
@@ -36,6 +42,11 @@ def read_records(path: str) -> Iterator[bytes]:
             if struct.unpack("<I", head[8:])[0] != mask_crc(crc32c(head[:8])):
                 raise RecordFormatError(f"{path}: record length checksum mismatch")
             (length,) = struct.unpack("<Q", head[:8])
+            if keep is not None and not keep():
+                if f.seek(length + 4, os.SEEK_CUR) > size:
+                    raise RecordFormatError(f"{path}: truncated record")
+                yield None
+                continue
             data = f.read(length)
             tail = f.read(4)
             if len(data) < length or len(tail) < 4:

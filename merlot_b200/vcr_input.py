@@ -25,10 +25,10 @@ from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
-from .dataloader import (DevicePipeline, decode_jpeg, interleave_records, plan_frames, plan_frames_eval, shard_files,
-                         shuffled_records, stage_frames, train_files)
+from .dataloader import (DEFAULT_NUM_THREADS, DevicePipeline, decode_jpeg, eval_decode_threads, plan_frames, plan_frames_eval,
+                         shard_files, shuffled_records, stage_frames, train_files)
 from .config import micro_batching
-from .sort_story import batch_records, val_files
+from .sort_story import eval_batches, val_files
 from .tfrecord import parse_example
 
 PADDING, START, END = 0, 2, 3  # utils/encode/encoder.py
@@ -175,21 +175,23 @@ class VCREvalPipeline(DevicePipeline):
     [b] (on `device`), annot_id, img_id (lists of str)} (dataloader.py:161-211 with is_training=False): the files in the given
     order, interleaved over min(data.num_threads, files) readers, no shuffle, no repeat.  `labelled=False` lets labels
     outside [0, 4) through (they are returned as read; no loss may be computed on them).  A last partial batch is not
-    returned; after the iteration ends `dropped` is the number of records it held."""
+    returned; after the iteration ends `dropped` is the number of records it held.  As rank `rank` of `world` evaluation
+    processes it returns the batches k with k % world == rank (sort_story.eval_batches); `dropped` stays the global count."""
 
     def __init__(self, config, files: Sequence[str], batch_size: int, mode: str, labelled: bool = True, device=None,
-                 prefetch: int = 2):
+                 prefetch: int = 2, rank: int = 0, world: int = 1):
         if mode not in MODES:
             raise ValueError(f"downstream.mode must be one of {MODES}, got {mode!r}")
         self.files = list(files)
         self.batch_size = batch_size
         self.mode, self.labelled = mode, labelled
+        self.rank, self.world = rank, world
         self.draw = config.data.get("draw", "segm")
         self.out_size = tuple(config.model["image_size"])
-        num_threads = config.data.get("num_threads", 64)
+        num_threads = config.data.get("num_threads", DEFAULT_NUM_THREADS)
         self.cycle_length = min(num_threads, len(self.files))
         self.dropped = None
-        super().__init__(device, num_threads, prefetch)
+        super().__init__(device, eval_decode_threads(config.data), prefetch)
 
     def _batch(self, records):
         modes = (self.mode,)
@@ -205,8 +207,7 @@ class VCREvalPipeline(DevicePipeline):
 
     def _produce(self):
         tail: List = []
-        recs = interleave_records(iter(self.files), self.cycle_length, self.files, self._stop)
-        for records in batch_records(recs, self.batch_size, tail):
+        for records in eval_batches(self.files, self.cycle_length, self.batch_size, tail, self._stop, self.rank, self.world):
             yield self._batch(records)
         self.dropped = len(tail)
 
@@ -216,7 +217,8 @@ def input_fn_builder(config, is_training: bool = True, rank: int = 0, world: int
     """dataloader_joint.input_fn_builder(is_training=True) or dataloader.input_fn_builder(is_training=False).  Training: the
     files of data.train_file sharded by rank (shard_files), batches of `batch_size` questions (default: the micro-batch of
     config.micro_batching, device.train_batch_size // world without device.micro_batch_size).  Evaluation: the files of data.val_file in sorted glob order, the downstream.mode
-    input, batches of `batch_size` questions (default device.val_batch_size).  Returns the running pipeline (close() it)."""
+    input, batches of `batch_size` questions (default device.val_batch_size), of which rank `rank` of `world` gets the
+    batches k with k % world == rank.  Returns the running pipeline (close() it)."""
     if is_training:
         files = train_files(config.data)
         if not files:
@@ -231,4 +233,4 @@ def input_fn_builder(config, is_training: bool = True, rank: int = 0, world: int
     if batch_size is None:
         batch_size = config.device.get("val_batch_size", 64)
     return VCREvalPipeline(config, files, batch_size, config.downstream.get("mode", "answer"), labelled=labelled,
-                           device=device)
+                           device=device, rank=rank, world=world)

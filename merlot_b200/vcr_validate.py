@@ -13,6 +13,11 @@ no dropout and no term across questions, so the means do not change.  One JSON l
 output_dir/eval/results.jsonl.  `--predictions PATH.npz` (with --checkpoint) also writes, per question, annot_id, img_id,
 log_prob [4], prediction and label: the reference's cls_metric / PREDICT dict.  `--unlabelled` scores records without
 labels: forward and head only, no loss, no accuracy and no results line.
+
+Under torchrun with WORLD_SIZE > 1 (eval_ranks): rank 0 alone follows device.output_dir and broadcasts each prefix it
+chooses, then "stop"; every rank restores the prefix and evaluates the global batches k with k % world == rank; every rank
+gathers the per-batch results in global batch order and computes the one-process result from them; rank 0 alone appends
+the results line and writes the predictions.  `--checkpoint`, `--chunk` and `--unlabelled` mean what they mean on one GPU.
 """
 from __future__ import annotations
 
@@ -21,7 +26,7 @@ import json
 import os
 import re
 import time
-from typing import Callable, Dict, Iterator
+from typing import Callable, Dict, Iterator, List
 
 import numpy as np
 
@@ -68,11 +73,15 @@ def log_softmax(logits: np.ndarray) -> np.ndarray:
 
 
 class Validator:
-    """Evaluates checkpoints of a VCR run on the evaluation input of config (data.val_file, downstream.mode)."""
+    """Evaluates checkpoints of a VCR run on the evaluation input of config (data.val_file, downstream.mode).  With an
+    eval_ranks.EvalGroup of several ranks, each rank evaluates the global batches k with k % world == rank, and every rank
+    gets the result one rank would compute."""
 
-    def __init__(self, config, chunk: int = 0, device="cuda"):
+    def __init__(self, config, chunk: int = 0, device="cuda", group=None):
+        from .eval_ranks import EvalGroup
         from .params import ParamStore
         from .vcr import vcr_model_fn_builder
+        self.group = group if group is not None else EvalGroup()
         self.config = config
         self.batch_size = int(config.device.get("val_batch_size", 64))
         self.chunk = chunk if chunk > 0 else self.batch_size
@@ -84,32 +93,57 @@ class Validator:
         self.model_fn = vcr_model_fn_builder(config, store=self.store, device=device)
         self.device = device
 
-    def evaluate(self, prefix: str, labelled: bool = True, keep_predictions: bool = False) -> Dict:
-        """Restore `prefix` and evaluate.  Returns {global_step, avg, loss, questions} (avg and loss None when not
-        labelled), plus per-question arrays under 'predictions' when keep_predictions."""
+    def _own_batches(self, prefix: str, labelled: bool, keep_predictions: bool) -> List[Dict]:
+        """Restore `prefix` and evaluate this rank's batches among the first num_batches.  Per batch: its loss (a device
+        scalar), the correct count of every chunk, and with keep_predictions every chunk's logits and the batch's ids and
+        labels.  With several ranks the tensors are copied to the host for the gather."""
         import torch
         from . import vcr_input
+        g = self.group
         self.store.restore_checkpoint(prefix)
         mode = "eval" if labelled else "predict"
-        losses, correct, logits, rows = [], [], [], {"annot_id": [], "img_id": [], "label": []}
-        with torch.no_grad(), vcr_input.input_fn_builder(self.config, is_training=False, batch_size=self.batch_size,
-                                                         device=self.device, labelled=labelled) as pipe:
-            for _, batch in zip(range(self.num_batches), pipe):
+        out = []
+        with torch.no_grad(), vcr_input.input_fn_builder(self.config, is_training=False, rank=g.rank, world=g.world,
+                                                         batch_size=self.batch_size, device=self.device,
+                                                         labelled=labelled) as pipe:
+            for _, batch in zip(range(len(range(g.rank, self.num_batches, g.world))), pipe):
                 batch_loss = torch.zeros((), dtype=torch.float32, device=self.device)
+                res = {"correct": [], "logits": []}
                 for a in range(0, self.batch_size, self.chunk):
                     feats = {k: batch[k][a:a + self.chunk] for k in ("images", "lm_input", "lm_targets")}
                     spec = self.model_fn(feats, None, mode)
                     n = feats["lm_targets"].shape[0]
                     if labelled:  # cls_loss gives chunk means; weigh them by the chunk's share of the batch
                         batch_loss += spec.metrics["loss"] * (n / self.batch_size)
-                        correct.append(spec.metrics["accuracy"] * n)
+                        res["correct"].append(spec.metrics["accuracy"] * n)
                     if keep_predictions:
-                        logits.append(spec.metrics["logits"].clone())
-                losses.append(batch_loss)
+                        res["logits"].append(spec.metrics["logits"].clone())
+                res["loss"] = batch_loss
                 if keep_predictions:
-                    rows["annot_id"] += batch["annot_id"]
-                    rows["img_id"] += batch["img_id"]
-                    rows["label"].append(batch["lm_targets"].cpu().numpy())
+                    res.update(annot_id=batch["annot_id"], img_id=batch["img_id"], label=batch["lm_targets"].cpu().numpy())
+                out.append(res)
+        if g.world > 1:  # host copies for the gather
+            for b in out:
+                b["loss"] = b["loss"].cpu()
+                b["correct"] = [c.cpu() for c in b["correct"]]
+                b["logits"] = [x.cpu() for x in b["logits"]]
+        return out
+
+    def evaluate(self, prefix: str, labelled: bool = True, keep_predictions: bool = False) -> Dict:
+        """Restore `prefix` and evaluate.  Returns {global_step, avg, loss, questions} (avg and loss None when not
+        labelled), plus per-question arrays under 'predictions' when keep_predictions.  With several ranks every rank
+        returns the same result, reduced in global batch order on this rank's device by the same operations one rank
+        runs; a failure on any rank raises RankFailure on every rank."""
+        import torch
+        from .eval_ranks import in_batch_order
+        per_rank = self.group.run_and_gather(lambda: self._own_batches(prefix, labelled, keep_predictions))
+        batches = in_batch_order(per_rank)
+        dev = self.device
+        losses = [b["loss"].to(dev) for b in batches]
+        correct = [c.to(dev) for b in batches for c in b["correct"]]
+        logits = [x.to(dev) for b in batches for x in b["logits"]]
+        rows = {"annot_id": [a for b in batches for a in b.get("annot_id", [])],
+                "img_id": [a for b in batches for a in b.get("img_id", [])], "label": [b["label"] for b in batches if "label" in b]}
         questions = len(losses) * self.batch_size
         if questions == 0:
             raise ValueError(f"data.val_file holds no whole batch of {self.batch_size} questions")
@@ -165,27 +199,32 @@ def main(argv=None, clock: Callable[[], float] = time.monotonic, sleep: Callable
     output_dir = str(config.device["output_dir"])
     if "://" in output_dir:
         raise ValueError(f"device.output_dir {output_dir!r}: only local directories are supported for checkpoints")
-    import torch
-    if torch.cuda.is_available():
-        torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
-    v = Validator(config, chunk=args.chunk)
-    if args.checkpoint:
-        prefixes = iter([args.checkpoint])
-    else:
-        prefixes = follow_checkpoints(output_dir, int(config.optimizer.get("num_train_steps", 10)),
-                                      float(config.validate.get("eval_timeout", 72000)), args.poll_interval, clock, sleep)
-    results = []
-    for prefix in prefixes:
-        res = v.evaluate(prefix, labelled=not args.unlabelled, keep_predictions=bool(args.predictions))
+    from .eval_ranks import eval_group
+
+    def follow(sleep_fn):
+        if args.checkpoint:
+            return iter([args.checkpoint])
+        return follow_checkpoints(output_dir, int(config.optimizer.get("num_train_steps", 10)),
+                                  float(config.validate.get("eval_timeout", 72000)), args.poll_interval, clock, sleep_fn)
+
+    def write(prefix, res):
         if args.predictions:
-            write_predictions(args.predictions, res.pop("predictions"))
+            write_predictions(args.predictions, res["predictions"])
         if not args.unlabelled:
             path = append_result(output_dir, res)
             print(f"{prefix}: global_step {res['global_step']} avg {res['avg']:.4f} loss {res['loss']:.4f} over "
                   f"{res['questions']} questions -> {path}", flush=True)
         else:
             print(f"{prefix}: predictions of {res['questions']} questions -> {args.predictions}", flush=True)
-        results.append(res)
+
+    results = []
+    with eval_group() as group:  # WORLD_SIZE > 1: rank 0 follows the checkpoints and writes, every rank evaluates
+        v = Validator(config, chunk=args.chunk, group=group)
+        for prefix in group.shared_prefixes(follow, sleep):
+            res = v.evaluate(prefix, labelled=not args.unlabelled, keep_predictions=bool(args.predictions))
+            group.on_rank0(lambda: write(prefix, res))
+            res.pop("predictions", None)
+            results.append(res)
     return results
 
 
