@@ -5,7 +5,8 @@ and metadata fields (`parse_text`), JPEG decoding with Pillow in a thread pool (
 resize_and_pad (`frame_draws`, `plan_frames`).  The per-pixel work -- convert, resize, crop, pad, augment, bf16 -- is K14
 (csrc/frames.cu, `ops.frames_prepare`) on a data stream of its own.  `input_fn_builder` (:129-278) ties them together.
 
-The random draws come from a NumPy generator keyed by (seed, rank), not from TensorFlow's bit stream, which cannot be
+The random draws come from a NumPy generator keyed by (seed, rank) -- (seed, batch index) for the evaluation input,
+EvalInputPipeline -- not from TensorFlow's bit stream, which cannot be
 reproduced without TensorFlow: the distributions are the reference's, the individual values are not.
 
 Batch-level step (`_process_example`, :210-272), below.  It runs on whatever device the feature tensors live on (plain index
@@ -31,6 +32,7 @@ import itertools
 import math
 import os
 import queue
+import re
 import threading
 from concurrent.futures import ThreadPoolExecutor
 from typing import Callable, Dict, Iterator, List, Optional, Sequence
@@ -406,6 +408,10 @@ class DevicePipeline:
         self.close()
 
 
+def _to_device(a: np.ndarray, device) -> torch.Tensor:
+    return torch.from_numpy(np.ascontiguousarray(a)).pin_memory().to(device, non_blocking=True)
+
+
 class InputPipeline(DevicePipeline):
     """Iterator of training batches in the feature dict model_fn takes (images [b*n, H, W, 3] bf16, input_ids [b, n, L],
     video_src_ids, shuffled_idx_img, plus youtube_id, chunk_num, mean_time and is_eoc), on `device`.
@@ -414,10 +420,12 @@ class InputPipeline(DevicePipeline):
     it packs a batch's frames into one pinned staging buffer, copies it to the device and runs K14 and `process_example` on
     the data stream.  `last_info` holds the records and draws behind the batch returned last (tests, debugging)."""
 
-    def __init__(self, config, files: Sequence[str], batch_size: int, rank: int = 0, seed: int = 0, device=None, prefetch: int = 2):
+    def __init__(self, config, files: Sequence[str], batch_size: int, rank: int = 0, seed: int = 0, device=None, prefetch: int = 2,
+                 decode_threads: Optional[int] = None):
         self.data_cfg, self.model_cfg = dict(config.data), dict(config.model)
         self.files = list(files)
         self.batch_size = batch_size
+        self.rank, self.seed = rank, seed
         self.num_chunks = self.data_cfg.get("num_chunks", self.model_cfg.get("num_chunks_in_group", 4))
         self.chunk_text_len = self.data_cfg.get("chunk_text_len", 32)
         self.out_size = tuple(self.model_cfg["image_size"])
@@ -425,53 +433,162 @@ class InputPipeline(DevicePipeline):
         self.cycle_length = min(num_threads, len(self.files))
         self.shuffle_buffer_size = self.data_cfg.get("shuffle_buffer_size", 256)
         self.rng = np.random.default_rng([seed, rank])
-        super().__init__(device, num_threads, prefetch)
+        super().__init__(device, decode_threads or num_threads, prefetch)
 
     # -- one batch --
-    def _batch(self, records):
+    def _batch(self, records, rng: np.random.Generator, k: Optional[int] = None):
+        """`_dataset_parser` of every record, with the clean-ASR coins and frame draws taken from `rng`, then K14, then
+        `_finish` (the training pipeline's process_example).  `k`, the global batch index, names records in errors."""
         b, n = self.batch_size, self.num_chunks
         Hd, Wd = self.out_size
         examples = [parse_example(r) for r in records]
         decodes = [self._pool.submit(decode_jpeg, jpg) for ex in examples for jpg in frame_bytes(ex, n)]
-        do_clean = self.rng.random(b) < self.data_cfg.get("clean_asr_prob", 0.5)  # sample_bernoulli, one per example (:101-102)
+        do_clean = rng.random(b) < self.data_cfg.get("clean_asr_prob", 0.5)  # sample_bernoulli, one per example (:101-102)
         text = [parse_text(ex, n, self.chunk_text_len, bool(c)) for ex, c in zip(examples, do_clean)]
-        draws = frame_draws(self.rng, b * n, self.data_cfg)
-        process_seed = int(self.rng.integers(1 << 62))
+        self._check(examples, text, k)
+        draws = frame_draws(rng, b * n, self.data_cfg)
+        info = {"records": list(records), "do_clean": do_clean, "frame_draws": draws}
+        finish = self._finisher(rng, info)
         staging, offsets, hw = stage_frames([d.result() for d in decodes])
         plan = plan_frames(hw[:, 0], hw[:, 1], self.out_size, draws["scale"], draws["u_y"], draws["u_x"])
         plan.update(src_offset=offsets, src_h=hw[:, 0], src_w=hw[:, 1], method=draws["method"], augment=draws["augment"],
                     factor=draws["factor"])
+        info["plan"] = plan
 
         from . import ops
         dev = self.device
         src = staging.to(dev, non_blocking=True)
         images = ops.frames_prepare(src, plan, Hd, Wd)
-        feats = {k: torch.from_numpy(np.stack([t[k] for t in text])).pin_memory().to(dev, non_blocking=True) for k in text[0]}
+        feats = {key: _to_device(np.stack([t[key] for t in text]), dev) for key in text[0]}
         feats["images"] = images.view(b, n, Hd, Wd, 3)
+        return finish(feats), info
+
+    def _check(self, examples, text, k):
+        """Host checks of a parsed batch before anything of it reaches the device (the evaluation input's)."""
+
+    def _finisher(self, rng: np.random.Generator, info: dict):
+        """The batch-level step, as a function of the device features: process_example with draws seeded from `rng`."""
+        b, n = self.batch_size, self.num_chunks
+        process_seed = int(rng.integers(1 << 62))
         g = self.model_cfg.get("num_chunks_in_group", n)
-        pdraws = make_draws(b, n, g, self.model_cfg.get("image_shuffle_prob", 0.5), process_seed, dev)
-        feats = process_example(feats, self.data_cfg, self.model_cfg, is_training=True, draws=pdraws)
-        info = {"records": list(records), "do_clean": do_clean, "frame_draws": draws, "plan": plan,
-                "process_draws": {k: v.cpu() for k, v in pdraws.items()}}
-        return feats, info
+
+        def finish(feats):
+            pdraws = make_draws(b, n, g, self.model_cfg.get("image_shuffle_prob", 0.5), process_seed, self.device)
+            info["process_draws"] = {k: v.cpu() for k, v in pdraws.items()}
+            return process_example(feats, self.data_cfg, self.model_cfg, is_training=True, draws=pdraws)
+        return finish
 
     def _produce(self):
         recs = shuffled_records(self.files, self.rng, self.cycle_length, self.shuffle_buffer_size, self._stop)
         while not self._stop.is_set():
-            yield self._batch([next(recs) for _ in range(self.batch_size)])  # batch(drop_remainder=True) of a repeated stream
+            # batch(drop_remainder=True) of a repeated stream
+            yield self._batch([next(recs) for _ in range(self.batch_size)], self.rng)
+
+
+_CHUNK_FRAME_KEY = re.compile(r"c(\d\d)/image/encoded")
+
+
+def _record_name(example, i: int, k: Optional[int]) -> str:
+    yid = _scalar(example, "c00/youtube_id", b"")
+    where = f"record {i} of evaluation batch {k}" if k is not None else f"record {i} of its batch"
+    return f"{where} (c00/youtube_id {bytes(yid).decode('utf-8', 'replace')!r})"
+
+
+class EvalInputPipeline(InputPipeline):
+    """Iterator of pretraining evaluation batches (model/dataloader.py:129-278 with is_training=False) on `device`:
+    images [b*n, H, W, 3] bf16 (not transposed), input_ids [b, n, L], video_src_ids, is_eoc, youtube_id, chunk_num,
+    mean_time and the identity shuffled_idx_img = tile(arange(num_chunks_in_group)) -- what process_example emits at
+    image_shuffle_prob < 1e-6; the reference applies no process_example here (DESIGN.md 2 item 8).
+
+    The records of `files` in order, interleaved over min(num_threads, files) readers, no repeat and no shuffle buffer, cut
+    into batches of `batch_size` with drop_remainder.  Global batch k goes whole to rank k % world (sort_story.eval_batches:
+    another rank's records are skipped by their headers).  Batch k's parser draws -- the clean-ASR coin per example and
+    frame_draws per frame -- come from a generator keyed by (seed, k), so they do not depend on the rank, the world size or
+    the checkpoint.  Every index a record gives the model (its chunk count, video_src_ids, token ids) is checked on the host
+    before its batch reaches the device; a bad one raises ValueError naming the record.  After the iteration ends
+    `dropped` is the global number of records in the last partial batch."""
+
+    def __init__(self, config, files: Sequence[str], batch_size: int, rank: int = 0, world: int = 1, seed: int = 0, device=None,
+                 prefetch: int = 2):
+        n = config.data.get("num_chunks", config.model.get("num_chunks_in_group", 4))
+        g = config.model.get("num_chunks_in_group", n)
+        if (batch_size * n) % g != 0:
+            raise ValueError(f"val_batch_size {batch_size} x data.num_chunks {n} = {batch_size * n} is not divisible by "
+                             f"model.num_chunks_in_group {g}")
+        max_vpe = int(config.model.get("max_vision_pos_embeddings", 1024))
+        if g > max_vpe:
+            raise ValueError(f"shuffled_idx_img of the evaluation input reaches {g - 1}: model.num_chunks_in_group {g} exceeds "
+                             f"max_vision_pos_embeddings {max_vpe}")
+        self.world = world
+        self.vocab_size = int(config.model.get("vocab_size", 50370))
+        self.dropped = None
+        super().__init__(config, files, batch_size, rank=rank, seed=seed, device=device, prefetch=prefetch,
+                         decode_threads=eval_decode_threads(config.data))
+
+    def _check(self, examples, text, k):
+        n = self.num_chunks
+        for i, (ex, t) in enumerate(zip(examples, text)):
+            chunks = sorted(int(m.group(1)) for m in map(_CHUNK_FRAME_KEY.fullmatch, ex) if m)
+            if chunks != list(range(n)):
+                raise ValueError(f"{_record_name(ex, i, k)}: {len(chunks)} chunks {chunks}, data.num_chunks is {n}")
+            vid = t["video_src_ids"]
+            if vid.min() < 0 or vid.max() >= n:
+                raise ValueError(f"{_record_name(ex, i, k)}: video_src_ids {vid.tolist()} outside [0, {n})")
+            ids = t["input_ids"]
+            if ids.min() < 0 or ids.max() >= self.vocab_size:
+                raise ValueError(f"{_record_name(ex, i, k)}: token id {int(ids.max() if ids.max() >= self.vocab_size else ids.min())} "
+                                 f"outside the vocabulary [0, {self.vocab_size})")
+
+    def _finisher(self, rng, info):
+        b, n = self.batch_size, self.num_chunks
+        g = self.model_cfg.get("num_chunks_in_group", n)
+
+        def finish(feats):
+            out = dict(feats)
+            out["images"] = feats["images"].reshape(b * n, *self.out_size, 3)
+            out["shuffled_idx_img"] = torch.arange(g, dtype=torch.int32, device=self.device).repeat(b * n // g)
+            return out
+        return finish
+
+    def _produce(self):
+        from .sort_story import eval_batches
+        tail = []
+        for j, records in enumerate(eval_batches(self.files, self.cycle_length, self.batch_size, tail, self._stop, self.rank,
+                                                 self.world)):
+            k = self.rank + j * self.world
+            feats, info = self._batch(records, eval_rng(self.seed, k), k)
+            info["batch"] = k
+            yield feats, info
+        self.dropped = len(tail)
+
+
+def eval_rng(seed: int, k: int) -> np.random.Generator:
+    """The generator of evaluation batch k's parser draws: keyed by (seed, k) only."""
+    return np.random.default_rng([seed, k])
 
 
 def input_fn_builder(config, is_training: bool = True, rank: int = 0, world: int = 1, seed: int = 0,
                      batch_size: Optional[int] = None, device=None) -> InputPipeline:
-    """model/dataloader.py:129-278 for training: the files of data.train_file (sharded by rank when world > 1), interleaved
+    """model/dataloader.py:129-278.  Training: the files of data.train_file (sharded by rank when world > 1), interleaved
     over min(num_threads, files) readers, a shuffle buffer of shuffle_buffer_size records, the parser, batches of
     `batch_size` (default: the micro-batch of config.micro_batching, device.train_batch_size // world without
-    device.micro_batch_size) with drop_remainder, and `process_example`.  Returns the running pipeline (an iterator of
-    feature dicts; close() it)."""
-    if not is_training:
-        raise NotImplementedError("only the training input is provided (val_file / eval input is not)")
+    device.micro_batch_size) with drop_remainder, and `process_example`.
+
+    Evaluation (is_training=False): EvalInputPipeline over the sorted globs of data.val_file, batches of `batch_size`
+    (default device.val_batch_size, 16 if unset); rank `rank` of `world` gets the global batches k with k % world == rank,
+    and batch k's draws are keyed by (seed, k).  An empty or unmatched data.val_file raises ValueError.
+
+    Returns the running pipeline (an iterator of feature dicts; close() it)."""
     if config.data.get("unbatch_size", 1) > 1:
         raise NotImplementedError("data.unbatch_size > 1 is not provided")
+    if not is_training:
+        from .sort_story import val_files
+        files = val_files(config)
+        if not files:
+            raise ValueError(f"data.val_file {config.data.get('val_file')!r} matches no file")
+        if batch_size is None:
+            batch_size = int(config.device.get("val_batch_size", 16))
+        return EvalInputPipeline(config, files, batch_size, rank=rank, world=world, seed=seed, device=device)
     files = train_files(config.data)
     if not files:
         raise ValueError(f"data.train_file {config.data.get('train_file')!r} matches no file")

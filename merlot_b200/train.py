@@ -247,30 +247,33 @@ def model_fn_builder(config: NeatConfig, *, store: Optional[ParamStore] = None, 
     skip = variables_without_gradient(config.model, store)
     world, rank = (dist.world, dist.rank) if dist is not None else (1, 0)
 
-    def build_model(features, dropout_seed, transpose=True, **kw):
+    def build_model(features, dropout_seed, transpose=True, replicas=dist, **kw):
         imgs = features["images"]
         if transpose and config.model.get("transpose_input", False) and imgs.shape[-1] != 3:
             imgs = imgs.permute(3, 0, 1, 2).contiguous()  # [H,W,3,N] -> [N,H,W,3], modeling.py:683-685
         return MerlotModel(config=config.model, is_training=True,  # the reference hard-codes True (:693, SURVEY quirk 3)
                            image=imgs, input_ids=features["input_ids"], use_tpu=config.device.get("use_tpu", False),
                            shuffled_idx_img=features.get("shuffled_idx_img", None), mask_input=True, params=store,
-                           dropout_seed=dropout_seed, dist=dist, **kw)
+                           dropout_seed=dropout_seed, dist=replicas, **kw)
 
     def temporal_loss(model, features):
         if config.model.get("temporal_coef", 1.0) > 0.0:
             return model.temporal_loss(features["shuffled_idx_img"], video_src_ids=features["video_src_ids"])
         return torch.zeros((), device=store.device), {}
 
-    def metrics_of(model, lang_losses, contr_losses, temp_losses):
+    def metrics_of(model, lang_losses, contr_losses, temp_losses, learning_rate=True):
         losses = {f"lang/{k}": v for k, v in lang_losses.items()}
         losses.update({f"contr/{k}": v for k, v in contr_losses.items()})
         losses.update({f"temporal/{k}": v for k, v in temp_losses.items()})
-        losses["learning_rate"] = optimizer.current_lr()
+        if learning_rate:  # a train metric (modeling.py:720-725); eval_metrics take `losses` alone (:708-711, :788-798)
+            losses["learning_rate"] = optimizer.current_lr()
         if log_attention_probs:  # modeling.py:709  losses.update(model.attention_log)
             losses.update({f"attn/{k}": v for k, v in model.attention_log.items()})
         return losses
 
     def model_fn(features, labels=None, mode="train", params=None):
+        if mode == "eval":
+            return eval_step(features, int((params or {}).get("eval_batch", 0)))
         if isinstance(features, (list, tuple)):
             return accumulated_step(list(features))
         model = build_model(features, seed + store.global_step * world + rank, transpose=mode == "train",
@@ -284,6 +287,22 @@ def model_fn_builder(config: NeatConfig, *, store: Optional[ParamStore] = None, 
             backward_and_apply(model, optimizer, dist, metrics=losses, skip=skip, vit_grad_buckets=vit_grad_buckets)
 
         return StepSpec(model, (lang_loss, contr_loss, temp_loss), losses, train_op)
+
+    def eval_step(features, k):
+        """EVAL mode (modeling.py:691-711, :788-798) on evaluation batch k: the training forward as the reference builds it
+        (is_training=True, mask_input=True), keeping nothing for a backward, with no collective (one batch is one replica:
+        its contrastive negatives are its own videos) and with the dropout and masking seed eval_seed(seed, k).  Returns a
+        StepSpec whose metrics are the `losses` dict without learning_rate, whose `total_loss` is lang + contr + temporal
+        (device scalars, which the next model on this store overwrites) and whose train_op is None."""
+        model = build_model(features, eval_seed(seed, k), transpose=False, replicas=None, save_for_backward=False,
+                            log_attention_probs=log_attention_probs)
+        lang_loss, lang_losses = model.mask_loss()
+        contr_loss, contr_losses = model.contrastive_loss()
+        temp_loss, temp_losses = temporal_loss(model, features)
+        spec = StepSpec(model, (lang_loss, contr_loss, temp_loss),
+                        metrics_of(model, lang_losses, contr_losses, temp_losses, learning_rate=False), None)
+        spec.total_loss = lang_loss + contr_loss + temp_loss
+        return spec
 
     def accumulated_step(micro):
         A = len(micro)
@@ -335,6 +354,12 @@ def model_fn_builder(config: NeatConfig, *, store: Optional[ParamStore] = None, 
     model_fn.store = store
     model_fn.optimizer = optimizer
     return model_fn
+
+
+def eval_seed(seed: int, k: int) -> int:
+    """Dropout and masking seed of evaluation batch k: a function of the run seed and k only, so every checkpoint and every
+    rank count draws the same masks for batch k (the reference reseeds from the clock)."""
+    return seed + k
 
 
 def _step_for(config: NeatConfig):
