@@ -634,6 +634,8 @@ __global__ void __launch_bounds__(256) ce_bwd_kernel(const float* __restrict__ l
 }
 
 static inline uint32_t thresh16(float p) { return (uint32_t)(p * 65536.0f + 0.5f); }
+// the row-wise kernels move 16 bytes per access (a null pointer passes: optional operands are checked where they are used)
+static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 }  // namespace mb
 
@@ -644,7 +646,10 @@ extern "C" int merlot_layernorm_fwd(const merlot_ln_t* d, void* stream_) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
   MB_REQUIRE(d && d->x && d->y && d->gamma && d->beta, MERLOT_EINVAL, "layernorm_fwd: null pointer");
   MB_REQUIRE(d->H % 8 == 0 && d->H <= 1024 && d->H > 0, MERLOT_ESHAPE, "layernorm: H must be a multiple of 8, <= 1024 (got %d)", d->H);
-  MB_REQUIRE(d->ld_x % 8 == 0 && d->ld_y % 8 == 0, MERLOT_ESHAPE, "layernorm: leading dims must be multiples of 8");
+  MB_REQUIRE(d->ld_x % 8 == 0 && d->ld_y % 8 == 0 && d->ld_x >= d->H && d->ld_y >= d->H, MERLOT_ESHAPE,
+             "layernorm: leading dims must be multiples of 8 and >= H (ld_x %d, ld_y %d, H %d)", d->ld_x, d->ld_y, d->H);
+  MB_REQUIRE(aligned16(d->x) && aligned16(d->y) && aligned16(d->gamma) && aligned16(d->beta), MERLOT_ESHAPE,
+             "layernorm: x, y, gamma, beta must be 16-byte aligned");
   if (d->rows == 0) return MERLOT_OK;
   const uint32_t th = d->dropout_p > 0.f ? thresh16(d->dropout_p) : 0;
   const float sc = d->dropout_p > 0.f ? 1.f / (1.f - d->dropout_p) : 1.f;
@@ -670,6 +675,14 @@ extern "C" int merlot_layernorm_bwd(const merlot_ln_bwd_t* d, void* stream_) {
   MB_REQUIRE(d && d->dy && d->x && d->mean && d->rstd && d->gamma && d->dx && d->workspace && d->dgamma && d->dbeta, MERLOT_EINVAL,
              "layernorm_bwd: null pointer");
   MB_REQUIRE(d->H % 8 == 0 && d->H <= 1024 && d->H > 0, MERLOT_ESHAPE, "layernorm_bwd: H must be a multiple of 8, <= 1024");
+  const bool dres_ok = d->dres == nullptr || (d->ld_dres % 8 == 0 && d->ld_dres >= d->H);
+  MB_REQUIRE(d->ld_dy % 8 == 0 && d->ld_x % 8 == 0 && d->ld_dx % 8 == 0 && d->ld_dy >= d->H && d->ld_x >= d->H && d->ld_dx >= d->H &&
+             dres_ok, MERLOT_ESHAPE, "layernorm_bwd: leading dims must be multiples of 8 and >= H (ld_dy %d, ld_x %d, ld_dres %d, "
+             "ld_dx %d, H %d)", d->ld_dy, d->ld_x, d->ld_dres, d->ld_dx, d->H);
+  MB_REQUIRE(aligned16(d->dy) && aligned16(d->x) && aligned16(d->gamma) && aligned16(d->dres) && aligned16(d->dx), MERLOT_ESHAPE,
+             "layernorm_bwd: dy, x, gamma, dres, dx must be 16-byte aligned");
+  MB_REQUIRE((d->x_f32 != 0) == (d->dx_f32 != 0), MERLOT_EINVAL, "layernorm_bwd: unsupported dtype combination x_f32=%d dy_f32=%d dx_f32=%d",
+             d->x_f32, d->dy_f32, d->dx_f32);
   if (d->rows == 0) return MERLOT_OK;
   const uint32_t th = d->dropout_p > 0.f ? thresh16(d->dropout_p) : 0;
   const float sc = d->dropout_p > 0.f ? 1.f / (1.f - d->dropout_p) : 1.f;
@@ -686,8 +699,7 @@ extern "C" int merlot_layernorm_bwd(const merlot_ln_bwd_t* d, void* stream_) {
   if (!d->x_f32 && !d->dy_f32 && !d->dx_f32) LNB(bf16, bf16, bf16);
   else if (d->x_f32 && !d->dy_f32 && d->dx_f32) LNB(float, bf16, float);
   else if (d->x_f32 && d->dy_f32 && d->dx_f32) LNB(float, float, float);
-  else if (!d->x_f32 && d->dy_f32 && !d->dx_f32) LNB(bf16, float, bf16);
-  else return set_error(MERLOT_EINVAL, "layernorm_bwd: unsupported dtype combination x_f32=%d dy_f32=%d dx_f32=%d", d->x_f32, d->dy_f32, d->dx_f32);
+  else LNB(bf16, float, bf16);
 #undef LNB
   MB_CHECK_LAUNCH();
   reduce_partials_kernel<<<dim3(ceil_div(2 * d->H, 256), RSPLIT), 256, 0, st>>>(part, grid, 2 * d->H, d->dgamma, d->dbeta, d->H);
@@ -703,6 +715,10 @@ extern "C" int merlot_layernorm_bwd_fused(const void* dy, const void* x, const f
   MB_REQUIRE(dy && x && mean && rstd && gamma && dx && dgamma && dbeta, MERLOT_EINVAL, "layernorm_bwd_fused: null pointer");
   MB_REQUIRE(H % 8 == 0 && H > 0 && H <= 1024, MERLOT_ESHAPE, "layernorm_bwd_fused: H must be a multiple of 8, <= 1024 (got %d)", H);
   MB_REQUIRE(dropout_p <= 0.f || (dmask && dbias), MERLOT_EINVAL, "layernorm_bwd_fused: dropout needs dmask and dbias");
+  // bulk copies and 16-byte stores on the rows, float4 loads of gamma, red.global.add.v4.f32 on the accumulators
+  MB_REQUIRE(aligned16(dy) && aligned16(x) && aligned16(dres) && aligned16(dx) && aligned16(dmask) && aligned16(gamma) &&
+             aligned16(dgamma) && aligned16(dbeta) && aligned16(dbias), MERLOT_EINVAL,
+             "layernorm_bwd_fused: dy, x, dres, dx, dmask, gamma, dgamma, dbeta, dbias must be 16-byte aligned");
   if (rows == 0) return MERLOT_OK;
   const uint32_t th = dropout_p > 0.f ? thresh16(dropout_p) : 0;
   const float sc = dropout_p > 0.f ? 1.f / (1.f - dropout_p) : 1.f;
@@ -710,9 +726,6 @@ extern "C" int merlot_layernorm_bwd_fused(const void* dy, const void* x, const f
   const int sms = num_sms();
   const int grid = (int)(want < sms ? want : sms);
   const size_t smem = lnf_smem_bytes(H);
-  MB_REQUIRE(((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dres) |
-               reinterpret_cast<uintptr_t>(dx) | reinterpret_cast<uintptr_t>(dmask)) & 15) == 0, MERLOT_EINVAL,
-             "layernorm_bwd_fused: dy, x, dres, dx, dmask must be 16-byte aligned");
   (void)workspace;
 #define LNF(N_)                                                                                                          \
   do {                                                                                                                   \
@@ -735,7 +748,9 @@ extern "C" int merlot_bias_grad(const void* dy, int dy_f32, int ld, long long ro
                                 uint64_t seed, uint32_t site, void* stream_) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
   MB_REQUIRE(dy && out, MERLOT_EINVAL, "bias_grad: null pointer");
-  MB_REQUIRE(N % 8 == 0 && ld % 8 == 0, MERLOT_ESHAPE, "bias_grad: N and ld must be multiples of 8");
+  MB_REQUIRE(N % 8 == 0 && ld % 8 == 0 && ld >= N, MERLOT_ESHAPE, "bias_grad: N and ld must be multiples of 8, ld >= N (N %d, ld %d)",
+             N, ld);
+  MB_REQUIRE(aligned16(dy), MERLOT_ESHAPE, "bias_grad: dy must be 16-byte aligned");
   if (rows == 0) return MERLOT_OK;
   const uint32_t th = dropout_p > 0.f ? thresh16(dropout_p) : 0;
   const float sc = dropout_p > 0.f ? 1.f / (1.f - dropout_p) : 1.f;
