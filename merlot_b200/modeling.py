@@ -33,6 +33,7 @@ START = 2
 _SITE_VIT, _SITE_LANGONLY, _SITE_JOINT, _SITE_EMB_LO, _SITE_EMB_J = 0, 100, 200, 300, 301
 # VCR classifier towers (merlot_b200/vcr.py cls_head): dropout of each tower's input and of its hidden layer
 _SITE_VCR_ANS_IN, _SITE_VCR_ANS_HID, _SITE_VCR_RAT_IN, _SITE_VCR_RAT_HID = 400, 401, 402, 403
+_VIT = "vision_backbone/vision_transformer"
 
 
 def get_shape_list_rank(t: torch.Tensor, expected_rank, name="tensor"):
@@ -193,6 +194,15 @@ def _layer_params(store: ParamStore, scope: str, layers: int):
     return arr
 
 
+def _grid_idxmap(bufs: _Buffers, nh: int, nw: int):
+    key = ("_grid", nh, nw)
+    if key not in bufs.d:
+        i = torch.arange(nh, device=bufs.dev)[:, None]
+        j = torch.arange(nw, device=bufs.dev)[None]
+        bufs.d[key] = (i * 64 + j).reshape(-1).to(torch.int32)
+    return bufs.d[key]
+
+
 class _Stack:
     """One transformer stack invocation (utils/transformer.py:171-247) through merlot_stack_forward/backward."""
 
@@ -248,6 +258,146 @@ class _Stack:
                 on_group_done(k)
         d.bwd_lo, d.bwd_hi = 0, 0
         return dh_in
+
+
+class _Embedding:
+    """embed_words (:262-297) of int32 ids [G, Lseq] into the rows of `out` through `remap`, run at construction."""
+
+    def __init__(self, store, bufs, cfg, tag, scope, ids, out, remap, dropout):
+        R, Lseq = ids.numel(), ids.shape[1]
+        if Lseq > cfg["max_position_embeddings"]:  # tf.assert_less_equal, utils/model_utils.py:282
+            raise ValueError(f"sequence length {Lseq} exceeds max_position_embeddings {cfg['max_position_embeddings']}")
+        self.st, self.bf, self.tag, self.scope, self.ids = store, bufs, tag, scope, ids
+        xsum = bufs.get(f"{tag}.xsum", (R, cfg["hidden_size"]), torch.float32)
+        ops.embed_fwd(ids, store.P("word_embeddings/word_embeddings"), store.P(f"{scope}/position_embeddings"), xsum, Lseq)
+        self.ln = _LayerNorm(store, f"{scope}/LayerNorm_embed_norm", xsum, bufs.get(f"{tag}.mean", (R,), torch.float32),
+                             bufs.get(f"{tag}.rstd", (R,), torch.float32), rows=R, remap=remap, dropout=dropout)
+        self.ln.forward(out)
+
+    def backward(self, dy):
+        st, (G, Lseq) = self.st, self.ids.shape
+        dx = self.ln.backward(dy, self.bf.get(f"bwd.dxsum.{self.tag}", self.ln.x.shape, torch.float32))
+        ops.scatter_add_rows(dx, self.ids.reshape(-1), st.G("word_embeddings/word_embeddings"))
+        ops.group_rowsum(dx, G, Lseq, 0, Lseq, None, st.G(f"{self.scope}/position_embeddings"), dx.shape[1])
+
+
+class _VitInput:
+    """The ViT input (utils/vision_transformer.py:189-232) of NHWC bf16 images, run at construction: the patch conv2d, or the
+    hybrid stem (:206-223) and its 1x1 conv_postresnet_proj; cls / position embeddings; the pre-LN into bf16 `out`."""
+
+    def __init__(self, store, bufs, cfg, img, save):
+        N, h0, w0, _ = img.shape
+        H, Pp, ncls, resnet_layers = cfg["hidden_size"], cfg["patch_size"], cfg.get("num_cls_emb", 2), cfg.get("resnet_layers")
+        self.st, self.bf, self.N, self.h1, self.w1, self.ncls = store, bufs, N, h0 // Pp, w0 // Pp, ncls
+        Mp, Mv = N * self.h1 * self.w1, N * (self.h1 * self.w1 + ncls)
+        patch = bufs.get("vit.patch", (Mp, H), torch.float32)
+        self.stem = None
+        if not resnet_layers:
+            self.proj, self.a = f"{_VIT}/conv2d", bufs.get("vit.A", (Mp, Pp * Pp * 3), torch.bfloat16)
+            ops.patch_im2col(img, self.a, Pp)
+        else:  # the stem, then conv_postresnet_proj: 1x1 with bias, not weight-standardised
+            if Pp != 16:
+                raise ValueError("the hybrid ResNet stem needs patch_size 16 (utils/vision_transformer.py:208)")
+            self.proj, self.stem = f"{_VIT}/conv_postresnet_proj", HybridStem(store, bufs, list(resnet_layers), save)
+            self.a, hs, ws_ = self.stem.forward(img, N, h0, w0)
+            if (hs, ws_) != (self.h1, self.w1):
+                raise ValueError(f"stem output {hs}x{ws_} != patch grid {self.h1}x{self.w1}")
+        ops.gemm(self.a, store.W(f"{self.proj}/kernel"), b_mn_major=True, bias=store.P(f"{self.proj}/bias"), out=patch)
+        xsum = bufs.get("vit.xsum", (Mv, H), torch.float32)
+        ops.vit_assemble_fwd(patch, store.P(f"{_VIT}/pos_embs/pos_embs"), store.P(f"{_VIT}/pos_embs/cls_emb"), xsum, N, self.h1,
+                             self.w1, ncls, H)
+        self.out = bufs.get("vit.h0", (Mv, H), torch.bfloat16)
+        self.ln = _LayerNorm(store, f"{_VIT}/LayerNorm_ctx_patches_pre_ln", xsum, bufs.get("vit.mean0", (Mv,), torch.float32),
+                             bufs.get("vit.rstd0", (Mv,), torch.float32))
+        self.ln.forward(self.out)
+
+    def backward(self, dy):
+        """dy: bf16 gradient of `out`.  Returns the gradient HybridStem.backward took (bf16, shaped as its output) or None."""
+        st, bf, N, ncls, H, np_ = self.st, self.bf, self.N, self.ncls, dy.shape[1], self.h1 * self.w1
+        dx = self.ln.backward(dy, bf.get("bwd.dxsum_v", self.ln.x.shape, torch.float32))
+        ops.group_rowsum(dx, N, np_ + ncls, 0, ncls, None, st.G(f"{_VIT}/pos_embs/cls_emb"), H)
+        ops.group_rowsum(dx, N, np_ + ncls, ncls, np_, _grid_idxmap(bf, self.h1, self.w1), st.G(f"{_VIT}/pos_embs/pos_embs"), H)
+        dpatch = bf.get("bwd.dpatch", (N * np_, H), torch.bfloat16)
+        ops.vit_assemble_bwd(dx, dpatch, N, np_, ncls, H)
+        ops.bias_grad(dpatch, st.G(f"{self.proj}/bias"), rows=N * np_, N=H)
+        ops.gemm(self.a, dpatch, a_mn_major=True, b_mn_major=True, out=st.G(f"{self.proj}/kernel"), atomic=True,
+                 M=self.a.shape[1], N=H, K=N * np_)
+        if self.stem is not None:
+            d_rc = bf.get("bwd.d_rc", self.a.shape, torch.bfloat16)
+            ops.gemm(dpatch, st.W(f"{self.proj}/kernel"), out=d_rc)  # [M, H] . [Cr, H]^T
+            self.stem.backward(d_rc)
+            return d_rc
+
+
+class _VizTokens:
+    """The viz tokens (:95-133) of the ViT output hv on the patch grid geom = (N, h1, w1, ncls, sp), run at construction: for
+    each of the nc frame copies, viz_assemble_fwd, then LayerNorm_final_ln into the joint-input rows of each of its nt texts."""
+
+    def __init__(self, store, bufs, hv, img_idx, joint_in, geom, Pz, Sj, nt, nc):
+        N, H, Bi = geom[0], hv.shape[1], joint_in.shape[0] // (Sj * nt * nc)  # Bi image groups
+        self.st, self.bf, self.img_idx, self.geom = store, bufs, img_idx, geom
+        # joint-input rows of copy d, text j (model/modeling.py:111-119): image group g's Pz rows at (g*nc*nt + d*nt + j) * Sj
+        self.remaps = [[(Pz, nt * nc * Sj, (d * nt + j) * Sj) for j in range(nt)] for d in range(nc)]
+        xsum = bufs.get("viz.xsum", (Bi * Pz, H), torch.float32)
+        self.img_trg = bufs.get("viz.img_trg", (N, H), torch.float32)
+        self.ln = _LayerNorm(store, "vision_backbone/LayerNorm_final_ln", xsum, bufs.get("viz.mean", (Bi * Pz,), torch.float32),
+                             bufs.get("viz.rstd", (Bi * Pz,), torch.float32), rows=Bi * Pz)
+        for d in range(nc):  # copy d of image group g: its own image indices, joint rows of group g*nc + d
+            idx_d = img_idx if img_idx.numel() == N else img_idx.view(Bi, nc, -1)[:, d].contiguous()
+            ops.viz_assemble_fwd(hv, store.P("vision_backbone/img_idx_pe"), idx_d, store.P("vision_backbone/final_pe/pos_embs"),
+                                 store.P("vision_backbone/final_pe/cls_emb"), xsum, self.img_trg, *geom, H)
+            for remap in self.remaps[d]:
+                self.ln.forward(joint_in, remap=remap)
+
+    def backward(self, d_joint_in, d_img_trg):
+        """The gradient of the one frame copy a backward allows (nc == 1); returns d_hv bf16, shaped as hv."""
+        st, bf, (N, h1, w1, ncls, sp), H = self.st, self.bf, self.geom, d_img_trg.shape[1]
+        dx = None
+        for j, remap in enumerate(self.remaps[0]):  # the nt texts of an image group all send gradient into its viz tokens
+            dx = self.ln.backward(d_joint_in, bf.get(f"bwd.dxsum_z.{j & 1}", self.ln.x.shape, torch.float32), dres=dx, remap=remap)
+        d_hv = bf.get("bwd.d_hv", (N * (h1 * w1 + ncls), H), torch.bfloat16)
+        ops.viz_assemble_bwd(dx, d_img_trg, d_hv, *self.geom, H)
+        h2, w2 = h1 // sp, w1 // sp
+        ops.segment_rowsum_scatter(dx, N, h2 * w2 + 1, self.img_idx, st.G("vision_backbone/img_idx_pe"), H)
+        ops.group_rowsum(dx, N, h2 * w2 + 1, 0, 1, None, st.G("vision_backbone/final_pe/cls_emb"), H)
+        ops.group_rowsum(dx, N, h2 * w2 + 1, 1, h2 * w2, _grid_idxmap(bf, h2, w2), st.G("vision_backbone/final_pe/pos_embs"), H)
+        return d_hv
+
+
+class _LangOnly:
+    """langonly_reps (:339-379) of model.input_ids with hidden dropout p, run at construction: the ids regrouped by
+    langonly_num_chunks_in_group, _Embedding, _Stack, and each chunk's first row gathered into fp32 `lang_trg`."""
+
+    def __init__(self, model, p):
+        cfg, st, bf, Lc, nch = model.config, model.store, model._bufs, model.lang_chunk_length, model.num_chunks
+        g = cfg.get("langonly_num_chunks_in_group", nch)
+        assert nch // g > 0 and nch % g == 0
+        ids = model.input_ids.reshape(-1, Lc * g).contiguous()
+        (Blo, Llo), H, layers = ids.shape, model.hidden_size, cfg["num_lang_transformer_hidden_layers"]
+        h0 = bf.get("lo.h0", (Blo * Llo, H), torch.bfloat16)
+        self.emb = _Embedding(st, bf, cfg, "emb_lo", "langonly_embeddings", ids, h0, (0, 0, 0), (p, model._seed, _SITE_EMB_LO))
+        valid = bf.get("lo.valid", (Blo * Llo,), torch.uint8)
+        ops.ids_valid(ids, valid)
+        summ = bf.get("lo.attn_summ", (Blo * Llo,), torch.float32, zero=True)
+        probs = bf.get("lo.probs", (layers, Blo, Llo, Llo), torch.float32) if model._export_probs else None
+        self.stack = _Stack(st, bf, "lo", "encoder", layers, Blo, Llo, valid, h0, cfg, p, model._seed, _SITE_LANGONLY,
+                            model._save_arenas, colsum=summ, probs=probs)
+        y = self.stack.forward()
+        self.bf, nrows = bf, model.batch_size * nch
+        self.pool_idx = bf.get("lo.pool_idx", (nrows,), torch.int32)
+        self.pool_idx.copy_(torch.arange(nrows, dtype=torch.int32, device=st.device) * Lc)
+        self.lang_trg = bf.get("lo.lang_trg", (nrows, H), torch.float32)
+        ops.gather_rows(y, self.pool_idx, self.lang_trg)
+        # lang_transformer_info; attention_summs of mask_inputs (:428-431): sum over (layers, queries) of head-mean probs, [B, L]
+        self.info = {"hidden_state": y.view(Blo, Llo, H), "attention_summs": summ.view(model.B, model.L)}
+        if probs is not None:
+            self.info["self_attn_probs"] = probs.permute(1, 0, 2, 3)
+
+    def backward(self, d_lang_trg):
+        d_y = self.bf.get("bwd.d_ylo", self.stack.y.shape, torch.bfloat16, zero=True)
+        ops.scatter_add_rows(d_lang_trg, self.pool_idx, d_y)
+        d_h0 = self.bf.get("bwd.d_h0lo", self.stack.y.shape, torch.bfloat16)
+        self.emb.backward(self.stack.backward(d_y, d_h0))
 
 
 def check_num_imgs(cfg, batch_size, num_chunks, B, n_images, img_mask=None, mask_input=False, shuffled_idx_img=None,
@@ -344,8 +494,6 @@ class MerlotModel(object):
                                       "shuffled_idx_img are not combined with it in the reference either (:319-320)")
         if not cfg.get("share_params", True):
             raise NotImplementedError("share_params: False (separate langonly_encoder, model/modeling.py:361) not provided yet")
-        # hybrid ResNet-lite stem (utils/vision_transformer.py:206-223) instead of the 16x16 patch embedding: forward provided
-        self._resnet_layers = list(cfg.get("resnet_layers", []) or [])
 
         input_ids_shape = get_shape_list_rank(input_ids, [2, 3], "input_ids")
         if len(input_ids_shape) == 2:  # :72-77
@@ -434,21 +582,15 @@ class MerlotModel(object):
                              f"{self.batch_size * self.num_chunks}")
         ncls = cfg.get("num_cls_emb", 2)
         h1, w1 = h0 // Pp, w0 // Pp
-        np_ = h1 * w1
-        Sv = np_ + ncls
-        Mv = N * Sv
-        sp = cfg["spatial_pool_size"]
-        h2, w2 = (h1 // sp, w1 // sp) if sp > 1 else (h1, w1)
-        self.vision_transformer_info = {"num_h": h2, "num_w": w2}
-        vcl, ncg, B, Lj = self.viz_chunk_length, self.num_chunks_in_group, self.B, self.L
+        Sv = h1 * w1 + ncls
+        sp = max(cfg["spatial_pool_size"], 1)
+        self.vision_transformer_info = {"num_h": h1 // sp, "num_w": w1 // sp}
+        ncg, B, Lj = self.num_chunks_in_group, self.B, self.L
         Pz = self.P * ni  # the ni images of a text side by side (model/modeling.py:121)
         Sj = Pz + Lj
-        self._dims = dict(N=N, h1=h1, w1=w1, np=np_, ncls=ncls, Sv=Sv, Mv=Mv, sp=max(sp, 1), h2=h2, w2=w2, vcl=vcl, Pz=Pz,
-                          Sj=Sj, Kp=Pp * Pp * 3)
-        train = self.is_training
-        p_hid = float(cfg["hidden_dropout_prob"] or 0.0)
-        p_vit = float(cfg.get("vit_hidden_dropout_prob", cfg["hidden_dropout_prob"]) or 0.0) if train else 0.0
-        vt = "vision_backbone/vision_transformer"
+        self._dims = dict(N=N, Sv=Sv, Pz=Pz, Sj=Sj)
+        p_hid = float(cfg["hidden_dropout_prob"] or 0.0)  # 0 unless training (:88-90)
+        p_vit = float(cfg.get("vit_hidden_dropout_prob", cfg["hidden_dropout_prob"]) or 0.0) if self.is_training else 0.0
 
         # ---- language-only encoder (:135-137) on a side stream: it only needs input_ids, and its small latency-bound grids
         # fill the SMs the ViT kernels leave idle.  Joined before mask_inputs.
@@ -456,62 +598,32 @@ class MerlotModel(object):
         if self._mask_input:
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
-                self._langonly_reps()
+                self._lo = _LangOnly(self, p_hid)
+            self.lang_trg_h, self.lang_transformer_info = self._lo.lang_trg, self._lo.info
 
         # ---- ViT (utils/vision_transformer.py:173-274) ----
-        img = image if image.dtype == torch.bfloat16 else image.to(torch.bfloat16)
-        img = img.contiguous()
-        patch = bf.get("vit.patch", (N * np_, H), torch.float32)
-        self._stem = self.d_rc = None  # d_rc: the gradient backward() hands to the hybrid stem
-        if not self._resnet_layers:
-            self._patch_A = bf.get("vit.A", (N * np_, Pp * Pp * 3), torch.bfloat16)
-            ops.patch_im2col(img, self._patch_A, Pp)
-            ops.gemm(self._patch_A, st.W(f"{vt}/conv2d/kernel"), b_mn_major=True, bias=st.P(f"{vt}/conv2d/bias"), out=patch)
-        else:  # hybrid stem (:206-223): lite_resnet50 -> 1x1 conv_postresnet_proj with bias (not standardised)
-            if Pp != 16:
-                raise ValueError("the hybrid ResNet stem needs patch_size 16 (utils/vision_transformer.py:208)")
-            self._stem = HybridStem(st, bf, self._resnet_layers, self._save_arenas)
-            self._rc, hs, ws_ = self._stem.forward(img, N, h0, w0)
-            if (hs, ws_) != (h1, w1):
-                raise ValueError(f"stem output {hs}x{ws_} != patch grid {h1}x{w1}")
-            ops.gemm(self._rc, st.W(f"{vt}/conv_postresnet_proj/kernel"), b_mn_major=True,
-                     bias=st.P(f"{vt}/conv_postresnet_proj/bias"), out=patch)
-        xsum_v = bf.get("vit.xsum", (Mv, H), torch.float32)
-        ops.vit_assemble_fwd(patch, st.P(f"{vt}/pos_embs/pos_embs"), st.P(f"{vt}/pos_embs/cls_emb"), xsum_v, N, h1, w1, ncls, H)
-        h0_v = bf.get("vit.h0", (Mv, H), torch.bfloat16)
-        self._vit_ln = _LayerNorm(st, f"{vt}/LayerNorm_ctx_patches_pre_ln", xsum_v, bf.get("vit.mean0", (Mv,), torch.float32),
-                                  bf.get("vit.rstd0", (Mv,), torch.float32))
-        self._vit_ln.forward(h0_v)
-        self._vit = _Stack(st, bf, "vit", vt, cfg.get("num_vision_transformer_hidden_layers", cfg["num_hidden_layers"]), N, Sv,
-                           None, h0_v, cfg, p_vit, self._seed, _SITE_VIT, self._save_arenas)
+        img = image.to(torch.bfloat16).contiguous()
+        self._vit_in = _VitInput(st, bf, cfg, img, self._save_arenas)
+        self._stem, self.d_rc = self._vit_in.stem, None  # d_rc: the gradient backward() hands to the hybrid stem
+        self._vit = _Stack(st, bf, "vit", _VIT, cfg.get("num_vision_transformer_hidden_layers", cfg["num_hidden_layers"]), N,
+                           Sv, None, self._vit_in.out, cfg, p_vit, self._seed, _SITE_VIT, self._save_arenas)
         hv = self._vit.forward()
 
         # ---- viz tokens (:95-133) ----
         if shuffled_idx_img is None:
             img_idx = bf.get("img_idx.arange", (N,), torch.int32)
             img_idx.copy_(torch.arange(ncg * ni, dtype=torch.int32, device=dev).repeat(B // (nt * nc)))  # :312-315
-            self._shuffled = None
         else:
             assert self.num_imgs == 1 and self.num_texts == 1  # :319-320
             img_idx = shuffled_idx_img.reshape(-1).to(torch.int32).contiguous()
             if img_idx.numel() != N * nc:
                 raise ValueError(f"shuffled_idx_img has {img_idx.numel()} entries, expected B*num_chunks_in_group = {N * nc}")
-        self._img_idx = img_idx
-        Bi = B // (nt * nc)  # image groups; with num_texts > 1 every group's tokens are tiled to its nt texts (model/modeling.py:111-119)
-        xsum_z = bf.get("viz.xsum", (Bi * Pz, H), torch.float32)
-        self.img_trg_h = bf.get("viz.img_trg", (N, H), torch.float32)
         joint_in = bf.get("joint.in", (B * Sj, H), torch.bfloat16)
-        self._viz_ln = _LayerNorm(st, "vision_backbone/LayerNorm_final_ln", xsum_z, bf.get("viz.mean", (Bi * Pz,), torch.float32),
-                                  bf.get("viz.rstd", (Bi * Pz,), torch.float32), rows=Bi * Pz)
-        for d in range(nc):  # copy d of image group g: its own image indices, joint rows of group g*nc + d
-            idx_d = img_idx if img_idx.numel() == N else img_idx.view(Bi, nc, ncg)[:, d].contiguous()
-            ops.viz_assemble_fwd(hv, st.P("vision_backbone/img_idx_pe"), idx_d, st.P("vision_backbone/final_pe/pos_embs"),
-                                 st.P("vision_backbone/final_pe/cls_emb"), xsum_z, self.img_trg_h, N, h1, w1, ncls, max(sp, 1), H)
-            for j in range(nt):  # image group g feeds joint rows of texts g*nt + j: row remap (group stride nt*Sj, offset j*Sj)
-                self._viz_ln.forward(joint_in, remap=(Pz, nt * nc * Sj, (d * nt + j) * Sj))
+        self._viz = _VizTokens(st, bf, hv, img_idx, joint_in, (N, h1, w1, ncls, sp), Pz, Sj, nt, nc)
+        self.img_trg_h = self._viz.img_trg
 
         # ---- language-only encoder + masking (:135-139) ----
-        ids_bl = self.input_ids.reshape(B, Lj)
+        ids_j = self.input_ids.reshape(B, Lj)
         if self._mask_input:
             torch.cuda.current_stream().wait_stream(side)
             if mask_override is not None:
@@ -519,25 +631,23 @@ class MerlotModel(object):
                                        "masked_idx": mask_override["masked_idx"].to(dev).to(torch.int32).contiguous()}
             else:
                 self.lang_mask_info = self.mask_inputs(mask_draws)
-            ids_to_use = self.lang_mask_info["masked_ids"].reshape(B, Lj)
-        else:
-            ids_to_use = ids_bl
-        self._ids_j = ids_to_use.contiguous()
+            ids_j = self.lang_mask_info["masked_ids"].reshape(B, Lj)
         self._mlm = self._ctr = self._tmp = None  # what mask_loss / contrastive_loss / temporal_loss keep for backward()
         if self.features_only:
             return
 
         # ---- joint encoder (:143-184) ----
-        self._emb_j_ln = self._embed_words_into(self._ids_j, "position_embeddings", "emb_j", _SITE_EMB_J, joint_in, remap=(Lj, Sj, Pz))
+        self._emb_j = _Embedding(st, bf, cfg, "emb_j", "position_embeddings", ids_j, joint_in, (Lj, Sj, Pz),
+                                 (p_hid, self._seed, _SITE_EMB_J))
         valid_j = bf.get("joint.valid", (B * Sj,), torch.uint8)
         if ni > 1 or img_mask is not None:  # :106-122: image i of row b valid iff img_mask[b // nt, i], over its P tokens
             mask_u8 = None
             if img_mask is not None:
                 mask_u8 = bf.get("joint.img_mask", (B // nt, ni), torch.uint8)
                 mask_u8.copy_(img_mask.reshape(B // nt, ni) != 0)
-            ops.joint_valid_img(self._ids_j, mask_u8, valid_j, B, nt, ni, self.P, Lj)
+            ops.joint_valid_img(ids_j, mask_u8, valid_j, B, nt, ni, self.P, Lj)
         else:
-            ops.joint_valid(self._ids_j, valid_j, B, Pz, Lj)
+            ops.joint_valid(ids_j, valid_j, B, Pz, Lj)
         c_viz = c_lang = None
         if self._log_attention_probs:  # split column sums of the joint attention maps for attention_log (:186-203)
             c_viz = bf.get("joint.c_viz", (B * Sj,), torch.float32, zero=True)
@@ -546,7 +656,7 @@ class MerlotModel(object):
         if self._export_probs:
             probs_j = bf.get("joint.probs", (cfg["num_hidden_layers"], B, Sj, Sj), torch.float32)
         self._joint = _Stack(st, bf, "joint", "encoder", cfg["num_hidden_layers"], B, Sj, valid_j, joint_in, cfg,
-                             p_hid if train else 0.0, self._seed, _SITE_JOINT, self._save, colsum=c_viz, colsum2=c_lang,
+                             p_hid, self._seed, _SITE_JOINT, self._save, colsum=c_viz, colsum2=c_lang,
                              colsum_split=Pz, colsum_valid_q=1, probs=probs_j,
                              # :160-168: language chunks attend to the vision tokens and to themselves only
                              pair=(Pz, self.lang_chunk_length) if cfg.get("disable_pairwise_lang_attn", False) else (0, 0))
@@ -573,68 +683,14 @@ class MerlotModel(object):
         return st._side
 
     # ---------------------------------------------------------------------------------------------------------
-    def _embed_words_into(self, ids_2d, norm_scope_name, tag, site, out, remap):
-        """embed_words (:262-297): E[ids] + Pos[0:L] -> LN embed_norm -> dropout -> bf16, written into `out` rows.  Returns the
-        embed_norm, for _embed_bwd."""
-        st, bf, cfg = self.store, self._bufs, self.config
-        H = self.hidden_size
-        R, Lseq = ids_2d.numel(), ids_2d.shape[1]
-        if Lseq > cfg["max_position_embeddings"]:  # tf.assert_less_equal, utils/model_utils.py:282
-            raise ValueError(f"sequence length {Lseq} exceeds max_position_embeddings {cfg['max_position_embeddings']}")
-        xsum = bf.get(f"{tag}.xsum", (R, H), torch.float32)
-        ops.embed_fwd(ids_2d, st.P("word_embeddings/word_embeddings"), st.P(f"{norm_scope_name}/position_embeddings"), xsum, Lseq)
-        p = float(self.dropout_prob or 0.0) if self.is_training else 0.0
-        ln = _LayerNorm(st, f"{norm_scope_name}/LayerNorm_embed_norm", xsum, bf.get(f"{tag}.mean", (R,), torch.float32),
-                        bf.get(f"{tag}.rstd", (R,), torch.float32), rows=R, remap=remap, dropout=(p, self._seed, site))
-        ln.forward(out)
-        return ln
-
     def embed_words(self, input_ids_2d, norm_scope_name="position_embeddings", reuse=None):
         """Public mirror of :262-297; returns bf16 [B, L, H]."""
         get_shape_list_rank(input_ids_2d, 2, "input_ids_2d")
         ids = input_ids_2d.to(torch.int32).contiguous()
         out = torch.empty((ids.numel(), self.hidden_size), dtype=torch.bfloat16, device=ids.device)
-        self._embed_words_into(ids, norm_scope_name, f"emb_pub.{norm_scope_name}", _SITE_EMB_J, out, (0, 0, 0))
+        _Embedding(self.store, self._bufs, self.config, f"emb_pub.{norm_scope_name}", norm_scope_name, ids, out, (0, 0, 0),
+                   (float(self.dropout_prob or 0.0), self._seed, _SITE_EMB_J))
         return out.view(ids.shape[0], ids.shape[1], -1)
-
-    def _langonly_reps(self):
-        """langonly_reps (:339-379)."""
-        cfg, st, bf = self.config, self.store, self._bufs
-        H = self.hidden_size
-        if "langonly_num_chunks_in_group" in cfg:
-            g = cfg["langonly_num_chunks_in_group"]
-            ng = self.num_chunks // g
-            assert ng > 0
-            assert self.num_chunks % g == 0
-            ids = self.input_ids.reshape(self.batch_size * ng, self.lang_chunk_length * g)
-        else:
-            ids = self.input_ids.reshape(self.batch_size, self.lang_chunk_length * self.num_chunks)
-        ids = ids.contiguous()
-        Blo, Llo = ids.shape
-        self._ids_lo = ids
-        h0 = bf.get("lo.h0", (Blo * Llo, H), torch.bfloat16)
-        self._emb_lo_ln = self._embed_words_into(ids, "langonly_embeddings", "emb_lo", _SITE_EMB_LO, h0, (0, 0, 0))
-        valid = bf.get("lo.valid", (Blo * Llo,), torch.uint8)
-        ops.ids_valid(ids, valid)
-        summ = bf.get("lo.attn_summ", (Blo * Llo,), torch.float32, zero=True)
-        p = float(self.dropout_prob or 0.0) if self.is_training else 0.0
-        probs_lo = None
-        if self._export_probs:
-            probs_lo = bf.get("lo.probs", (cfg["num_lang_transformer_hidden_layers"], Blo, Llo, Llo), torch.float32)
-        self._lo = _Stack(st, bf, "lo", "encoder", cfg["num_lang_transformer_hidden_layers"], Blo, Llo, valid, h0, cfg, p,
-                          self._seed, _SITE_LANGONLY, self._save_arenas, colsum=summ, probs=probs_lo)
-        y = self._lo.forward()
-        nch = self.batch_size * self.num_chunks
-        pool_idx = bf.get("lo.pool_idx", (nch,), torch.int32)
-        pool_idx.copy_(torch.arange(nch, dtype=torch.int32, device=st.device) * self.lang_chunk_length)
-        self._pool_idx_lo = pool_idx
-        self.lang_trg_h = bf.get("lo.lang_trg", (nch, H), torch.float32)
-        ops.gather_rows(y, pool_idx, self.lang_trg_h)
-        # attention_summs of mask_inputs (:428-431): sum over (layers, queries) of head-mean probabilities, as [B, L]
-        self.lang_transformer_info = {"hidden_state": y.view(Blo, Llo, H), "attention_summs": summ.view(self.B, self.L)}
-        if probs_lo is not None:
-            self.lang_transformer_info["self_attn_probs"] = probs_lo.permute(1, 0, 2, 3)
-        return self.lang_trg_h, self.lang_transformer_info
 
     def langonly_reps(self):
         return self.lang_trg_h, self.lang_transformer_info
@@ -899,16 +955,13 @@ class MerlotModel(object):
                 raise ValueError("d_contrastive_features replaces this model's contrastive_loss(): do not call both")
             if not self._mask_input:
                 raise ValueError("d_contrastive_features needs mask_input=True (the language features)")
-        cfg, st, bf, D = self.config, self.store, self._bufs, self._dims
-        H, B, N = self.hidden_size, self.B, D["N"]
-        Sj, Pz, vcl, Sv, Mv, np_, ncls = D["Sj"], D["Pz"], D["vcl"], D["Sv"], D["Mv"], D["np"], D["ncls"]
-        vt = "vision_backbone/vision_transformer"
+        bf, H, B, Sj = self._bufs, self.hidden_size, self.B, self._dims["Sj"]
         d_yj = bf.get("bwd.d_yj", (B * Sj, H), torch.bfloat16, zero=True)
         if d_hidden_state is not None:  # gradient of an external head (e.g. downstream/vcr's classifier) w.r.t. encoder_info['hidden_state']
             if tuple(d_hidden_state.shape) not in ((B * Sj, H), (B, Sj, H)) or d_hidden_state.dtype != torch.bfloat16:
                 raise ValueError("d_hidden_state must be bf16 [B, P+L, H]")
             d_yj.copy_(d_hidden_state.reshape(B * Sj, H))
-        d_img_trg = bf.get("bwd.d_img_trg", (N, H), torch.float32, zero=True)
+        d_img_trg = bf.get("bwd.d_img_trg", self.img_trg_h.shape, torch.float32, zero=True)
         d_lang_trg = None
         if self._mask_input:
             d_lang_trg = bf.get("bwd.d_lang_trg", (self.batch_size * self.num_chunks, H), torch.float32, zero=True)
@@ -938,72 +991,19 @@ class MerlotModel(object):
         side.wait_stream(main)
         with torch.cuda.stream(side):
             if self._mask_input:
-                Blo, Llo = self._ids_lo.shape
-                d_ylo = bf.get("bwd.d_ylo", (Blo * Llo, H), torch.bfloat16, zero=True)
-                ops.scatter_add_rows(d_lang_trg, self._pool_idx_lo, d_ylo)
-                d_h0lo = bf.get("bwd.d_h0lo", (Blo * Llo, H), torch.bfloat16)
-                self._lo.backward(d_ylo, d_h0lo)
-                self._embed_bwd("emb_lo", "langonly_embeddings", self._emb_lo_ln, self._ids_lo, d_h0lo)
-        # ---- joint encoder ----
+                self._lo.backward(d_lang_trg)
         d_jin = bf.get("bwd.d_jin", (B * Sj, H), torch.bfloat16)
         self._joint.backward(d_yj, d_jin)
-        # lang piece: embed_norm(position_embeddings) -> word / position tables
-        self._embed_bwd("emb_j", "position_embeddings", self._emb_j_ln, self._ids_j, d_jin)
-        # viz piece: final_ln -> K7 backward
-        nt = self.num_texts
-        Bi = B // nt
-        dxz = None
-        for j in range(nt):  # the nt texts of an image group all send gradient into the same viz tokens: summed through `dres`
-            dxj = bf.get(f"bwd.dxsum_z.{j & 1}", (Bi * Pz, H), torch.float32)
-            dxz = self._viz_ln.backward(d_jin, dxj, dres=dxz, remap=(Pz, nt * Sj, j * Sj))
-        d_hv = bf.get("bwd.d_hv", (Mv, H), torch.bfloat16)
-        ops.viz_assemble_bwd(dxz, d_img_trg, d_hv, N, D["h1"], D["w1"], ncls, D["sp"], H)
-        ops.segment_rowsum_scatter(dxz, N, vcl, self._img_idx, st.G("vision_backbone/img_idx_pe"), H)
-        ops.group_rowsum(dxz, N, vcl, 0, 1, None, st.G("vision_backbone/final_pe/cls_emb"), H)
-        ops.group_rowsum(dxz, N, vcl, 1, D["h2"] * D["w2"], self._grid_idxmap(D["h2"], D["w2"]),
-                         st.G("vision_backbone/final_pe/pos_embs"), H)
+        self._emb_j.backward(d_jin)
+        d_hv = self._viz.backward(d_jin, d_img_trg)
         # join the language-only backward (side stream); every gradient outside the ViT is final now
         main.wait_stream(side)
         if on_non_vit_grads_ready is not None:
             on_non_vit_grads_ready()
         # ---- ViT ----
-        d_h0v = bf.get("bwd.d_h0v", (Mv, H), torch.bfloat16)
+        d_h0v = bf.get("bwd.d_h0v", self._vit_in.out.shape, torch.bfloat16)
         self._vit.backward(d_hv, d_h0v, vit_layer_groups, on_vit_group_done)
-        dxv = self._vit_ln.backward(d_h0v, bf.get("bwd.dxsum_v", (Mv, H), torch.float32))
-        ops.group_rowsum(dxv, N, Sv, 0, ncls, None, st.G(f"{vt}/pos_embs/cls_emb"), H)
-        ops.group_rowsum(dxv, N, Sv, ncls, np_, self._grid_idxmap(D["h1"], D["w1"]), st.G(f"{vt}/pos_embs/pos_embs"), H)
-        dpatch = bf.get("bwd.dpatch", (N * np_, H), torch.bfloat16)
-        ops.vit_assemble_bwd(dxv, dpatch, N, np_, ncls, H)
-        if not self._resnet_layers:
-            ops.bias_grad(dpatch, st.G(f"{vt}/conv2d/bias"), rows=N * np_, N=H)
-            ops.gemm(self._patch_A, dpatch, a_mn_major=True, b_mn_major=True, out=st.G(f"{vt}/conv2d/kernel"), atomic=True,
-                     M=D["Kp"], N=H, K=N * np_)
-        else:  # conv_postresnet_proj (1x1 + bias, not standardised), then the stem's tape
-            Cr = self._rc.shape[1]
-            ops.bias_grad(dpatch, st.G(f"{vt}/conv_postresnet_proj/bias"), rows=N * np_, N=H)
-            ops.gemm(self._rc, dpatch, a_mn_major=True, b_mn_major=True, out=st.G(f"{vt}/conv_postresnet_proj/kernel"), atomic=True,
-                     M=Cr, N=H, K=N * np_)
-            self.d_rc = bf.get("bwd.d_rc", (N * np_, Cr), torch.bfloat16)
-            ops.gemm(dpatch, st.W(f"{vt}/conv_postresnet_proj/kernel"), out=self.d_rc)  # [M, H] . [Cr, H]^T
-            self._stem.backward(self.d_rc)
-
-    def _embed_bwd(self, tag, norm_scope_name, ln, ids_2d, dy):
-        """Backward of _embed_words_into, whose embed_norm is `ln`."""
-        st, bf = self.store, self._bufs
-        (groups, Lseq), H = ids_2d.shape, self.hidden_size
-        dx = ln.backward(dy, bf.get(f"bwd.dxsum.{tag}", (ids_2d.numel(), H), torch.float32),
-                         dropout=ln.kw["dropout"] if self.is_training else (0.0, 0, 0))
-        ops.scatter_add_rows(dx, ids_2d.reshape(-1), st.G("word_embeddings/word_embeddings"))
-        ops.group_rowsum(dx, groups, Lseq, 0, Lseq, None, st.G(f"{norm_scope_name}/position_embeddings"), H)
-
-    def _grid_idxmap(self, nh, nw):
-        key = ("_grid", nh, nw)
-        d = self._bufs.d
-        if key not in d:
-            i = torch.arange(nh, device=self.store.device)[:, None]
-            j = torch.arange(nw, device=self.store.device)[None]
-            d[key] = (i * 64 + j).reshape(-1).to(torch.int32)
-        return d[key]
+        self.d_rc = self._vit_in.backward(d_h0v)
 
 
 def _pad8(k: int) -> int:
