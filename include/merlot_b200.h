@@ -142,9 +142,14 @@ int merlot_attention_bwd(const merlot_attn_t* a, void* stream);
 int merlot_attention_bwd_dq_parts(int S);                          /* slices used by bwd for this S; 0 = atomic single slice */
 size_t merlot_attention_bwd_workspace_bytes(int B, int S, int heads); /* bytes of dq_accum (ld_dq = heads*64) */
 int merlot_attention_colsum(const merlot_attn_t* a, void* stream);
-/* Export path (PREDICT): probs_bss f32 [B,S,S] <- head-mean probabilities of this layer = one layer of `self_attn_probs`
- * (utils/transformer.py:208-209,238 with compress_attn=True), recomputed from qkv + lse. */
-int merlot_attention_probs(const merlot_attn_t* a, float* probs_bss, void* stream);
+/* Export path (PREDICT): probs_bss f32 [B,S,S] <- beta * probs_bss + alpha * (head-mean probabilities of this layer), the
+ * head mean being one layer of `self_attn_probs` (utils/transformer.py:208-209,238 with compress_attn=True), recomputed from
+ * qkv + lse in one kernel.  alpha = 1, beta = 0 writes the layer's map; beta = 0 never reads probs_bss.  alpha = 1/layers
+ * with beta = 0 for layer 0 and beta = 1 after it leaves the layer mean (model_fn PREDICT, model/modeling.py:762-765). */
+int merlot_attention_probs(const merlot_attn_t* a, float* probs_bss, float alpha, float beta, void* stream);
+/* attention_log (model/modeling.py:186-203) from a layer-mean map probs_bss f32 [B,S,S] (valid: uint8 [B*S], the first P
+ * positions the vision piece): out4 as merlot_attention_log_blocks, in a fixed summation order (no atomics). */
+int merlot_attention_log_probs(const float* probs_bss, const void* valid, int B, int S, int P, float* out4, void* stream);
 /* attention_log (model/modeling.py:186-203): out4 = {lang2lang, lang2viz, viz2lang, viz2viz} normalised block sums of the
  * layer/head/batch-mean attention map, from the two split column sums (queries in the viz piece / in the lang piece). */
 int merlot_attention_log_blocks(const float* c_viz, const float* c_lang, const void* valid_u8, int B, int S, int P, float* out4,
@@ -262,6 +267,7 @@ typedef struct merlot_stack {
   float* attn_colsum;                          /* optional f32 [B,S]: += sum over layers,queries of head-mean probs */
   float* attn_colsum2; int attn_colsum_split; int attn_colsum_valid_q;  /* optional split by query piece (attention_log) */
   float* attn_probs;                           /* optional f32 [layers][B,S,S]: head-mean probabilities of every layer (export) */
+  int attn_probs_layer_mean;                   /* 1: attn_probs is ONE f32 [B,S,S] that receives their mean over layers */
   /* backward */
   const void* dy;                              /* bf16 [B*S, H] gradient wrt y */
   void* dh_in;                                 /* bf16 [B*S, H] gradient wrt h_in (optional) */

@@ -3,6 +3,8 @@
 // An export path, not a hot one: the probabilities are recomputed from the saved (q, k, log-sum-exp) with plain fp32 dot
 // products -- [B, S, S] fp32 per layer would be 60 MB per joint layer at configs[1], which is why the training path never
 // materialises them (K2/K3/K4 keep them on chip).
+#include <cmath>
+
 #include "host_common.h"
 #include "ptx.cuh"
 
@@ -22,11 +24,15 @@ __device__ __forceinline__ bool attn_keep_one(uint64_t seed, uint32_t site, uint
 
 // grid (ceil(S / EXQ), B); 256 threads, thread t walks keys t, t + 256, ...
 // DROP: the head mean of the dropped probabilities P o Z / (1 - p) (self_attn_probs is built from them, transformer.py:138)
+// out = beta * out + alpha * (head mean); beta == 0 never reads out.  alpha = 1, beta = 0 is the plain per-layer export
+// (alpha folds into the 1 / heads factor, exact for alpha = 1); alpha = 1 / layers with beta = 0 on the first layer and 1
+// on the others accumulates the layer mean in one [B, S, S] buffer.
 template <bool DROP>
 __global__ void __launch_bounds__(256) attn_probs_export_kernel(const bf16* __restrict__ qkv, int ld_qkv, const uint8_t* __restrict__ valid,
                                                                 const float* __restrict__ lse, float* __restrict__ out, int B, int S,
                                                                 int heads, float scale, int pair_P, int pair_chunk, uint32_t drop_thresh16,
-                                                                float drop_scale, uint64_t drop_seed, uint32_t drop_site) {
+                                                                float drop_scale, uint64_t drop_seed, uint32_t drop_site, float alpha,
+                                                                float beta) {
   extern __shared__ float sm[];
   const int H = heads * 64;
   float* sq = sm;                 // [EXQ][H]   queries of this CTA (fp32), pre-scaled
@@ -50,7 +56,7 @@ __global__ void __launch_bounds__(256) attn_probs_export_kernel(const bf16* __re
   int sq_seg[EXQ];
 #pragma unroll
   for (int r = 0; r < EXQ; ++r) sq_seg[r] = seg_of(q0 + r);
-  const float inv_heads = (DROP ? drop_scale : 1.0f) / (float)heads;
+  const float inv_heads = (DROP ? drop_scale : 1.0f) / (float)heads * alpha;
   for (int k = threadIdx.x; k < S; k += 256) {
     const bool vk = valid == nullptr || valid[tok0 + k] != 0;
     const int k_seg = seg_of(k);
@@ -86,7 +92,41 @@ __global__ void __launch_bounds__(256) attn_probs_export_kernel(const bf16* __re
     }
 #pragma unroll
     for (int r = 0; r < EXQ; ++r)
-      if (q0 + r < S) out[((size_t)b * S + q0 + r) * S + k] = acc[r] * inv_heads;
+      if (q0 + r < S) {
+        float* o = out + ((size_t)b * S + q0 + r) * S + k;
+        *o = beta == 0.f ? acc[r] * inv_heads : fmaf(beta, *o, acc[r] * inv_heads);
+      }
+  }
+}
+
+// attention_log (model/modeling.py:186-203) of a layer-mean map: the four block sums of probs masked by valid[q] * valid[k],
+// over the total.  One CTA of 1024 threads: warp w takes rows w, w + 32, ..., lane j keys j, j + 32, ...; a fixed tree adds
+// the partial sums, so a given map always gives the same four values (the column-sum route, K4, adds with float atomics).
+__global__ void __launch_bounds__(1024) attn_log_probs_kernel(const float* __restrict__ probs, const uint8_t* __restrict__ valid,
+                                                              int B, int S, int P, float* __restrict__ out) {
+  __shared__ float red[4][1024];
+  float a[4] = {0.f, 0.f, 0.f, 0.f};  // [q viz k viz, q viz k lang, q lang k viz, q lang k lang]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (long long row = warp; row < (long long)B * S; row += 32) {
+    if (!valid[row]) continue;
+    const int b = (int)(row / S), q_lang = (int)(row % S) >= P;
+    const float* pr = probs + row * S;
+    for (int k = lane; k < S; k += 32)
+      if (valid[(size_t)b * S + k]) a[2 * q_lang + (k >= P)] += pr[k];
+  }
+  for (int j = 0; j < 4; ++j) red[j][threadIdx.x] = a[j];
+  __syncthreads();
+  for (int o = 512; o > 0; o >>= 1) {
+    if (threadIdx.x < o)
+      for (int j = 0; j < 4; ++j) red[j][threadIdx.x] += red[j][threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const float tot = red[0][0] + red[1][0] + red[2][0] + red[3][0];
+    out[0] = red[3][0] / tot;  // lang2lang : keys lang, queries lang
+    out[1] = red[1][0] / tot;  // lang2viz  : keys lang, queries viz
+    out[2] = red[2][0] / tot;  // viz2lang  : keys viz,  queries lang
+    out[3] = red[0][0] / tot;  // viz2viz
   }
 }
 
@@ -94,7 +134,17 @@ __global__ void __launch_bounds__(256) attn_probs_export_kernel(const bf16* __re
 
 using namespace mb;
 
-extern "C" int merlot_attention_probs(const merlot_attn_t* a, float* probs_bss, void* stream_) {
+extern "C" int merlot_attention_log_probs(const float* probs_bss, const void* valid, int B, int S, int P, float* out4,
+                                          void* stream_) {
+  MB_REQUIRE(probs_bss && valid && out4, MERLOT_EINVAL, "attention_log_probs: null pointer");
+  MB_REQUIRE(B > 0 && S > 0 && P >= 0 && P <= S, MERLOT_ESHAPE, "attention_log_probs: bad dims B=%d S=%d P=%d", B, S, P);
+  attn_log_probs_kernel<<<1, 1024, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      probs_bss, reinterpret_cast<const uint8_t*>(valid), B, S, P, out4);
+  MB_CHECK_LAUNCH();
+  return MERLOT_OK;
+}
+
+extern "C" int merlot_attention_probs(const merlot_attn_t* a, float* probs_bss, float alpha, float beta, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   MB_REQUIRE(a && probs_bss && a->qkv && a->lse, MERLOT_EINVAL, "attention_probs: qkv, lse and the output are required");
   MB_REQUIRE(a->head_dim == 64 && a->B > 0 && a->S > 0 && a->heads > 0 && (a->ld_qkv % 8) == 0, MERLOT_ESHAPE,
@@ -103,6 +153,7 @@ extern "C" int merlot_attention_probs(const merlot_attn_t* a, float* probs_bss, 
              "attention_probs: pair_chunk_len > 0 (disable_pairwise_lang_attn) needs the token-validity mask");
   MB_REQUIRE(a->dropout_p >= 0.f && a->dropout_p < 1.f, MERLOT_EINVAL, "attention_probs: dropout_p must lie in [0, 1) (got %g)",
              (double)a->dropout_p);
+  MB_REQUIRE(std::isfinite(alpha) && std::isfinite(beta), MERLOT_EINVAL, "attention_probs: alpha and beta must be finite");
   const int H = a->heads * 64;
   const size_t smem = (size_t)(EXQ * H + EXQ * a->heads) * sizeof(float);
   MB_REQUIRE(smem <= 200 * 1024, MERLOT_ESHAPE, "attention_probs: hidden size too large");
@@ -119,7 +170,7 @@ extern "C" int merlot_attention_probs(const merlot_attn_t* a, float* probs_bss, 
   auto kern = a->dropout_p > 0.f ? attn_probs_export_kernel<true> : attn_probs_export_kernel<false>;
   kern<<<grid, 256, smem, stream>>>(reinterpret_cast<const bf16*>(a->qkv), a->ld_qkv, reinterpret_cast<const uint8_t*>(a->valid), a->lse,
                                     probs_bss, a->B, a->S, a->heads, a->scale, a->pair_viz_len, a->pair_chunk_len, th, ds,
-                                    a->dropout_seed, a->dropout_site);
+                                    a->dropout_seed, a->dropout_site, alpha, beta);
   MB_CHECK_LAUNCH();
   return MERLOT_OK;
 }

@@ -205,7 +205,10 @@ extern "C" int merlot_stack_forward(const merlot_stack_t* s, void* stream_) {
         a.colsum2 = s->attn_colsum2; a.colsum_split = s->attn_colsum_split; a.colsum_valid_q = s->attn_colsum_valid_q;
         RC(merlot_attention_colsum(&a, st));
       }
-      if (s->attn_probs) RC(merlot_attention_probs(&a, s->attn_probs + (size_t)l * s->B * s->S * s->S, st));
+      if (s->attn_probs && s->attn_probs_layer_mean)  // the layer mean, accumulated in place: (1/layers) * sum_l P_l
+        RC(merlot_attention_probs(&a, s->attn_probs, 1.0f / (float)s->layers, l == 0 ? 0.f : 1.f, st));
+      else if (s->attn_probs)
+        RC(merlot_attention_probs(&a, s->attn_probs + (size_t)l * s->B * s->S * s->S, 1.f, 0.f, st));
     }
     {
       merlot_gemm_t e = gemm_base(0, 0, 0);

@@ -207,7 +207,9 @@ class _Stack:
     """One transformer stack invocation (utils/transformer.py:171-247) through merlot_stack_forward/backward."""
 
     def __init__(self, store, bufs, tag, scope, layers, B, S, valid, h_in, cfg, dropout_p, seed, site, save, colsum=None,
-                 colsum2=None, colsum_split=0, colsum_valid_q=0, probs=None, pair=(0, 0)):
+                 colsum2=None, colsum_split=0, colsum_valid_q=0, probs=None, pair=(0, 0), probs_layer_mean=False):
+        """probs: f32 [layers, B, S, S] of every layer's head-mean attention map, or with probs_layer_mean one [B, S, S]
+        that receives their mean over layers."""
         H, I, heads = cfg["hidden_size"], cfg["intermediate_size"], cfg["num_attention_heads"]
         if H % heads != 0 or H // heads != 64:
             raise ValueError("passed in a tensor of shape {} when size_per_head={} and num_attention_heads={}".format(
@@ -233,6 +235,7 @@ class _Stack:
         d.attn_colsum2 = colsum2.data_ptr() if colsum2 is not None else None
         d.attn_colsum_split, d.attn_colsum_valid_q = int(colsum_split), int(colsum_valid_q)
         d.attn_probs = probs.data_ptr() if probs is not None else None
+        d.attn_probs_layer_mean = int(probs_layer_mean)
         d.pair_viz_len, d.pair_chunk_len = int(pair[0]), int(pair[1])  # disable_pairwise_lang_attn (model/modeling.py:160-168)
         self.d, self.bufs, self.tag, self.keep = d, bufs, tag, (valid, h_in, colsum, probs)
 
@@ -449,7 +452,7 @@ class MerlotModel(object):
     def __init__(self, config, is_training, use_tpu, image, input_ids, mask_input=False, shuffled_idx_img=None,
                  img_mask=None, log_attention_probs=True, *, params: ParamStore, mask_draws: Optional[Dict] = None,
                  mask_override: Optional[Dict] = None, dropout_seed: int = 0, save_for_backward: Optional[bool] = None,
-                 dist=None, export_attention_probs: bool = False, frame_copies: int = 1, features_only: bool = False):
+                 dist=None, export_attention_probs=False, frame_copies: int = 1, features_only: bool = False):
         """Arguments as model/modeling.py:48-66.  `use_tpu` is accepted and ignored (it only selects one-hot vs gather
         embedding lookups in the reference, utils/model_utils.py:259-263 -- same values either way).
 
@@ -461,6 +464,14 @@ class MerlotModel(object):
         `num_imgs` = ni > 1 in the config and `img_mask` (model/modeling.py:106-122) put several images before every text:
         `image` holds (batch_size // num_texts) * ni images, the joint sequence P * ni viz tokens then L language tokens, and
         an image masked in `img_mask` [B // num_texts, ni] drops out of the joint attention (check_num_imgs has the rules).
+
+        `export_attention_probs` materialises the head-mean attention maps model_fn's PREDICT mode returns
+        (model/modeling.py:762-770): True puts every layer's into encoder_info and lang_transformer_info['self_attn_probs'],
+        [B, layers, S, S] each; "layer_mean" puts the joint encoder's mean over layers, [B, S, S], into encoder_info (the
+        reduce_mean of :765, accumulated layer by layer in one buffer, so no per-layer buffer of the joint encoder exists)
+        and keeps the language-only encoder's maps per layer, as the reference returns them.  With "layer_mean",
+        attention_log is the reference's block sums of that map (:186-203) in a fixed summation order, so two runs on the
+        same input give the same bits; otherwise it comes from K4's column sums, which add with float atomics.
 
         `features_only` runs what contrastive_features() needs and nothing more: the ViT, the language-only encoder and
         mask_inputs (with the dropout of is_training), but not the joint encoder, and it allows no backward.  The
@@ -524,7 +535,10 @@ class MerlotModel(object):
         self._log_attention_probs = log_attention_probs
         # PREDICT-mode outputs of model_fn (model/modeling.py:762-770): encoder_info / lang_transformer_info['self_attn_probs']
         # = head-mean probabilities [B, layers, S, S].  Materialised only on request (60 MB per joint layer at configs[1]).
-        self._export_probs = bool(export_attention_probs)
+        if export_attention_probs not in (False, True, "layer_mean"):
+            raise ValueError(f"export_attention_probs must be False, True or 'layer_mean', got {export_attention_probs!r}")
+        self._export_probs = export_attention_probs is True or export_attention_probs == "layer_mean"
+        self._probs_layer_mean = export_attention_probs == "layer_mean"
         self._forward(image, shuffled_idx_img, img_mask, mask_draws, mask_override)
 
     # ---- shapes (:226-260) ----
@@ -649,26 +663,34 @@ class MerlotModel(object):
         else:
             ops.joint_valid(ids_j, valid_j, B, Pz, Lj)
         c_viz = c_lang = None
-        if self._log_attention_probs:  # split column sums of the joint attention maps for attention_log (:186-203)
+        # with the layer-mean map at hand attention_log is taken from it (a fixed summation order), not from K4's column sums
+        log_from_colsum = self._log_attention_probs and not self._probs_layer_mean
+        if log_from_colsum:  # split column sums of the joint attention maps for attention_log (:186-203)
             c_viz = bf.get("joint.c_viz", (B * Sj,), torch.float32, zero=True)
             c_lang = bf.get("joint.c_lang", (B * Sj,), torch.float32, zero=True)
         probs_j = None
-        if self._export_probs:
+        if self._probs_layer_mean:
+            probs_j = bf.get("joint.probs_mean", (B, Sj, Sj), torch.float32)
+        elif self._export_probs:
             probs_j = bf.get("joint.probs", (cfg["num_hidden_layers"], B, Sj, Sj), torch.float32)
         self._joint = _Stack(st, bf, "joint", "encoder", cfg["num_hidden_layers"], B, Sj, valid_j, joint_in, cfg,
                              p_hid, self._seed, _SITE_JOINT, self._save, colsum=c_viz, colsum2=c_lang,
-                             colsum_split=Pz, colsum_valid_q=1, probs=probs_j,
+                             colsum_split=Pz, colsum_valid_q=1, probs=probs_j, probs_layer_mean=self._probs_layer_mean,
                              # :160-168: language chunks attend to the vision tokens and to themselves only
                              pair=(Pz, self.lang_chunk_length) if cfg.get("disable_pairwise_lang_attn", False) else (0, 0))
         self._y_j = self._joint.forward()
         self._attn_log = None
-        if self._log_attention_probs:
+        if log_from_colsum:
             out4 = bf.get("joint.attn_log", (4,), torch.float32)
             L.lib().merlot_attention_log_blocks(c_viz.data_ptr(), c_lang.data_ptr(), valid_j.data_ptr(), B, Sj, Pz,
                                                 out4.data_ptr(), ops._stream())
             self._attn_log = out4
+        elif self._log_attention_probs:
+            self._attn_log = ops.attention_log_probs(probs_j, valid_j, Pz, bf.get("joint.attn_log", (4,), torch.float32))
         self.encoder_info = {"hidden_state": self._y_j.view(B, Sj, H)}
-        if probs_j is not None:  # [layers,B,S,S] -> the reference's [B, layers, S, S] (utils/transformer.py:238), a view
+        if self._probs_layer_mean:  # already the mean over layers, [B, S, S]
+            self.encoder_info["self_attn_probs"] = probs_j
+        elif probs_j is not None:  # [layers,B,S,S] -> the reference's [B, layers, S, S] (utils/transformer.py:238), a view
             self.encoder_info["self_attn_probs"] = probs_j.permute(1, 0, 2, 3)
         self._hidden_f32 = {}
         self.encoder_pieces = [{"name": "viz", "start": 0, "end": Pz}, {"name": "lang", "start": Pz, "end": Sj}]

@@ -166,14 +166,31 @@ def attention_bwd(qkv, ctx, d_ctx, lse, B, S, heads, valid=None, dqkv=None, dq_a
     return dqkv
 
 
-def attention_probs(qkv, lse, B, S, heads, valid=None, out=None, pair=(0, 0), dropout=(0.0, 0, 0)):
-    """Export path: head-mean probabilities [B,S,S] fp32 of one layer (one layer of `self_attn_probs`), after the
-    forward's dropout=(p, seed, site)."""
+def attention_probs(qkv, lse, B, S, heads, valid=None, out=None, pair=(0, 0), dropout=(0.0, 0, 0), alpha=1.0, beta=0.0):
+    """Export path: out = beta * out + alpha * (head-mean probabilities [B,S,S] fp32 of one layer, one layer of
+    `self_attn_probs`), after the forward's dropout=(p, seed, site).  The defaults write the layer's map; beta = 0 never
+    reads `out`."""
     a = _attn_desc(qkv, B, S, heads, valid, pair, dropout)
     if out is None:
+        assert beta == 0.0, "beta != 0 accumulates into an existing `out`"
         out = torch.empty((B, S, S), dtype=torch.float32, device=qkv.device)
+    _require_cuda(out)
+    assert out.dtype == torch.float32 and out.numel() == B * S * S and out.is_contiguous()
     a.lse = lse.data_ptr()
-    L.lib().merlot_attention_probs(C.byref(a), out.data_ptr(), _stream())
+    L.lib().merlot_attention_probs(C.byref(a), out.data_ptr(), float(alpha), float(beta), _stream())
+    return out
+
+
+def attention_log_probs(probs, valid, P, out=None):
+    """attention_log (model/modeling.py:186-203) of a layer-mean map probs [B,S,S] fp32 with token validity uint8 [B*S]
+    and P vision positions: out[4] = {lang2lang, lang2viz, viz2lang, viz2viz} block sums over the total, in a fixed order."""
+    _require_cuda(probs, valid, out)
+    B, S, _ = probs.shape
+    assert probs.dtype == torch.float32 and probs.is_contiguous() and probs.shape == (B, S, S)
+    assert valid.dtype == torch.uint8 and valid.numel() == B * S and valid.is_contiguous()
+    if out is None:
+        out = torch.empty(4, dtype=torch.float32, device=probs.device)
+    L.lib().merlot_attention_log_probs(probs.data_ptr(), valid.data_ptr(), B, S, int(P), out.data_ptr(), _stream())
     return out
 
 

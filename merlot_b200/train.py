@@ -230,6 +230,8 @@ def model_fn_builder(config: NeatConfig, *, store: Optional[ParamStore] = None, 
     span lengths, 10/80/10 options, replacement ids): replica r at step t uses seed + t*world + r, so replicas draw
     independently like the reference's per-core tf.random ops and two runs with different seeds differ.
     `log_attention_probs` defaults to the reference's model_fn (modeling.py:691-709 computes attn/* every step).
+    Modes: "train" (the default), "eval" (eval_step) and "predict" (predict_step), the last two with params
+    {"eval_batch": k} and, for "predict", the reference's params["batch_size"].
 
     Gradient accumulation: model_fn([f_0, ..., f_{A-1}]) with A feature dicts of one micro-batch each is the step of the
     world * A virtual replicas v = rank * A + j, with seed + t*world*A + v (config.replica_seed).  The contrastive loss of
@@ -274,6 +276,10 @@ def model_fn_builder(config: NeatConfig, *, store: Optional[ParamStore] = None, 
     def model_fn(features, labels=None, mode="train", params=None):
         if mode == "eval":
             return eval_step(features, int((params or {}).get("eval_batch", 0)))
+        if mode == "predict":
+            params = params or {}
+            return predict_step(features, int(params.get("eval_batch", 0)),
+                                int(params.get("batch_size", features["input_ids"].shape[0])))
         if isinstance(features, (list, tuple)):
             return accumulated_step(list(features))
         model = build_model(features, seed + store.global_step * world + rank, transpose=mode == "train",
@@ -288,14 +294,14 @@ def model_fn_builder(config: NeatConfig, *, store: Optional[ParamStore] = None, 
 
         return StepSpec(model, (lang_loss, contr_loss, temp_loss), losses, train_op)
 
-    def eval_step(features, k):
+    def eval_step(features, k, **kw):
         """EVAL mode (modeling.py:691-711, :788-798) on evaluation batch k: the training forward as the reference builds it
         (is_training=True, mask_input=True), keeping nothing for a backward, with no collective (one batch is one replica:
         its contrastive negatives are its own videos) and with the dropout and masking seed eval_seed(seed, k).  Returns a
         StepSpec whose metrics are the `losses` dict without learning_rate, whose `total_loss` is lang + contr + temporal
         (device scalars, which the next model on this store overwrites) and whose train_op is None."""
-        model = build_model(features, eval_seed(seed, k), transpose=False, replicas=None, save_for_backward=False,
-                            log_attention_probs=log_attention_probs)
+        kw.setdefault("log_attention_probs", log_attention_probs)
+        model = build_model(features, eval_seed(seed, k), transpose=False, replicas=None, save_for_backward=False, **kw)
         lang_loss, lang_losses = model.mask_loss()
         contr_loss, contr_losses = model.contrastive_loss()
         temp_loss, temp_losses = temporal_loss(model, features)
@@ -303,6 +309,30 @@ def model_fn_builder(config: NeatConfig, *, store: Optional[ParamStore] = None, 
                         metrics_of(model, lang_losses, contr_losses, temp_losses, learning_rate=False), None)
         spec.total_loss = lang_loss + contr_loss + temp_loss
         return spec
+
+    def predict_step(features, k, bsz):
+        """PREDICT mode (modeling.py:760-787) on evaluation batch k of bsz videos: eval_step's forward (same seed, dropout
+        and masks, no backward, no collective) with the joint encoder's attention maps exported as their layer mean.
+        Returns the reference's predictions dict on the host (predictions()): self_attn_probs [bsz, B // bsz, S, S], the
+        layer and head mean of the joint maps; lang_attn_probs, the language-only encoder's per-layer head means reshaped
+        to lead with bsz; masked_ids; every lang/ attn/ contr/ temporal/ loss tiled to [bsz]; and the batch's other
+        features.  attn/* are the block sums of the exported map (MerlotModel's "layer_mean" export).
+
+        `images` is left out on purpose, unlike the reference: it is the model's input, the evaluation pipeline reproduces
+        it from the same seed and batch index, and keeping it would roughly double the output."""
+        spec = eval_step(features, k, export_attention_probs="layer_mean")
+        m = spec.model
+        if m.batch_size != bsz:
+            raise ValueError(f"predict: params batch_size {bsz} is not the batch's {m.batch_size} videos")
+        out = {name: v for name, v in features.items() if name != "images"}
+        sap = m.encoder_info["self_attn_probs"]  # [B, S, S], already the mean over layers
+        out["self_attn_probs"] = sap.reshape(bsz, m.B // bsz, *sap.shape[1:])
+        lap = m.lang_transformer_info["self_attn_probs"]  # [B_lo, layers, L, L]
+        lead = [bsz] if lap.shape[0] == bsz else [bsz, lap.shape[0] // bsz]  # the reference reshapes to [bsz] + shape[1:]
+        out["lang_attn_probs"] = lap.reshape(lead + list(lap.shape[1:]))
+        out["masked_ids"] = m.lang_mask_info["masked_ids"]
+        out.update(spec.metrics)
+        return predictions(out, bsz)
 
     def accumulated_step(micro):
         A = len(micro)
@@ -354,6 +384,24 @@ def model_fn_builder(config: NeatConfig, *, store: Optional[ParamStore] = None, 
     model_fn.store = store
     model_fn.optimizer = optimizer
     return model_fn
+
+
+def predictions(features: Dict, bsz: int) -> Dict:
+    """The last step of the reference's PREDICT mode (modeling.py:774-784) on the host: every entry, by sorted name, as a
+    NumPy array -- a scalar tiled to [bsz], an array whose leading axis is not bsz reshaped to [bsz, -1] -- with
+    floating-point values as float32 and integers and booleans as int32."""
+    import numpy as np
+    out = {}
+    for name in sorted(features):
+        v = features[name]
+        v = v.detach().cpu() if torch.is_tensor(v) else torch.as_tensor(v)
+        v = v.float() if v.is_floating_point() else v.to(torch.int32)
+        if v.dim() == 0:
+            v = v[None].repeat(bsz)
+        elif v.shape[0] != bsz:
+            v = v.reshape(bsz, -1)
+        out[name] = np.ascontiguousarray(v.numpy())
+    return out
 
 
 def eval_seed(seed: int, k: int) -> int:
