@@ -369,21 +369,30 @@ class _VizTokens:
 
 class _LangOnly:
     """langonly_reps (:339-379) of model.input_ids with hidden dropout p, run at construction: the ids regrouped by
-    langonly_num_chunks_in_group, _Embedding, _Stack, and each chunk's first row gathered into fp32 `lang_trg`."""
+    langonly_num_chunks_in_group, _Embedding, _Stack, and each chunk's first row gathered into fp32 `lang_trg`.  The stack is
+    the joint encoder's `encoder/` variables with share_params (the default), its own `langonly_encoder/` without
+    (:356-362)."""
 
     def __init__(self, model, p):
         cfg, st, bf, Lc, nch = model.config, model.store, model._bufs, model.lang_chunk_length, model.num_chunks
+        layers = cfg["num_lang_transformer_hidden_layers"]
+        scope = "encoder" if cfg.get("share_params", True) else "langonly_encoder"
+        need = [f"{scope}/layer{l:02d}/qkv/kernel" for l in range(layers)] + [f"{scope}/LayerNorm_ln_final/gamma"]
+        if any(n not in st.entries for n in need):
+            raise ValueError(f"share_params: {cfg.get('share_params', True)} runs the language-only encoder on {scope}/ "
+                             f"({layers} layers), but the ParamStore has no such stack: build it from a config with the "
+                             f"same share_params and num_lang_transformer_hidden_layers")
         g = cfg.get("langonly_num_chunks_in_group", nch)
         assert nch // g > 0 and nch % g == 0
         ids = model.input_ids.reshape(-1, Lc * g).contiguous()
-        (Blo, Llo), H, layers = ids.shape, model.hidden_size, cfg["num_lang_transformer_hidden_layers"]
+        (Blo, Llo), H = ids.shape, model.hidden_size
         h0 = bf.get("lo.h0", (Blo * Llo, H), torch.bfloat16)
         self.emb = _Embedding(st, bf, cfg, "emb_lo", "langonly_embeddings", ids, h0, (0, 0, 0), (p, model._seed, _SITE_EMB_LO))
         valid = bf.get("lo.valid", (Blo * Llo,), torch.uint8)
         ops.ids_valid(ids, valid)
         summ = bf.get("lo.attn_summ", (Blo * Llo,), torch.float32, zero=True)
         probs = bf.get("lo.probs", (layers, Blo, Llo, Llo), torch.float32) if model._export_probs else None
-        self.stack = _Stack(st, bf, "lo", "encoder", layers, Blo, Llo, valid, h0, cfg, p, model._seed, _SITE_LANGONLY,
+        self.stack = _Stack(st, bf, "lo", scope, layers, Blo, Llo, valid, h0, cfg, p, model._seed, _SITE_LANGONLY,
                             model._save_arenas, colsum=summ, probs=probs)
         y = self.stack.forward()
         self.bf, nrows = bf, model.batch_size * nch
@@ -428,6 +437,9 @@ def check_num_imgs(cfg, batch_size, num_chunks, B, n_images, img_mask=None, mask
                                   "mask (model/modeling.py:162) for a P * num_imgs + L sequence")
     if frame_copies > 1:
         raise NotImplementedError("num_imgs > 1 / img_mask with frame_copies > 1 (the zero-shot story forward) is not provided")
+    if not cfg.get("share_params", True):
+        raise NotImplementedError("num_imgs > 1 / img_mask with share_params: False is not provided: the separate "
+                                  "language-only encoder is a pretraining path and does not extend the multi-image input")
     max_vpe = int(cfg.get("max_vision_pos_embeddings", 1024))
     if ni > max_vpe:
         raise ValueError(f"num_imgs {ni} exceeds max_vision_pos_embeddings {max_vpe} (model/modeling.py:305-311)")
@@ -503,8 +515,6 @@ class MerlotModel(object):
         if cfg.get("num_texts", 1) > 1 and (mask_input or shuffled_idx_img is not None):
             raise NotImplementedError("num_texts > 1 (VCR, model/modeling.py:111-119) is a finetuning/inference path: mask_input and "
                                       "shuffled_idx_img are not combined with it in the reference either (:319-320)")
-        if not cfg.get("share_params", True):
-            raise NotImplementedError("share_params: False (separate langonly_encoder, model/modeling.py:361) not provided yet")
 
         input_ids_shape = get_shape_list_rank(input_ids, [2, 3], "input_ids")
         if len(input_ids_shape) == 2:  # :72-77

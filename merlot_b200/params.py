@@ -12,7 +12,9 @@ Storage differs from the TF variables in three places (converted by load_tf_dict
   * the patch conv kernel [P,P,3,H] is stored as the im2col matrix [P*P*3, H] (same memory order).
 
 `task` selects the variable set of one reference graph: "pretrain" (model/modeling.py model_fn, every head) or "vcr"
-(downstream/vcr/modeling.py model_fn: MerlotModel(mask_input=False) + the answer / rationale classifier towers).
+(downstream/vcr/modeling.py model_fn: MerlotModel(mask_input=False) + the answer / rationale classifier towers).  In
+pretraining, `share_params: False` gives the language-only pass its own `langonly_encoder/` stack of
+num_lang_transformer_hidden_layers layers beside the joint `encoder/`; the VCR graph has no language-only pass and ignores it.
 
 save_checkpoint / restore_checkpoint write and read the whole training state (parameters, Adam slots, global_step) as the
 TensorFlow V2 checkpoints the reference's Estimator keeps in output_dir.
@@ -106,7 +108,11 @@ def _entries(cfg: dict, task: str = "pretrain") -> List[Entry]:
     for sc in ("position_embeddings", "langonly_embeddings"):
         add(f"{sc}/position_embeddings", (cfg["max_position_embeddings"], H))
         ln(f"{sc}/LayerNorm_embed_norm")
-    stack("encoder", max(cfg["num_hidden_layers"], cfg.get("num_lang_transformer_hidden_layers", 0)))
+    if cfg.get("share_params", True):  # one stack for both text passes, deep enough for either (model/modeling.py:171-172)
+        stack("encoder", max(cfg["num_hidden_layers"], cfg.get("num_lang_transformer_hidden_layers", 0)))
+    else:  # langonly_reps builds its own stack (:356-379); after the ViT in every group, so it stays in rest_ranges
+        stack("encoder", cfg["num_hidden_layers"])
+        stack("langonly_encoder", cfg["num_lang_transformer_hidden_layers"])
     if cfg.get("do_projection", False):
         lin("lm_head/projection", H, H)
         ln("lm_head/LayerNorm")

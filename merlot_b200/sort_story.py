@@ -335,12 +335,12 @@ def zero_shot_predict(config, store, batch: Dict, duplication_factor: int = 2, s
 
 
 def zero_shot_variables(store) -> List[str]:
-    """The entries the zero-shot forward reads: everything but the language-only embeddings, the pretraining heads and the
-    encoder layers beyond the joint encoder's depth."""
+    """The entries the zero-shot forward reads: everything but the language-only embeddings and encoder (share_params:
+    False), the pretraining heads and the encoder layers beyond the joint encoder's depth."""
     joint = store.cfg["num_hidden_layers"]
 
     def read(name):
-        if name.startswith(("langonly_embeddings/", "lm_head/", "contrastive/")):
+        if name.startswith(("langonly_embeddings/", "langonly_encoder/", "lm_head/", "contrastive/")):
             return False
         m = re.match(r"encoder/layer(\d+)/", name)
         return m is None or int(m.group(1)) < joint
