@@ -33,6 +33,8 @@ START = 2
 _SITE_VIT, _SITE_LANGONLY, _SITE_JOINT, _SITE_EMB_LO, _SITE_EMB_J = 0, 100, 200, 300, 301
 # VCR classifier towers (merlot_b200/vcr.py cls_head): dropout of each tower's input and of its hidden layer
 _SITE_VCR_ANS_IN, _SITE_VCR_ANS_HID, _SITE_VCR_RAT_IN, _SITE_VCR_RAT_HID = 400, 401, 402, 403
+# the multiple-choice video QA tower (merlot_b200/video_mc.py mc_head): dropout of its input and of its hidden layer
+_SITE_MC_IN, _SITE_MC_HID = 410, 411
 _VIT = "vision_backbone/vision_transformer"
 
 

@@ -11,10 +11,12 @@ Storage differs from the TF variables in three places (converted by load_tf_dict
     to 8 columns so their rows are 16-byte aligned for TMA; `Entry.ref_cols` records how many columns the reference has;
   * the patch conv kernel [P,P,3,H] is stored as the im2col matrix [P*P*3, H] (same memory order).
 
-`task` selects the variable set of one reference graph: "pretrain" (model/modeling.py model_fn, every head) or "vcr"
-(downstream/vcr/modeling.py model_fn: MerlotModel(mask_input=False) + the answer / rationale classifier towers).  In
-pretraining, `share_params: False` gives the language-only pass its own `langonly_encoder/` stack of
-num_lang_transformer_hidden_layers layers beside the joint `encoder/`; the VCR graph has no language-only pass and ignores it.
+`task` selects the variable set of one reference graph: "pretrain" (model/modeling.py model_fn, every head), "vcr"
+(downstream/vcr/modeling.py model_fn: MerlotModel(mask_input=False) + the answer / rationale classifier towers) or
+"video_mc" (multiple-choice video QA, merlot_b200/video_mc.py: the VCR graph's model variables + one `mc_cls` tower of the
+answer tower's shapes and initialisers).  In pretraining, `share_params: False` gives the language-only pass its own
+`langonly_encoder/` stack of num_lang_transformer_hidden_layers layers beside the joint `encoder/`; the VCR and video_mc
+graphs have no language-only pass and ignore it.
 
 save_checkpoint / restore_checkpoint write and read the whole training state (parameters, Adam slots, global_step) as the
 TensorFlow V2 checkpoints the reference's Estimator keeps in output_dir.
@@ -34,8 +36,9 @@ from .stem import stem_ops
 
 PAD = 64
 TEMPORAL_PAD_N = 8
-TASKS = ("pretrain", "vcr")
+TASKS = ("pretrain", "vcr", "video_mc")
 VCR_TOWERS = ("answer_cls", "rationale_cls")
+VIDEO_MC_TOWERS = ("mc_cls",)
 VCR_BIAS_PI = 0.25  # cls_head(hidden_state, bias_pi=0.25), downstream/vcr/modeling.py:77
 
 
@@ -96,11 +99,12 @@ def _entries(cfg: dict, task: str = "pretrain") -> List[Entry]:
     add("vision_backbone/final_pe/cls_emb", (1, H))
     ln("vision_backbone/LayerNorm_final_ln")
     add("word_embeddings/word_embeddings", (V, H))
-    if task == "vcr":  # mask_input=False: no language-only encoder, no masking, no pretraining heads
+    if task in ("vcr", "video_mc"):  # mask_input=False: no language-only encoder, no masking, no pretraining heads
         add("position_embeddings/position_embeddings", (cfg["max_position_embeddings"], H))
         ln("position_embeddings/LayerNorm_embed_norm")
         stack("encoder", cfg["num_hidden_layers"])
-        for tower in VCR_TOWERS:  # downstream/vcr/modeling.py:86-121, in creation order
+        # VCR: downstream/vcr/modeling.py:86-121, in creation order; video_mc: one tower of VCR's shapes over C candidates
+        for tower in (VCR_TOWERS if task == "vcr" else VIDEO_MC_TOWERS):
             lin(f"{tower}/classifier_mlp0", H, H // 2)
             add(f"{tower}/classifier_mlp1/kernel", (H // 2, TEMPORAL_PAD_N), ref_cols=1)
             add(f"{tower}/classifier_mlp1/bias", (TEMPORAL_PAD_N,), ref_cols=1)

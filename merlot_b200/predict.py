@@ -116,8 +116,8 @@ def main(argv=None) -> Optional[List[str]]:
     ap.add_argument("--seed", type=int, default=0, help="seed of the evaluation draws (parser, dropout and masking)")
     args = ap.parse_args(argv)
     config = NeatConfig.from_yaml(args.config_file)
-    if config.downstream.get("task") == "vcr":
-        raise ValueError("downstream.task is 'vcr': PREDICT runs on the pretraining model")
+    if config.downstream.get("task") in ("vcr", "video_mc"):
+        raise ValueError(f"downstream.task is {config.downstream.get('task')!r}: PREDICT runs on the pretraining model")
     check_val_file(config)
     eval_batch_count(config)
     prefix = args.checkpoint

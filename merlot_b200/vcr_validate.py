@@ -75,12 +75,15 @@ def log_softmax(logits: np.ndarray) -> np.ndarray:
 class Validator:
     """Evaluates checkpoints of a VCR run on the evaluation input of config (data.val_file, downstream.mode).  With an
     eval_ranks.EvalGroup of several ranks, each rank evaluates the global batches k with k % world == rank, and every rank
-    gets the result one rank would compute."""
+    gets the result one rank would compute.  video_mc_validate.Validator is this class over another task: the class
+    attributes and the three methods after __init__ are what a task sets."""
+    TASK = "vcr"
+    METRIC = "avg"                     # the results line's name of the mean accuracy
+    ID_KEYS = ("annot_id", "img_id")   # per-question host strings of a batch, kept in the predictions
 
     def __init__(self, config, chunk: int = 0, device="cuda", group=None):
         from .eval_ranks import EvalGroup
         from .params import ParamStore
-        from .vcr import vcr_model_fn_builder
         self.group = group if group is not None else EvalGroup()
         self.config = config
         self.batch_size = int(config.device.get("val_batch_size", 64))
@@ -89,28 +92,39 @@ class Validator:
         if self.num_batches < 1:
             raise ValueError(f"validate.eval_samples {config.validate.get('eval_samples')!r} is less than one batch of "
                              f"device.val_batch_size {self.batch_size}")
-        self.store = ParamStore(config.model, device=device, optimizer_cfg=config.optimizer, task="vcr")
-        self.model_fn = vcr_model_fn_builder(config, store=self.store, device=device)
+        self.store = ParamStore(config.model, device=device, optimizer_cfg=config.optimizer, task=self.TASK)
+        self.model_fn = self._model_fn_builder()(config, store=self.store, device=device)
         self.device = device
+
+    def _model_fn_builder(self):
+        from .vcr import vcr_model_fn_builder
+        return vcr_model_fn_builder
+
+    def _input(self, labelled: bool):
+        from . import vcr_input
+        g = self.group
+        return vcr_input.input_fn_builder(self.config, is_training=False, rank=g.rank, world=g.world,
+                                          batch_size=self.batch_size, device=self.device, labelled=labelled)
+
+    def _chunk(self, batch, a: int, n: int) -> Dict:
+        """The features of questions a .. a+n-1 of an evaluation batch."""
+        return {k: batch[k][a:a + n] for k in ("images", "lm_input", "lm_targets")}
 
     def _own_batches(self, prefix: str, labelled: bool, keep_predictions: bool) -> List[Dict]:
         """Restore `prefix` and evaluate this rank's batches among the first num_batches.  Per batch: its loss (a device
         scalar), the correct count of every chunk, and with keep_predictions every chunk's logits and the batch's ids and
         labels.  With several ranks the tensors are copied to the host for the gather."""
         import torch
-        from . import vcr_input
         g = self.group
         self.store.restore_checkpoint(prefix)
         mode = "eval" if labelled else "predict"
         out = []
-        with torch.no_grad(), vcr_input.input_fn_builder(self.config, is_training=False, rank=g.rank, world=g.world,
-                                                         batch_size=self.batch_size, device=self.device,
-                                                         labelled=labelled) as pipe:
+        with torch.no_grad(), self._input(labelled) as pipe:
             for _, batch in zip(range(len(range(g.rank, self.num_batches, g.world))), pipe):
                 batch_loss = torch.zeros((), dtype=torch.float32, device=self.device)
                 res = {"correct": [], "logits": []}
                 for a in range(0, self.batch_size, self.chunk):
-                    feats = {k: batch[k][a:a + self.chunk] for k in ("images", "lm_input", "lm_targets")}
+                    feats = self._chunk(batch, a, self.chunk)
                     spec = self.model_fn(feats, None, mode)
                     n = feats["lm_targets"].shape[0]
                     if labelled:  # cls_loss gives chunk means; weigh them by the chunk's share of the batch
@@ -120,7 +134,7 @@ class Validator:
                         res["logits"].append(spec.metrics["logits"].clone())
                 res["loss"] = batch_loss
                 if keep_predictions:
-                    res.update(annot_id=batch["annot_id"], img_id=batch["img_id"], label=batch["lm_targets"].cpu().numpy())
+                    res.update({k: batch[k] for k in self.ID_KEYS}, label=batch["lm_targets"].cpu().numpy())
                 out.append(res)
         if g.world > 1:  # host copies for the gather
             for b in out:
@@ -130,7 +144,7 @@ class Validator:
         return out
 
     def evaluate(self, prefix: str, labelled: bool = True, keep_predictions: bool = False) -> Dict:
-        """Restore `prefix` and evaluate.  Returns {global_step, avg, loss, questions} (avg and loss None when not
+        """Restore `prefix` and evaluate.  Returns {global_step, METRIC, loss, questions} (METRIC and loss None when not
         labelled), plus per-question arrays under 'predictions' when keep_predictions.  With several ranks every rank
         returns the same result, reduced in global batch order on this rank's device by the same operations one rank
         runs; a failure on any rank raises RankFailure on every rank."""
@@ -142,30 +156,31 @@ class Validator:
         losses = [b["loss"].to(dev) for b in batches]
         correct = [c.to(dev) for b in batches for c in b["correct"]]
         logits = [x.to(dev) for b in batches for x in b["logits"]]
-        rows = {"annot_id": [a for b in batches for a in b.get("annot_id", [])],
-                "img_id": [a for b in batches for a in b.get("img_id", [])], "label": [b["label"] for b in batches if "label" in b]}
+        rows = {k: [a for b in batches for a in b.get(k, [])] for k in self.ID_KEYS}
+        rows["label"] = [b["label"] for b in batches if "label" in b]
         questions = len(losses) * self.batch_size
         if questions == 0:
             raise ValueError(f"data.val_file holds no whole batch of {self.batch_size} questions")
-        res = {"global_step": self.store.global_step, "avg": None, "loss": None, "questions": questions}
+        res = {"global_step": self.store.global_step, self.METRIC: None, "loss": None, "questions": questions}
         if labelled:
-            res["avg"] = float(torch.stack(correct).sum()) / questions
+            res[self.METRIC] = float(torch.stack(correct).sum()) / questions
             res["loss"] = float(torch.stack(losses).mean())
         if keep_predictions:
             lg = torch.cat(logits).float().cpu().numpy()
             lp = log_softmax(lg)
-            res["predictions"] = {"annot_id": np.array(rows["annot_id"]), "img_id": np.array(rows["img_id"]),
-                                  "log_prob": lp, "prediction": lp.argmax(-1).astype(np.int64),
-                                  "label": np.concatenate(rows["label"]).astype(np.int64)}
+            res["predictions"] = dict({k: np.array(rows[k]) for k in self.ID_KEYS}, log_prob=lp,
+                                      prediction=lp.argmax(-1).astype(np.int64),
+                                      label=np.concatenate(rows["label"]).astype(np.int64))
         return res
 
 
-def append_result(output_dir: str, res: Dict) -> str:
-    """Append {global_step, avg, loss, questions} as one JSON line to output_dir/eval/results.jsonl; returns its path."""
+def append_result(output_dir: str, res: Dict, metric: str = "avg") -> str:
+    """Append {global_step, <metric>, loss, questions} as one JSON line to output_dir/eval/results.jsonl; returns its
+    path."""
     path = os.path.join(output_dir, RESULTS_FILE)
     os.makedirs(os.path.dirname(path), exist_ok=True)
     with open(path, "a", encoding="utf-8") as f:
-        f.write(json.dumps({k: res[k] for k in ("global_step", "avg", "loss", "questions")}) + "\n")
+        f.write(json.dumps({k: res[k] for k in ("global_step", metric, "loss", "questions")}) + "\n")
     return path
 
 
@@ -175,8 +190,15 @@ def write_predictions(path: str, predictions: Dict[str, np.ndarray]) -> None:
 
 def main(argv=None, clock: Callable[[], float] = time.monotonic, sleep: Callable[[float], None] = time.sleep):
     """Returns the result dict of every evaluated checkpoint, in order."""
+    return run(Validator, "Validate VCR fine-tuning checkpoints (downstream/vcr/validate.py)", "VCR", argv, clock, sleep)
+
+
+def run(validator_cls, description: str, task_name: str, argv=None, clock: Callable[[], float] = time.monotonic,
+        sleep: Callable[[float], None] = time.sleep):
+    """The command line of a validator: follow device.output_dir (or evaluate --checkpoint) with `validator_cls` on every
+    rank, rank 0 writing the results lines and predictions.  Returns the result dict of every evaluated checkpoint."""
     from .config import NeatConfig
-    ap = argparse.ArgumentParser(description="Validate VCR fine-tuning checkpoints (downstream/vcr/validate.py)")
+    ap = argparse.ArgumentParser(description=description)
     ap.add_argument("config_file")
     ap.add_argument("--checkpoint", help="evaluate this checkpoint prefix once instead of following device.output_dir")
     ap.add_argument("--predictions", help="write per-question predictions to this .npz (needs --checkpoint)")
@@ -194,8 +216,9 @@ def main(argv=None, clock: Callable[[], float] = time.monotonic, sleep: Callable
     if args.chunk < 0:
         raise ValueError(f"--chunk {args.chunk} must be >= 0")
     config = NeatConfig.from_yaml(args.config_file)
-    if config.downstream.get("task") != "vcr":
-        raise ValueError(f"downstream.task is {config.downstream.get('task')!r}, VCR validation needs 'vcr'")
+    if config.downstream.get("task") != validator_cls.TASK:
+        raise ValueError(f"downstream.task is {config.downstream.get('task')!r}, {task_name} validation needs "
+                         f"{validator_cls.TASK!r}")
     output_dir = str(config.device["output_dir"])
     if "://" in output_dir:
         raise ValueError(f"device.output_dir {output_dir!r}: only local directories are supported for checkpoints")
@@ -211,15 +234,16 @@ def main(argv=None, clock: Callable[[], float] = time.monotonic, sleep: Callable
         if args.predictions:
             write_predictions(args.predictions, res["predictions"])
         if not args.unlabelled:
-            path = append_result(output_dir, res)
-            print(f"{prefix}: global_step {res['global_step']} avg {res['avg']:.4f} loss {res['loss']:.4f} over "
+            metric = validator_cls.METRIC
+            path = append_result(output_dir, res, metric)
+            print(f"{prefix}: global_step {res['global_step']} {metric} {res[metric]:.4f} loss {res['loss']:.4f} over "
                   f"{res['questions']} questions -> {path}", flush=True)
         else:
             print(f"{prefix}: predictions of {res['questions']} questions -> {args.predictions}", flush=True)
 
     results = []
     with eval_group() as group:  # WORLD_SIZE > 1: rank 0 follows the checkpoints and writes, every rank evaluates
-        v = Validator(config, chunk=args.chunk, group=group)
+        v = validator_cls(config, chunk=args.chunk, group=group)
         for prefix in group.shared_prefixes(follow, sleep):
             res = v.evaluate(prefix, labelled=not args.unlabelled, keep_predictions=bool(args.predictions))
             group.on_rank0(lambda: write(prefix, res))
