@@ -35,6 +35,8 @@ _SITE_VIT, _SITE_LANGONLY, _SITE_JOINT, _SITE_EMB_LO, _SITE_EMB_J = 0, 100, 200,
 _SITE_VCR_ANS_IN, _SITE_VCR_ANS_HID, _SITE_VCR_RAT_IN, _SITE_VCR_RAT_HID = 400, 401, 402, 403
 # the multiple-choice video QA tower (merlot_b200/video_mc.py mc_head): dropout of its input and of its hidden layer
 _SITE_MC_IN, _SITE_MC_HID = 410, 411
+# the open-ended video QA tower (merlot_b200/video_qa.py qa_head): dropout of its input and of its hidden layer
+_SITE_QA_IN, _SITE_QA_HID = 420, 421
 _VIT = "vision_backbone/vision_transformer"
 
 

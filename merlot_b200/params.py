@@ -14,9 +14,10 @@ Storage differs from the TF variables in three places (converted by load_tf_dict
 `task` selects the variable set of one reference graph: "pretrain" (model/modeling.py model_fn, every head), "vcr"
 (downstream/vcr/modeling.py model_fn: MerlotModel(mask_input=False) + the answer / rationale classifier towers) or
 "video_mc" (multiple-choice video QA, merlot_b200/video_mc.py: the VCR graph's model variables + one `mc_cls` tower of the
-answer tower's shapes and initialisers).  In pretraining, `share_params: False` gives the language-only pass its own
+answer tower's shapes and initialisers) or "video_qa" (open-ended video QA, merlot_b200/video_qa.py: the VCR graph's model
+variables + one `qa_cls` tower whose output layer has A = `num_answers` columns, zero-padded to a multiple of 8).  In pretraining, `share_params: False` gives the language-only pass its own
 `langonly_encoder/` stack of num_lang_transformer_hidden_layers layers beside the joint `encoder/`; the VCR and video_mc
-graphs have no language-only pass and ignore it.
+graphs have no language-only pass and ignore it (as do video_qa's).
 
 save_checkpoint / restore_checkpoint write and read the whole training state (parameters, Adam slots, global_step) as the
 TensorFlow V2 checkpoints the reference's Estimator keeps in output_dir.
@@ -36,9 +37,10 @@ from .stem import stem_ops
 
 PAD = 64
 TEMPORAL_PAD_N = 8
-TASKS = ("pretrain", "vcr", "video_mc")
+TASKS = ("pretrain", "vcr", "video_mc", "video_qa")
 VCR_TOWERS = ("answer_cls", "rationale_cls")
 VIDEO_MC_TOWERS = ("mc_cls",)
+VIDEO_QA_TOWER = "qa_cls"
 VCR_BIAS_PI = 0.25  # cls_head(hidden_state, bias_pi=0.25), downstream/vcr/modeling.py:77
 
 
@@ -54,7 +56,12 @@ class Entry:
     ref_cols: int = 0           # > 0: the last dim is zero-padded; the reference variable has this many columns
 
 
-def _entries(cfg: dict, task: str = "pretrain") -> List[Entry]:
+def padded_answers(num_answers: int) -> int:
+    """A8: the columns of the video_qa tower's output layer, num_answers rounded up to a multiple of 8 (16-byte rows)."""
+    return (num_answers + TEMPORAL_PAD_N - 1) // TEMPORAL_PAD_N * TEMPORAL_PAD_N
+
+
+def _entries(cfg: dict, task: str = "pretrain", num_answers: int = 0) -> List[Entry]:
     H, I, V = cfg["hidden_size"], cfg["intermediate_size"], cfg["vocab_size"]
     P = cfg["patch_size"]
     out: List[Entry] = []
@@ -99,10 +106,16 @@ def _entries(cfg: dict, task: str = "pretrain") -> List[Entry]:
     add("vision_backbone/final_pe/cls_emb", (1, H))
     ln("vision_backbone/LayerNorm_final_ln")
     add("word_embeddings/word_embeddings", (V, H))
-    if task in ("vcr", "video_mc"):  # mask_input=False: no language-only encoder, no masking, no pretraining heads
+    if task in ("vcr", "video_mc", "video_qa"):  # mask_input=False: no language-only encoder, no masking, no pretraining heads
         add("position_embeddings/position_embeddings", (cfg["max_position_embeddings"], H))
         ln("position_embeddings/LayerNorm_embed_norm")
         stack("encoder", cfg["num_hidden_layers"])
+        if task == "video_qa":  # dense(H/2) + gelu, then dense(A) stored as A8 columns
+            lin(f"{VIDEO_QA_TOWER}/classifier_mlp0", H, H // 2)
+            A8 = padded_answers(num_answers)
+            add(f"{VIDEO_QA_TOWER}/classifier_mlp1/kernel", (H // 2, A8), ref_cols=num_answers)
+            add(f"{VIDEO_QA_TOWER}/classifier_mlp1/bias", (A8,), ref_cols=num_answers)
+            return out
         # VCR: downstream/vcr/modeling.py:86-121, in creation order; video_mc: one tower of VCR's shapes over C candidates
         for tower in (VCR_TOWERS if task == "vcr" else VIDEO_MC_TOWERS):
             lin(f"{tower}/classifier_mlp0", H, H // 2)
@@ -182,18 +195,24 @@ def hyper_for(tf_name: str, optimizer_cfg: dict) -> Tuple[float, float, float, f
 class ParamStore:
     """Flat arenas + named views.  `optimizer_cfg` fixes the hyper-parameter grouping (needed only for training) and the
     Adam moments' storage: fp32 unless it sets use_bfloat16_adam (the reference's default is False); without an
-    optimizer_cfg the moments are bf16."""
+    optimizer_cfg the moments are bf16.  `num_answers` (task "video_qa" only, >= 2) is the answer vocabulary's size A."""
 
     def __init__(self, model_cfg: dict, device="cuda", optimizer_cfg: Optional[dict] = None, with_optimizer_state=True,
-                 task: str = "pretrain"):
+                 task: str = "pretrain", num_answers: Optional[int] = None):
         # resnet_layers != [] selects the hybrid ResNet-lite stem (utils/vision_transformer.py:206-223); forward and backward
         # are provided (K13), its variables follow the reference's creation order (stem_variables).
         if task not in TASKS:
             raise ValueError(f"ParamStore task must be one of {TASKS}, got {task!r}")
+        if (task == "video_qa") != (num_answers is not None):
+            raise ValueError(f"num_answers is the size of the video_qa answer vocabulary: task={task!r}, "
+                             f"num_answers={num_answers!r}")
+        if task == "video_qa" and int(num_answers) < 2:
+            raise ValueError(f"video_qa: num_answers must be >= 2, got {num_answers}")
         self.cfg = model_cfg
         self.task = task
+        self.num_answers = None if num_answers is None else int(num_answers)
         self.device = torch.device(device)
-        ents = _entries(model_cfg, task)
+        ents = _entries(model_cfg, task, self.num_answers or 0)
         ocfg = optimizer_cfg or {"learning_rate": 0.0, "param_overrides": [
             [["LayerNorm", "layer_norm", "GroupNorm", "bias"], {"weight_decay_rate": 0}]]}
         for e in ents:
@@ -484,7 +503,8 @@ class ParamStore:
 
     def init_reference(self, seed: int = 0):
         """Reference initialisers (truncated normal 0.02 / variance-scaling patch kernel / LN 1,0 / zero biases; the VCR
-        towers' output bias is -log((1 - pi) / pi), downstream/vcr/modeling.py:71)."""
+        towers' output bias is -log((1 - pi) / pi), downstream/vcr/modeling.py:71, and so is video_mc's; video_qa's output
+        bias stays zero, so that no answer is favoured)."""
         g = torch.Generator().manual_seed(seed)
         std = self.cfg.get("initializer_range", 0.02)
         with torch.no_grad():
@@ -494,7 +514,7 @@ class ParamStore:
                     t = torch.ones(e.shape)
                 elif leaf in ("beta", "bias", "output_bias"):
                     t = torch.zeros(e.shape)
-                    if e.name.endswith("_cls/classifier_mlp1/bias"):
+                    if e.name.endswith("_cls/classifier_mlp1/bias") and not e.name.startswith(VIDEO_QA_TOWER + "/"):
                         t[0] = -math.log((1 - VCR_BIAS_PI) / VCR_BIAS_PI)
                 else:
                     s_ = std

@@ -75,11 +75,12 @@ def log_softmax(logits: np.ndarray) -> np.ndarray:
 class Validator:
     """Evaluates checkpoints of a VCR run on the evaluation input of config (data.val_file, downstream.mode).  With an
     eval_ranks.EvalGroup of several ranks, each rank evaluates the global batches k with k % world == rank, and every rank
-    gets the result one rank would compute.  video_mc_validate.Validator is this class over another task: the class
-    attributes and the three methods after __init__ are what a task sets."""
+    gets the result one rank would compute.  video_mc_validate.Validator and video_qa_validate.Validator are this class
+    over other tasks: the class attributes and the methods between __init__ and _own_batches are what a task sets."""
     TASK = "vcr"
     METRIC = "avg"                     # the results line's name of the mean accuracy
     ID_KEYS = ("annot_id", "img_id")   # per-question host strings of a batch, kept in the predictions
+    EXTRA_KEYS = ()                    # results-line entries after global_step, METRIC, loss and questions
 
     def __init__(self, config, chunk: int = 0, device="cuda", group=None):
         from .eval_ranks import EvalGroup
@@ -92,9 +93,14 @@ class Validator:
         if self.num_batches < 1:
             raise ValueError(f"validate.eval_samples {config.validate.get('eval_samples')!r} is less than one batch of "
                              f"device.val_batch_size {self.batch_size}")
-        self.store = ParamStore(config.model, device=device, optimizer_cfg=config.optimizer, task=self.TASK)
+        self.store = ParamStore(config.model, device=device, optimizer_cfg=config.optimizer, task=self.TASK,
+                                **self._store_options())
         self.model_fn = self._model_fn_builder()(config, store=self.store, device=device)
         self.device = device
+
+    def _store_options(self) -> Dict:
+        """Keyword arguments of the task's ParamStore besides the model config and the task."""
+        return {}
 
     def _model_fn_builder(self):
         from .vcr import vcr_model_fn_builder
@@ -110,6 +116,25 @@ class Validator:
         """The features of questions a .. a+n-1 of an evaluation batch."""
         return {k: batch[k][a:a + n] for k in ("images", "lm_input", "lm_targets")}
 
+    def _score(self, res: Dict, metrics: Dict, n: int) -> None:
+        """Add the eval metrics of a labelled chunk of n questions to its batch's `res` (res['loss'], a device scalar, and
+        the lists of device scalars in res)."""
+        res["loss"] += metrics["loss"] * (n / self.batch_size)  # cls_loss gives chunk means; weigh them by the chunk's share
+        res["correct"].append(metrics["accuracy"] * n)
+
+    def _metrics(self, batches: List[Dict], questions: int) -> Dict:
+        """{METRIC, loss} of the labelled batches in global batch order, on this rank's device."""
+        import torch
+        dev = self.device
+        losses = [b["loss"].to(dev) for b in batches]
+        correct = [c.to(dev) for b in batches for c in b["correct"]]
+        return {self.METRIC: float(torch.stack(correct).sum()) / questions, "loss": float(torch.stack(losses).mean())}
+
+    def _prediction_arrays(self, logits: np.ndarray) -> Dict[str, np.ndarray]:
+        """The per-question arrays of the predictions file computed from the fp32 logits [n, classes]."""
+        lp = log_softmax(logits)
+        return {"log_prob": lp, "prediction": lp.argmax(-1).astype(np.int64)}
+
     def _own_batches(self, prefix: str, labelled: bool, keep_predictions: bool) -> List[Dict]:
         """Restore `prefix` and evaluate this rank's batches among the first num_batches.  Per batch: its loss (a device
         scalar), the correct count of every chunk, and with keep_predictions every chunk's logits and the batch's ids and
@@ -121,26 +146,25 @@ class Validator:
         out = []
         with torch.no_grad(), self._input(labelled) as pipe:
             for _, batch in zip(range(len(range(g.rank, self.num_batches, g.world))), pipe):
-                batch_loss = torch.zeros((), dtype=torch.float32, device=self.device)
-                res = {"correct": [], "logits": []}
+                res = {"loss": torch.zeros((), dtype=torch.float32, device=self.device), "correct": [], "logits": []}
                 for a in range(0, self.batch_size, self.chunk):
                     feats = self._chunk(batch, a, self.chunk)
                     spec = self.model_fn(feats, None, mode)
                     n = feats["lm_targets"].shape[0]
-                    if labelled:  # cls_loss gives chunk means; weigh them by the chunk's share of the batch
-                        batch_loss += spec.metrics["loss"] * (n / self.batch_size)
-                        res["correct"].append(spec.metrics["accuracy"] * n)
+                    if labelled:
+                        self._score(res, spec.metrics, n)
                     if keep_predictions:
                         res["logits"].append(spec.metrics["logits"].clone())
-                res["loss"] = batch_loss
                 if keep_predictions:
                     res.update({k: batch[k] for k in self.ID_KEYS}, label=batch["lm_targets"].cpu().numpy())
                 out.append(res)
         if g.world > 1:  # host copies for the gather
             for b in out:
-                b["loss"] = b["loss"].cpu()
-                b["correct"] = [c.cpu() for c in b["correct"]]
-                b["logits"] = [x.cpu() for x in b["logits"]]
+                for k, v in b.items():
+                    if torch.is_tensor(v):
+                        b[k] = v.cpu()
+                    elif isinstance(v, list) and v and torch.is_tensor(v[0]):
+                        b[k] = [x.cpu() for x in v]
         return out
 
     def evaluate(self, prefix: str, labelled: bool = True, keep_predictions: bool = False) -> Dict:
@@ -153,34 +177,30 @@ class Validator:
         per_rank = self.group.run_and_gather(lambda: self._own_batches(prefix, labelled, keep_predictions))
         batches = in_batch_order(per_rank)
         dev = self.device
-        losses = [b["loss"].to(dev) for b in batches]
-        correct = [c.to(dev) for b in batches for c in b["correct"]]
         logits = [x.to(dev) for b in batches for x in b["logits"]]
         rows = {k: [a for b in batches for a in b.get(k, [])] for k in self.ID_KEYS}
         rows["label"] = [b["label"] for b in batches if "label" in b]
-        questions = len(losses) * self.batch_size
+        questions = len(batches) * self.batch_size
         if questions == 0:
             raise ValueError(f"data.val_file holds no whole batch of {self.batch_size} questions")
         res = {"global_step": self.store.global_step, self.METRIC: None, "loss": None, "questions": questions}
+        res.update({k: None for k in self.EXTRA_KEYS})
         if labelled:
-            res[self.METRIC] = float(torch.stack(correct).sum()) / questions
-            res["loss"] = float(torch.stack(losses).mean())
+            res.update(self._metrics(batches, questions))
         if keep_predictions:
             lg = torch.cat(logits).float().cpu().numpy()
-            lp = log_softmax(lg)
-            res["predictions"] = dict({k: np.array(rows[k]) for k in self.ID_KEYS}, log_prob=lp,
-                                      prediction=lp.argmax(-1).astype(np.int64),
+            res["predictions"] = dict({k: np.array(rows[k]) for k in self.ID_KEYS}, **self._prediction_arrays(lg),
                                       label=np.concatenate(rows["label"]).astype(np.int64))
         return res
 
 
-def append_result(output_dir: str, res: Dict, metric: str = "avg") -> str:
-    """Append {global_step, <metric>, loss, questions} as one JSON line to output_dir/eval/results.jsonl; returns its
-    path."""
+def append_result(output_dir: str, res: Dict, metric: str = "avg", extra=()) -> str:
+    """Append {global_step, <metric>, loss, questions, *extra} as one JSON line to output_dir/eval/results.jsonl; returns
+    its path."""
     path = os.path.join(output_dir, RESULTS_FILE)
     os.makedirs(os.path.dirname(path), exist_ok=True)
     with open(path, "a", encoding="utf-8") as f:
-        f.write(json.dumps({k: res[k] for k in ("global_step", metric, "loss", "questions")}) + "\n")
+        f.write(json.dumps({k: res[k] for k in ("global_step", metric, "loss", "questions") + tuple(extra)}) + "\n")
     return path
 
 
@@ -235,8 +255,9 @@ def run(validator_cls, description: str, task_name: str, argv=None, clock: Calla
             write_predictions(args.predictions, res["predictions"])
         if not args.unlabelled:
             metric = validator_cls.METRIC
-            path = append_result(output_dir, res, metric)
-            print(f"{prefix}: global_step {res['global_step']} {metric} {res[metric]:.4f} loss {res['loss']:.4f} over "
+            path = append_result(output_dir, res, metric, validator_cls.EXTRA_KEYS)
+            loss = "none" if res["loss"] is None else f"{res['loss']:.4f}"  # video_qa: no in-vocabulary question
+            print(f"{prefix}: global_step {res['global_step']} {metric} {res[metric]:.4f} loss {loss} over "
                   f"{res['questions']} questions -> {path}", flush=True)
         else:
             print(f"{prefix}: predictions of {res['questions']} questions -> {args.predictions}", flush=True)

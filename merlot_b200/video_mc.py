@@ -9,7 +9,9 @@ tower instead of two and C candidates instead of 4:
     ParamStore(task="video_mc"); the backward writes the tower's gradients into store.g and returns the gradient that
     enters the model through MerlotModel.backward(d_hidden_state=...);
   * `video_mc_model_fn_builder`: the fine-tuning step (train), the validation forward (eval) and the scoring forward
-    (predict), with the call shape of vcr.vcr_model_fn_builder.
+    (predict), with the call shape of vcr.vcr_model_fn_builder;
+  * `tower_forward` / `tower_backward`: the tower's kernel sequence on given rows of the hidden state, which the open-ended
+    video QA head (video_qa.py) runs as well.
 All arithmetic runs in libmerlot_b200.so: the row gather / scatter, dropout, the K1 GEMM with its fused epilogues, the
 strided fp32 small GEMM, the CE kernel and the bias-gradient kernel -- the kernels of VCR's head.  C <= 8 because the tower's
 dense(1) output is padded to 8 columns, and the logits of a question are a row of those 8 columns.
@@ -64,24 +66,13 @@ def mc_head(model, store, dropout=(0.0, 0)) -> torch.Tensor:
     if not MIN_CHOICES <= C <= MAX_CHOICES or B % C != 0:
         raise ValueError(f"the video_mc head scores {MIN_CHOICES}..{MAX_CHOICES} candidates per question: batch {B}, "
                          f"num_texts {C}")
-    b, H2 = B // C, H // 2
+    b = B // C
     p, seed = float(dropout[0]), int(dropout[1])
     bf = model._bufs
     idx, sel = _head_index(model, b, C, Sj)
-    x = bf.get("mc.x", (B, H), torch.bfloat16)
-    ops.gather_rows(y.reshape(B * Sj, H), idx, x)
-    xd = x
-    if p > 0.0:
-        xd = bf.get("mc.xd", (B, H), torch.bfloat16)
-        ops.dropout_apply(x, xd, p, seed, _SITE_MC_IN)
-    # dense(H/2) + erf-GeLU, dropout: h <- drop(gelu(pre)); gp <- gelu'(pre) for the backward
-    h = bf.get("mc.h", (B, H2), torch.bfloat16)
-    gp = bf.get("mc.gp", (B, H2), torch.bfloat16)
-    ops.gemm(xd, store.W(f"{TOWER}/classifier_mlp0/kernel"), b_mn_major=True, bias=store.P(f"{TOWER}/classifier_mlp0/bias"),
-             gelu=True, out_pre=gp, gelu_grad_out=True, out=h, dropout_p=p, dropout_seed=seed, dropout_site=_SITE_MC_HID)
     # dense(1) with N = 1 padded to 8: z[q*C + c, 0] is the logit of question q, candidate c
     z = bf.get("mc.z", (B, 8), torch.float32)
-    ops.gemm(h, store.W(f"{TOWER}/classifier_mlp1/kernel"), b_mn_major=True, bias=store.P(f"{TOWER}/classifier_mlp1/bias"), out=z)
+    xd, h, gp = tower_forward(bf, store, TOWER, y, idx, z, (p, seed, _SITE_MC_IN, _SITE_MC_HID), "mc")
     # logits[q, c] = sum_k z[q, k] E[k, c] over z viewed as [b, 8C]: an exact strided copy of column 0
     logits = torch.empty((b, 8), dtype=torch.float32, device=y.device)
     ops.small_gemm(z, 8 * C, 1, sel, 1, C, logits, b, C, 8 * C)
@@ -115,32 +106,65 @@ def mc_head_backward(model, store) -> torch.Tensor:
         raise RuntimeError("mc_head_backward needs mc_head(model, store, ...) and mc_loss(model, target) first")
     logits, x, h, gp, p, seed, C = (st[k] for k in ("logits", "x", "h", "gp", "p", "seed", "C"))
     y = model.encoder_info["hidden_state"]
-    B, Sj, H = y.shape
-    b, H2 = B // C, H // 2
+    B = y.shape[0]
+    b = B // C
     bf = model._bufs
-    idx, sel = _head_index(model, b, C, Sj)
+    idx, sel = _head_index(model, b, C, y.shape[1])
     dlog = bf.get("mc.dlogits", (b, 8), torch.float32)
     ops.softmax_ce_bwd(logits, st["target"], C, st["lse"], st["coeff"], dlog)
     # dz[q*C + c, 0] = dlogits[q, c], columns 1..7 zero: dz viewed as [b, 8C] = dlogits[:, :C] E^T
     dz = bf.get("mc.dz", (B, 8), torch.float32)
     ops.small_gemm(dlog, 8, 1, sel, C, 1, dz.view(b, 8 * C), b, 8 * C, C)
-    ops.bias_grad(dz, store.G(f"{TOWER}/classifier_mlp1/bias"), rows=B, N=8)
-    dzb = bf.get("mc.dzb", (B, 8), torch.bfloat16)
+    return tower_backward(bf, store, TOWER, y, idx, dz, x, h, gp, (p, seed, _SITE_MC_IN, _SITE_MC_HID), "mc")
+
+
+def tower_forward(bf, store, tower: str, y, idx, z, dropout, key: str):
+    """The classifier tower `tower` of a ParamStore on rows `idx` (int32 [n]) of the bf16 hidden state y [B, Sj, H]:
+    gather -> dropout -> dense(H/2) + erf-GeLU -> dropout -> dense(N) into the fp32 z [n, N] (N = the stored columns of
+    classifier_mlp1, a multiple of 8).  dropout = (p, seed, input site, hidden site); buffers are named `key`.*.  Returns
+    what tower_backward reads: the tower's (dropped) input, its hidden layer and gelu'(pre)."""
+    B, Sj, H = y.shape
+    n, H2 = idx.numel(), H // 2
+    p, seed, site_in, site_hid = dropout
+    x = bf.get(f"{key}.x", (n, H), torch.bfloat16)
+    ops.gather_rows(y.reshape(B * Sj, H), idx, x)
+    xd = x
+    if p > 0.0:
+        xd = bf.get(f"{key}.xd", (n, H), torch.bfloat16)
+        ops.dropout_apply(x, xd, p, seed, site_in)
+    # dense(H/2) + erf-GeLU, dropout: h <- drop(gelu(pre)); gp <- gelu'(pre) for the backward
+    h = bf.get(f"{key}.h", (n, H2), torch.bfloat16)
+    gp = bf.get(f"{key}.gp", (n, H2), torch.bfloat16)
+    ops.gemm(xd, store.W(f"{tower}/classifier_mlp0/kernel"), b_mn_major=True, bias=store.P(f"{tower}/classifier_mlp0/bias"),
+             gelu=True, out_pre=gp, gelu_grad_out=True, out=h, dropout_p=p, dropout_seed=seed, dropout_site=site_hid)
+    ops.gemm(h, store.W(f"{tower}/classifier_mlp1/kernel"), b_mn_major=True, bias=store.P(f"{tower}/classifier_mlp1/bias"), out=z)
+    return xd, h, gp
+
+
+def tower_backward(bf, store, tower: str, y, idx, dz, x, h, gp, dropout, key: str):
+    """Backward of tower_forward from dz fp32 [n, N], the gradient of its output z.  ACCUMULATES the tower's parameter
+    gradients into store.g and returns the bf16 d_hidden_state [B*Sj, H], non-zero only at the rows `idx`."""
+    B, Sj, H = y.shape
+    n, N = dz.shape
+    H2 = H // 2
+    p, seed, site_in, site_hid = dropout
+    ops.bias_grad(dz, store.G(f"{tower}/classifier_mlp1/bias"), rows=n, N=N)
+    dzb = bf.get(f"{key}.dzb", (n, N), torch.bfloat16)
     ops.cast_f32_to_bf16(dz, dzb)
-    ops.gemm(h, dzb, a_mn_major=True, b_mn_major=True, out=store.G(f"{TOWER}/classifier_mlp1/kernel"), atomic=True,
-             M=H2, N=8, K=B)
+    ops.gemm(h, dzb, a_mn_major=True, b_mn_major=True, out=store.G(f"{tower}/classifier_mlp1/kernel"), atomic=True,
+             M=H2, N=N, K=n)
     # d pre = (dz W1^T) * keep/(1-p) * gelu'(pre): the hidden dropout and the GeLU backward in the dgrad epilogue
-    dpre = bf.get("mc.dpre", (B, H2), torch.bfloat16)
-    ops.gemm(dzb, store.W(f"{TOWER}/classifier_mlp1/kernel"), out=dpre, mul_aux=gp, dropout_p=p, dropout_seed=seed,
-             dropout_site=_SITE_MC_HID, M=B, N=H2, K=8)
-    ops.bias_grad(dpre, store.G(f"{TOWER}/classifier_mlp0/bias"), rows=B, N=H2)
-    ops.gemm(x, dpre, a_mn_major=True, b_mn_major=True, out=store.G(f"{TOWER}/classifier_mlp0/kernel"), atomic=True,
-             M=H, N=H2, K=B)
+    dpre = bf.get(f"{key}.dpre", (n, H2), torch.bfloat16)
+    ops.gemm(dzb, store.W(f"{tower}/classifier_mlp1/kernel"), out=dpre, mul_aux=gp, dropout_p=p, dropout_seed=seed,
+             dropout_site=site_hid, M=n, N=H2, K=N)
+    ops.bias_grad(dpre, store.G(f"{tower}/classifier_mlp0/bias"), rows=n, N=H2)
+    ops.gemm(x, dpre, a_mn_major=True, b_mn_major=True, out=store.G(f"{tower}/classifier_mlp0/kernel"), atomic=True,
+             M=H, N=H2, K=n)
     # d first-token = (dpre W0^T) * keep/(1-p): the input dropout in the dgrad epilogue
-    dx = bf.get("mc.dx", (B, H), torch.float32)
-    ops.gemm(dpre, store.W(f"{TOWER}/classifier_mlp0/kernel"), out=dx, dropout_p=p, dropout_seed=seed, dropout_site=_SITE_MC_IN,
-             M=B, N=H, K=H2)
-    d_hidden = bf.get("mc.d_hidden", (B * Sj, H), torch.bfloat16, zero=True)
+    dx = bf.get(f"{key}.dx", (n, H), torch.float32)
+    ops.gemm(dpre, store.W(f"{tower}/classifier_mlp0/kernel"), out=dx, dropout_p=p, dropout_seed=seed, dropout_site=site_in,
+             M=n, N=H, K=H2)
+    d_hidden = bf.get(f"{key}.d_hidden", (B * Sj, H), torch.bfloat16, zero=True)
     ops.scatter_add_rows(dx, idx, d_hidden)
     return d_hidden
 

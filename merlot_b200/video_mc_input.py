@@ -43,16 +43,16 @@ def _id(example) -> str:
     return bytes(v[0]).decode("utf-8", "replace") if v else ""
 
 
-def _tokens(example, key: str, rid: str, vocab_size: int, required: bool) -> np.ndarray:
+def _tokens(example, key: str, rid: str, vocab_size: int, required: bool, task: str = "video_mc") -> np.ndarray:
     v = example.get(key)
     if v is None:
         if required:
-            raise ValueError(f"video_mc record id={rid!r}: {key} is missing")
+            raise ValueError(f"{task} record id={rid!r}: {key} is missing")
         v = []
     t = np.asarray(v, dtype=np.int64)
     bad = np.flatnonzero((t < 0) | (t >= vocab_size))
     if len(bad):
-        raise ValueError(f"video_mc record id={rid!r}: {key} holds token id {int(t[bad[0]])} outside the vocabulary "
+        raise ValueError(f"{task} record id={rid!r}: {key} holds token id {int(t[bad[0]])} outside the vocabulary "
                          f"[0, {vocab_size})")
     return t
 
@@ -84,12 +84,12 @@ def check_labels(questions: Sequence[Dict], num_choices: int) -> None:
                              f"unlabelled record can only be scored without a loss)")
 
 
-def decode_frame(question: Dict, k: int) -> np.ndarray:
-    """Frame k of a parsed question as uint8 [h, w, 3] RGB; an undecodable frame raises naming the id."""
+def decode_frame(question: Dict, k: int, task: str = "video_mc") -> np.ndarray:
+    """Frame k of a parsed question as uint8 [h, w, 3] RGB; an undecodable frame raises naming the id (and `task`)."""
     try:
         return decode_jpeg(question["jpegs"][k])
     except Exception as e:
-        raise ValueError(f"video_mc record id={question['id']!r}: frame {k} cannot be decoded ({type(e).__name__}: {e})") from e
+        raise ValueError(f"{task} record id={question['id']!r}: frame {k} cannot be decoded ({type(e).__name__}: {e})") from e
 
 
 def img_mask(questions: Sequence[Dict], num_frames: int) -> np.ndarray:
@@ -105,13 +105,13 @@ def train_draws(rng: np.random.Generator, n: int) -> Dict[str, np.ndarray]:
     return {"scale": lo + rng.random(n, dtype=f32) * (hi - lo), "u_y": rng.random(n, dtype=f32), "u_x": rng.random(n, dtype=f32)}
 
 
-def _prepare(pool, device, questions, num_frames, out_size, draws=None):
+def _prepare(pool, device, questions, num_frames, out_size, draws=None, task: str = "video_mc"):
     """Decode every frame in `pool`, plan every slot of the batch (question-major, frame-minor) and run K14 once: bf16
     [b * num_frames, H, W, 3] on `device`, the img_mask [b, num_frames] and the plan.  `draws` (train_draws of the
-    questions) selects the training plan, None the evaluation plan."""
+    questions) selects the training plan, None the evaluation plan.  Errors name the record's id and `task`."""
     from . import ops
     mask = img_mask(questions, num_frames)
-    decodes = {(i, k): pool.submit(decode_frame, q, k) for i, q in enumerate(questions) for k in range(len(q["jpegs"]))}
+    decodes = {(i, k): pool.submit(decode_frame, q, k, task) for i, q in enumerate(questions) for k in range(len(q["jpegs"]))}
     black = np.zeros((1, 1, 3), np.uint8)  # the source of every empty slot
     frames = [decodes[(i, k)].result() if mask[i, k] else black for i in range(len(questions)) for k in range(num_frames)]
     staging, offsets, hw = stage_frames(frames)
@@ -126,7 +126,7 @@ def _prepare(pool, device, questions, num_frames, out_size, draws=None):
     bad = np.flatnonzero((plan["scaled_h"] < 1) | (plan["scaled_w"] < 1))
     if len(bad):
         s = int(bad[0])
-        raise ValueError(f"video_mc record id={questions[s // num_frames]['id']!r}: frame {s % num_frames} of "
+        raise ValueError(f"{task} record id={questions[s // num_frames]['id']!r}: frame {s % num_frames} of "
                          f"{hw[s, 0]}x{hw[s, 1]} pixels resizes to {plan['scaled_h'][s]}x{plan['scaled_w'][s]} for "
                          f"image_size {list(out_size)}")
     n = len(hw)
@@ -136,10 +136,12 @@ def _prepare(pool, device, questions, num_frames, out_size, draws=None):
 
 
 class _Pipeline(DevicePipeline):
-    """What the training and evaluation pipelines share: the shapes of the config and the batch of parsed records."""
+    """What the training and evaluation pipelines share: the shapes of the config and the batch of parsed records.  A
+    task with other records (video_qa_input) overrides TASK and the three methods after __init__."""
+    TASK = "video_mc"
 
     def __init__(self, config, files, batch_size, labelled, num_threads, device, prefetch):
-        self.num_frames, self.num_choices = check_config(config.model)
+        self._configure(config)
         self.max_len = int(config.downstream.get("max_text_len", DEFAULT_MAX_TEXT_LEN))
         self.vocab_size = int(config.model["vocab_size"])
         self.out_size = tuple(config.model["image_size"])
@@ -148,17 +150,28 @@ class _Pipeline(DevicePipeline):
         self.labelled = labelled
         super().__init__(device, num_threads, prefetch)
 
-    def _batch(self, records, draws_fn=None):
-        qs = [parse_question(parse_example(r), self.num_frames, self.num_choices, self.max_len, self.vocab_size)
-              for r in records]
+    def _configure(self, config):
+        self.num_frames, self.num_choices = check_config(config.model)
+
+    def _parse(self, record) -> Dict:
+        """One record as its parsed question (parse_question)."""
+        return parse_question(parse_example(record), self.num_frames, self.num_choices, self.max_len, self.vocab_size)
+
+    def _text_fields(self, qs) -> Dict[str, np.ndarray]:
+        """The batch's host arrays besides the frames: lm_input [b*C, L] and lm_targets [b]; checks labels if labelled."""
         if self.labelled:
             check_labels(qs, self.num_choices)
+        return {"lm_input": np.stack([q["lm_input"] for q in qs]).reshape(len(qs) * self.num_choices, self.max_len),
+                "lm_targets": np.array([q["label"] for q in qs], dtype=np.int32)}
+
+    def _batch(self, records, draws_fn=None, qs=None):
+        if qs is None:
+            qs = [self._parse(r) for r in records]
+        text = self._text_fields(qs)
         draws = draws_fn(len(qs)) if draws_fn is not None else None
-        images, mask, plan = _prepare(self._pool, self.device, qs, self.num_frames, self.out_size, draws)
-        lm = np.stack([q["lm_input"] for q in qs]).reshape(len(qs) * self.num_choices, self.max_len)
-        feats = {"images": images, "img_mask": _to_device(mask, self.device), "lm_input": _to_device(lm, self.device),
-                 "lm_targets": _to_device(np.array([q["label"] for q in qs], dtype=np.int32), self.device),
-                 "id": [q["id"] for q in qs]}
+        images, mask, plan = _prepare(self._pool, self.device, qs, self.num_frames, self.out_size, draws, self.TASK)
+        feats = {"images": images, "img_mask": _to_device(mask, self.device),
+                 **{k: _to_device(v, self.device) for k, v in text.items()}, "id": [q["id"] for q in qs]}
         return feats, {"records": list(records), "id": feats["id"], "plan": plan, "draws": draws}
 
 
@@ -209,6 +222,12 @@ def input_fn_builder(config, is_training: bool = True, rank: int = 0, world: int
     the micro-batch of config.micro_batching).  Evaluation: the files of data.val_file in sorted glob order, batches of
     `batch_size` questions (default device.val_batch_size), of which rank `rank` of `world` gets the global batches k with
     k % world == rank.  Returns the running pipeline (close() it)."""
+    return _input_fn(VideoMCTrainPipeline, VideoMCEvalPipeline, config, is_training, rank, world, seed, batch_size, device,
+                     labelled)
+
+
+def _input_fn(train_cls, eval_cls, config, is_training, rank, world, seed, batch_size, device, labelled):
+    """input_fn_builder with the training and evaluation pipeline classes of a task."""
     if is_training:
         files = train_files(config.data)
         if not files:
@@ -216,10 +235,10 @@ def input_fn_builder(config, is_training: bool = True, rank: int = 0, world: int
         files = shard_files(files, rank, world)
         if batch_size is None:
             batch_size = micro_batching(config.device, world, default_batch_size=64)[1]
-        return VideoMCTrainPipeline(config, files, batch_size, rank=rank, seed=seed, device=device)
+        return train_cls(config, files, batch_size, rank=rank, seed=seed, device=device)
     files = val_files(config)
     if not files:
         raise ValueError(f"data.val_file {config.data.get('val_file')!r} matches no file")
     if batch_size is None:
         batch_size = config.device.get("val_batch_size", 64)
-    return VideoMCEvalPipeline(config, files, batch_size, labelled=labelled, device=device, rank=rank, world=world)
+    return eval_cls(config, files, batch_size, labelled=labelled, device=device, rank=rank, world=world)
