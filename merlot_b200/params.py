@@ -15,9 +15,13 @@ Storage differs from the TF variables in three places (converted by load_tf_dict
 (downstream/vcr/modeling.py model_fn: MerlotModel(mask_input=False) + the answer / rationale classifier towers) or
 "video_mc" (multiple-choice video QA, merlot_b200/video_mc.py: the VCR graph's model variables + one `mc_cls` tower of the
 answer tower's shapes and initialisers) or "video_qa" (open-ended video QA, merlot_b200/video_qa.py: the VCR graph's model
-variables + one `qa_cls` tower whose output layer has A = `num_answers` columns, zero-padded to a multiple of 8).  In pretraining, `share_params: False` gives the language-only pass its own
-`langonly_encoder/` stack of num_lang_transformer_hidden_layers layers beside the joint `encoder/`; the VCR and video_mc
-graphs have no language-only pass and ignore it (as do video_qa's).
+variables + one `qa_cls` tower whose output layer has A = `num_answers` columns, zero-padded to a multiple of 8) or
+"video_fib" (fill-in-the-blank video QA, merlot_b200/video_fib.py: the VCR graph's model variables + the pretraining MLM
+head's `lm_head/projection` and `lm_head/LayerNorm` (with do_projection) + a `fib_cls/answers` dense layer of A columns,
+zero-padded as video_qa's, whose initial values derive_fib_answers computes from the word embeddings).  In pretraining,
+`share_params: False` gives the language-only pass its own `langonly_encoder/` stack of num_lang_transformer_hidden_layers
+layers beside the joint `encoder/`; the VCR and video_mc graphs have no language-only pass and ignore it (as do video_qa's
+and video_fib's).
 
 save_checkpoint / restore_checkpoint write and read the whole training state (parameters, Adam slots, global_step) as the
 TensorFlow V2 checkpoints the reference's Estimator keeps in output_dir.
@@ -37,10 +41,12 @@ from .stem import stem_ops
 
 PAD = 64
 TEMPORAL_PAD_N = 8
-TASKS = ("pretrain", "vcr", "video_mc", "video_qa")
+TASKS = ("pretrain", "vcr", "video_mc", "video_qa", "video_fib")
+ANSWER_TASKS = ("video_qa", "video_fib")  # the tasks whose store holds an answer vocabulary of num_answers
 VCR_TOWERS = ("answer_cls", "rationale_cls")
 VIDEO_MC_TOWERS = ("mc_cls",)
 VIDEO_QA_TOWER = "qa_cls"
+VIDEO_FIB_ANSWERS = "fib_cls/answers"
 VCR_BIAS_PI = 0.25  # cls_head(hidden_state, bias_pi=0.25), downstream/vcr/modeling.py:77
 
 
@@ -57,8 +63,35 @@ class Entry:
 
 
 def padded_answers(num_answers: int) -> int:
-    """A8: the columns of the video_qa tower's output layer, num_answers rounded up to a multiple of 8 (16-byte rows)."""
+    """A8: the columns of an answer layer (video_qa's tower output, video_fib's fib_cls/answers), num_answers rounded up to
+    a multiple of 8 (16-byte rows)."""
     return (num_answers + TEMPORAL_PAD_N - 1) // TEMPORAL_PAD_N * TEMPORAL_PAD_N
+
+
+def derive_fib_answers(store: "ParamStore", answer_tokens, output_bias: Optional[torch.Tensor] = None) -> None:
+    """Write video_fib's answer layer from the MLM head's output layer: column a of fib_cls/answers/kernel is the mean of
+    the word-embedding rows (store.P, fp32) of answer a's token ids, bias[a] the mean of `output_bias` [vocab_size] at those
+    ids (lm_head/output_bias of a checkpoint; None: zero, the reference's do_bias: False).  Means are taken in float64 and
+    rounded to fp32; the padding columns are zero.  For a one-token answer this is that token's MLM logit exactly.  Then
+    refreshes the bf16 copy.  Runs once, when a store is set up; the layer is its own variable afterwards."""
+    if store.task != "video_fib":
+        raise ValueError(f"the fill-in-the-blank answer layer lives in a ParamStore(task='video_fib'), got {store.task!r}")
+    A = store.num_answers
+    if len(answer_tokens) != A:
+        raise ValueError(f"{len(answer_tokens)} answers given, the store holds {A}")
+    dev = store.device
+    tokens = torch.tensor([t for toks in answer_tokens for t in toks], dtype=torch.int64, device=dev)
+    seg = torch.repeat_interleave(torch.arange(A, device=dev), torch.tensor([len(t) for t in answer_tokens], device=dev))
+    count = torch.bincount(seg, minlength=A).to(torch.float64)
+    with torch.no_grad():
+        emb = store.P("word_embeddings/word_embeddings")
+        kern = torch.zeros((A, emb.shape[1]), dtype=torch.float64, device=dev).index_add_(0, seg, emb[tokens].double())
+        store.P(f"{VIDEO_FIB_ANSWERS}/kernel").zero_()[:, :A] = (kern / count[:, None]).float().t()
+        bias = store.P(f"{VIDEO_FIB_ANSWERS}/bias").zero_()
+        if output_bias is not None:
+            ob = output_bias.to(device=dev, dtype=torch.float64).reshape(-1)
+            bias[:A] = (torch.zeros(A, dtype=torch.float64, device=dev).index_add_(0, seg, ob[tokens]) / count).float()
+    store.sync_bf16()
 
 
 def _entries(cfg: dict, task: str = "pretrain", num_answers: int = 0) -> List[Entry]:
@@ -106,10 +139,18 @@ def _entries(cfg: dict, task: str = "pretrain", num_answers: int = 0) -> List[En
     add("vision_backbone/final_pe/cls_emb", (1, H))
     ln("vision_backbone/LayerNorm_final_ln")
     add("word_embeddings/word_embeddings", (V, H))
-    if task in ("vcr", "video_mc", "video_qa"):  # mask_input=False: no language-only encoder, no masking, no pretraining heads
+    if task in ("vcr", "video_mc", "video_qa", "video_fib"):  # mask_input=False: no language-only encoder, no masking
         add("position_embeddings/position_embeddings", (cfg["max_position_embeddings"], H))
         ln("position_embeddings/LayerNorm_embed_norm")
         stack("encoder", cfg["num_hidden_layers"])
+        if task == "video_fib":  # the MLM head's projection (model/modeling.py:205-224), then dense(A) stored as A8 columns
+            if cfg.get("do_projection", False):
+                lin("lm_head/projection", H, H)
+                ln("lm_head/LayerNorm")
+            A8 = padded_answers(num_answers)
+            add(f"{VIDEO_FIB_ANSWERS}/kernel", (H, A8), ref_cols=num_answers)
+            add(f"{VIDEO_FIB_ANSWERS}/bias", (A8,), ref_cols=num_answers)
+            return out
         if task == "video_qa":  # dense(H/2) + gelu, then dense(A) stored as A8 columns
             lin(f"{VIDEO_QA_TOWER}/classifier_mlp0", H, H // 2)
             A8 = padded_answers(num_answers)
@@ -195,7 +236,8 @@ def hyper_for(tf_name: str, optimizer_cfg: dict) -> Tuple[float, float, float, f
 class ParamStore:
     """Flat arenas + named views.  `optimizer_cfg` fixes the hyper-parameter grouping (needed only for training) and the
     Adam moments' storage: fp32 unless it sets use_bfloat16_adam (the reference's default is False); without an
-    optimizer_cfg the moments are bf16.  `num_answers` (task "video_qa" only, >= 2) is the answer vocabulary's size A."""
+    optimizer_cfg the moments are bf16.  `num_answers` (tasks "video_qa" and "video_fib" only, >= 2) is the answer
+    vocabulary's size A."""
 
     def __init__(self, model_cfg: dict, device="cuda", optimizer_cfg: Optional[dict] = None, with_optimizer_state=True,
                  task: str = "pretrain", num_answers: Optional[int] = None):
@@ -203,11 +245,11 @@ class ParamStore:
         # are provided (K13), its variables follow the reference's creation order (stem_variables).
         if task not in TASKS:
             raise ValueError(f"ParamStore task must be one of {TASKS}, got {task!r}")
-        if (task == "video_qa") != (num_answers is not None):
-            raise ValueError(f"num_answers is the size of the video_qa answer vocabulary: task={task!r}, "
-                             f"num_answers={num_answers!r}")
-        if task == "video_qa" and int(num_answers) < 2:
-            raise ValueError(f"video_qa: num_answers must be >= 2, got {num_answers}")
+        if (task in ANSWER_TASKS) != (num_answers is not None):
+            raise ValueError(f"num_answers is the size of the {task if task in ANSWER_TASKS else 'video_qa'} answer "
+                             f"vocabulary: task={task!r}, num_answers={num_answers!r}")
+        if task in ANSWER_TASKS and int(num_answers) < 2:
+            raise ValueError(f"{task}: num_answers must be >= 2, got {num_answers}")
         self.cfg = model_cfg
         self.task = task
         self.num_answers = None if num_answers is None else int(num_answers)

@@ -116,7 +116,7 @@ def main(argv=None) -> Optional[List[str]]:
     ap.add_argument("--seed", type=int, default=0, help="seed of the evaluation draws (parser, dropout and masking)")
     args = ap.parse_args(argv)
     config = NeatConfig.from_yaml(args.config_file)
-    if config.downstream.get("task") in ("vcr", "video_mc", "video_qa"):
+    if config.downstream.get("task") in ("vcr", "video_mc", "video_qa", "video_fib"):
         raise ValueError(f"downstream.task is {config.downstream.get('task')!r}: PREDICT runs on the pretraining model")
     check_val_file(config)
     eval_batch_count(config)

@@ -133,7 +133,7 @@ def main(argv=None, clock: Callable[[], float] = time.monotonic, sleep: Callable
     ap.add_argument("--seed", type=int, default=0, help="seed of the evaluation draws (parser, dropout and masking)")
     args = ap.parse_args(argv)
     config = NeatConfig.from_yaml(args.config_file)
-    if config.downstream.get("task") in ("vcr", "video_mc", "video_qa"):
+    if config.downstream.get("task") in ("vcr", "video_mc", "video_qa", "video_fib"):
         task = config.downstream.get("task")
         raise ValueError(f"downstream.task is {task!r}: validate {'VCR' if task == 'vcr' else task} fine-tuning with "
                          f"merlot_b200.{task}_validate")

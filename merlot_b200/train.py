@@ -6,6 +6,7 @@
   * `synthetic_vcr_batch` -- the same for VCR fine-tuning (downstream/vcr/dataloader_joint.py:135-189,257-271).
   * `synthetic_video_mc_batch` -- the same for multiple-choice video QA (video_mc_input.py's training batches).
   * `synthetic_video_qa_batch` -- the same for open-ended video QA (video_qa_input.py's training batches).
+  * `synthetic_video_fib_batch` -- the same for fill-in-the-blank video QA (video_fib_input.py's training batches).
   * `model_fn_builder` -- same name and call shape as the reference; returns a model_fn(features, labels, mode, params)
                           that builds MerlotModel(is_training=True, mask_input=True), sums lang + contr + temp losses
                           (modeling.py:700-713) and exposes `train_op()` = backward + gradient all-reduce + AdamW.
@@ -23,7 +24,7 @@ import torch
 
 from .config import NeatConfig, micro_batching, replica_seed
 from .dataloader import input_fn_builder, train_files
-from .modeling import MerlotModel, START, _Buffers, contrastive_head, contrastive_head_bwd
+from .modeling import MASK, MerlotModel, START, _Buffers, contrastive_head, contrastive_head_bwd
 from .optimization import build_optimizer_from_config
 from .params import ParamStore
 
@@ -177,6 +178,30 @@ def synthetic_video_qa_batch(config: NeatConfig, questions: int, seed: int = 0, 
     ids = ids * (torch.arange(L)[None] < lens[:, None]).int()
     targets = torch.randint(0, A, (questions,), generator=g, dtype=torch.int32)
     feats = {"images": images.to(torch.bfloat16), "img_mask": img_mask, "lm_input": ids, "lm_targets": targets}
+    return {k: v.to(device) for k, v in feats.items()}
+
+
+def synthetic_video_fib_batch(config: NeatConfig, questions: int, seed: int = 0, device="cuda") -> Dict[str, torch.Tensor]:
+    """Training features of `questions` fill-in-the-blank video questions with video_fib_input's shapes: images, img_mask
+    and lm_input drawn as synthetic_video_qa_batch's, then one MASK at a random position of every text's words,
+    blank_pos [q] int32 its position, and lm_targets [q] int32 in [0, A) (A = the answers of downstream.answer_tokens)."""
+    from .video_fib import check_config
+    m = config.model
+    Hh, Ww = m["image_size"]
+    F, answers = check_config(m, config.downstream)
+    L = int(config.downstream.get("max_text_len", 128))
+    g = torch.Generator().manual_seed(seed)
+    img_mask = torch.arange(F)[None] < (1 + torch.arange(questions) % F)[:, None]
+    images = torch.rand(questions * F, Hh, Ww, 3, generator=g) * img_mask.reshape(-1, 1, 1, 1)
+    ids = torch.randint(100, m["vocab_size"], (questions, L), generator=g, dtype=torch.int32)
+    ids[:, 0] = START
+    lens = torch.randint(min(16, L), L + 1, (questions,), generator=g)
+    ids = ids * (torch.arange(L)[None] < lens[:, None]).int()
+    blank = 1 + (torch.rand(questions, generator=g) * (lens - 1)).long()  # one of the words after START
+    ids[torch.arange(questions), blank] = MASK
+    targets = torch.randint(0, len(answers), (questions,), generator=g, dtype=torch.int32)
+    feats = {"images": images.to(torch.bfloat16), "img_mask": img_mask, "lm_input": ids, "lm_targets": targets,
+             "blank_pos": blank.to(torch.int32)}
     return {k: v.to(device) for k, v in feats.items()}
 
 
@@ -457,7 +482,7 @@ def eval_seed(seed: int, k: int) -> int:
 def _step_for(config: NeatConfig):
     """(model_fn_builder, synthetic batch) of the configured task: downstream.task 'vcr' fine-tunes on VCR
     (downstream/vcr/train.py), 'video_mc' on multiple-choice video QA (video_mc.py), 'video_qa' on open-ended video QA
-    (video_qa.py), anything else pretrains (model/train.py)."""
+    (video_qa.py), 'video_fib' on fill-in-the-blank video QA (video_fib.py), anything else pretrains (model/train.py)."""
     if config.downstream.get("task") == "vcr":
         from .vcr import vcr_model_fn_builder
         return vcr_model_fn_builder, synthetic_vcr_batch
@@ -467,15 +492,18 @@ def _step_for(config: NeatConfig):
     if config.downstream.get("task") == "video_qa":
         from .video_qa import video_qa_model_fn_builder
         return video_qa_model_fn_builder, synthetic_video_qa_batch
+    if config.downstream.get("task") == "video_fib":
+        from .video_fib import video_fib_model_fn_builder
+        return video_fib_model_fn_builder, synthetic_video_fib_batch
     return model_fn_builder, synthetic_batch
 
 
 def variables_without_gradient(model_cfg: dict, store: ParamStore):
     """Entries whose gradient is None in the training graph, so the reference's apply_gradients neither updates them nor
     creates their Adam slots: the `skip` list model_fn_builder hands AdamW (no viz_viz temporal head without image
-    shuffling, no temporal heads at temporal_coef 0).  The VCR, video_mc and video_qa graphs reach every variable of their
-    store."""
-    if store.task in ("vcr", "video_mc", "video_qa"):
+    shuffling, no temporal heads at temporal_coef 0).  The VCR, video_mc, video_qa and video_fib graphs reach every variable
+    of their store."""
+    if store.task in ("vcr", "video_mc", "video_qa", "video_fib"):
         return []
     if model_cfg.get("temporal_coef", 1.0) > 0.0:
         return [] if model_cfg.get("image_shuffle_prob", 0) > 0 else [n for n in store.entries if n.startswith("viz_viz_temporal/")]
@@ -483,11 +511,12 @@ def variables_without_gradient(model_cfg: dict, store: ParamStore):
 
 
 def main(argv=None):
-    """`python -m merlot_b200.train configs/merlot.yaml` (or merlot_vcr.yaml, or a downstream.task: video_mc or video_qa
-    config) -- the role of model/train.py:9-26 and downstream/vcr/train.py.  Every task reads data.train_file when it
-    matches at least one file (pretraining through dataloader.input_fn_builder, VCR fine-tuning through
+    """`python -m merlot_b200.train configs/merlot.yaml` (or merlot_vcr.yaml, or a downstream.task: video_mc, video_qa or
+    video_fib config) -- the role of model/train.py:9-26 and downstream/vcr/train.py.  Every task reads data.train_file
+    when it matches at least one file (pretraining through dataloader.input_fn_builder, VCR fine-tuning through
     vcr_input.input_fn_builder, video_mc through video_mc_input.input_fn_builder, video_qa through
-    video_qa_input.input_fn_builder) and otherwise trains on synthetic batches.
+    video_qa_input.input_fn_builder, video_fib through video_fib_input.input_fn_builder) and otherwise trains on synthetic
+    batches.
 
     Checkpoints, as the reference's Estimator keeps them (utils/neat_config.py:136-141): when device.output_dir already names
     a latest checkpoint, every rank restores it (parameters, Adam slots, global_step; this takes precedence over
@@ -533,13 +562,15 @@ def main(argv=None):
     accum, per_rank = micro_batching(config.device, world)  # A micro-batches of per_rank examples per step and rank
     pipeline = None
     if train_files(config.data):
-        from . import vcr_input, video_mc_input, video_qa_input
+        from . import vcr_input, video_fib_input, video_mc_input, video_qa_input
         if make_batch is synthetic_batch:
             build_input = input_fn_builder
         elif make_batch is synthetic_video_mc_batch:
             build_input = video_mc_input.input_fn_builder
         elif make_batch is synthetic_video_qa_batch:
             build_input = video_qa_input.input_fn_builder
+        elif make_batch is synthetic_video_fib_batch:
+            build_input = video_fib_input.input_fn_builder
         else:
             build_input = vcr_input.input_fn_builder
         pipeline = build_input(config, is_training=True, rank=rank, world=world, seed=store.global_step if resume else 0,
@@ -547,7 +578,8 @@ def main(argv=None):
     elif rank == 0:
         what = {synthetic_batch: f"data.train_file {config.data.get('train_file')!r} matches no file",
                 synthetic_video_mc_batch: "video_mc fine-tuning",
-                synthetic_video_qa_batch: "video_qa fine-tuning"}.get(make_batch, "VCR fine-tuning")
+                synthetic_video_qa_batch: "video_qa fine-tuning",
+                synthetic_video_fib_batch: "video_fib fine-tuning"}.get(make_batch, "VCR fine-tuning")
         print(f"{what}: training on synthetic batches", flush=True)
     try:
         for step in range(store.global_step, num_steps):

@@ -75,8 +75,9 @@ def log_softmax(logits: np.ndarray) -> np.ndarray:
 class Validator:
     """Evaluates checkpoints of a VCR run on the evaluation input of config (data.val_file, downstream.mode).  With an
     eval_ranks.EvalGroup of several ranks, each rank evaluates the global batches k with k % world == rank, and every rank
-    gets the result one rank would compute.  video_mc_validate.Validator and video_qa_validate.Validator are this class
-    over other tasks: the class attributes and the methods between __init__ and _own_batches are what a task sets."""
+    gets the result one rank would compute.  video_mc_validate.Validator, video_qa_validate.Validator and
+    video_fib_validate.Validator are this class over other tasks: the class attributes and the methods between __init__ and
+    _own_batches are what a task sets."""
     TASK = "vcr"
     METRIC = "avg"                     # the results line's name of the mean accuracy
     ID_KEYS = ("annot_id", "img_id")   # per-question host strings of a batch, kept in the predictions
@@ -98,9 +99,22 @@ class Validator:
         self.model_fn = self._model_fn_builder()(config, store=self.store, device=device)
         self.device = device
 
+    @classmethod
+    def add_arguments(cls, ap: argparse.ArgumentParser) -> None:
+        """Add the task's own command-line options to `run`'s parser."""
+
+    @classmethod
+    def options(cls, args) -> Dict:
+        """Keyword arguments of the constructor from the parsed command line besides config, chunk and group."""
+        return {}
+
     def _store_options(self) -> Dict:
         """Keyword arguments of the task's ParamStore besides the model config and the task."""
         return {}
+
+    def _restore(self, prefix: str) -> None:
+        """Fill self.store from checkpoint `prefix`: the trainer's strict restore (parameters, slots, global_step)."""
+        self.store.restore_checkpoint(prefix)
 
     def _model_fn_builder(self):
         from .vcr import vcr_model_fn_builder
@@ -141,7 +155,7 @@ class Validator:
         labels.  With several ranks the tensors are copied to the host for the gather."""
         import torch
         g = self.group
-        self.store.restore_checkpoint(prefix)
+        self._restore(prefix)
         mode = "eval" if labelled else "predict"
         out = []
         with torch.no_grad(), self._input(labelled) as pipe:
@@ -226,6 +240,7 @@ def run(validator_cls, description: str, task_name: str, argv=None, clock: Calla
                     help="the records have no labels: predictions only, no loss or accuracy (needs --predictions)")
     ap.add_argument("--chunk", type=int, default=0, help="questions per forward (default: device.val_batch_size)")
     ap.add_argument("--poll-interval", type=float, default=60.0, help="seconds between looks at device.output_dir")
+    validator_cls.add_arguments(ap)
     args = ap.parse_args(argv)
     if args.predictions and not args.checkpoint:
         raise ValueError("--predictions writes one checkpoint's predictions: pass --checkpoint PREFIX")
@@ -235,6 +250,7 @@ def run(validator_cls, description: str, task_name: str, argv=None, clock: Calla
         raise ValueError("--unlabelled computes no metrics: pass --predictions PATH.npz")
     if args.chunk < 0:
         raise ValueError(f"--chunk {args.chunk} must be >= 0")
+    options = validator_cls.options(args)
     config = NeatConfig.from_yaml(args.config_file)
     if config.downstream.get("task") != validator_cls.TASK:
         raise ValueError(f"downstream.task is {config.downstream.get('task')!r}, {task_name} validation needs "
@@ -264,7 +280,7 @@ def run(validator_cls, description: str, task_name: str, argv=None, clock: Calla
 
     results = []
     with eval_group() as group:  # WORLD_SIZE > 1: rank 0 follows the checkpoints and writes, every rank evaluates
-        v = validator_cls(config, chunk=args.chunk, group=group)
+        v = validator_cls(config, chunk=args.chunk, group=group, **options)
         for prefix in group.shared_prefixes(follow, sleep):
             res = v.evaluate(prefix, labelled=not args.unlabelled, keep_predictions=bool(args.predictions))
             group.on_rank0(lambda: write(prefix, res))

@@ -30,31 +30,33 @@ from .vcr_input import END, PADDING, START
 from .video_mc_input import VideoMCEvalPipeline, VideoMCTrainPipeline, _id, _input_fn, _tokens, train_draws
 from .video_qa import check_config
 
-def parse_question(example, num_frames: int, max_len: int, vocab_size: int) -> Dict:
+def parse_question(example, num_frames: int, max_len: int, vocab_size: int, task: str = "video_qa") -> Dict:
     """One parsed record without its pixels: {id (str), jpegs (list of 1..num_frames bytes), answer (int, None if
-    absent), lm_input int32 [max_len]}.  Raises ValueError naming the id on the record errors the module lists."""
+    absent), lm_input int32 [max_len]}.  Raises ValueError naming the id (and `task`) on the record errors the module
+    lists."""
     rid = _id(example)
     jpegs = [bytes(x) for x in example.get("frames/encoded", [])]
     if not 1 <= len(jpegs) <= num_frames:
-        raise ValueError(f"video_qa record id={rid!r}: {len(jpegs)} frames, expected 1 to {num_frames} (model.num_imgs)")
-    q = _tokens(example, "question", rid, vocab_size, required=False, task="video_qa")
+        raise ValueError(f"{task} record id={rid!r}: {len(jpegs)} frames, expected 1 to {num_frames} (model.num_imgs)")
+    q = _tokens(example, "question", rid, vocab_size, required=False, task=task)
     toks = np.concatenate([[START], q, [END]]).astype(np.int64).astype(np.int32)[:max_len]
     lm = np.full(max_len, PADDING, dtype=np.int32)
     lm[:len(toks)] = toks
     v = example.get("answer")
     if v is not None and len(v) != 1:
-        raise ValueError(f"video_qa record id={rid!r}: answer has {len(v)} values, expected 1")
+        raise ValueError(f"{task} record id={rid!r}: answer has {len(v)} values, expected 1")
     return {"id": rid, "jpegs": jpegs, "answer": int(v[0]) if v is not None else None, "lm_input": lm}
 
 
-def check_answers(questions: Sequence[Dict], num_answers: int) -> None:
-    """Raise ValueError naming the id of the first question without an answer or with one outside [-1, num_answers)."""
+def check_answers(questions: Sequence[Dict], num_answers: int, task: str = "video_qa") -> None:
+    """Raise ValueError naming the id (and `task`) of the first question without an answer or with one outside
+    [-1, num_answers)."""
     for q in questions:
         if q["answer"] is None:
-            raise ValueError(f"video_qa record id={q['id']!r}: answer is missing (an unlabelled record can only be scored "
+            raise ValueError(f"{task} record id={q['id']!r}: answer is missing (an unlabelled record can only be scored "
                              f"without a loss)")
         if not -1 <= q["answer"] < num_answers:
-            raise ValueError(f"video_qa record id={q['id']!r}: answer is {q['answer']}, outside [-1, {num_answers}) "
+            raise ValueError(f"{task} record id={q['id']!r}: answer is {q['answer']}, outside [-1, {num_answers}) "
                              f"(-1 marks an answer outside the vocabulary)")
 
 
@@ -63,14 +65,15 @@ def labels(questions: Sequence[Dict]) -> np.ndarray:
     return np.array([-1 if q["answer"] is None else q["answer"] for q in questions], dtype=np.int32)
 
 
-def take_answerable(records: Iterator, n: int, parse, num_answers: int) -> Tuple[List, List[Dict], int]:
+def take_answerable(records: Iterator, n: int, parse, num_answers: int,
+                    task: str = "video_qa") -> Tuple[List, List[Dict], int]:
     """The next n records of `records` whose answer is in the vocabulary, their parsed questions, and the number of OOV
     questions passed over on the way.  Every record is parsed and checked (check_answers) first."""
     recs, qs, skipped = [], [], 0
     while len(qs) < n:
         r = next(records)
         q = parse(r)
-        check_answers([q], num_answers)
+        check_answers([q], num_answers, task)
         if q["answer"] < 0:
             skipped += 1
             continue
@@ -107,7 +110,7 @@ class VideoQATrainPipeline(_QA, VideoMCTrainPipeline):
     def _produce(self):
         recs = shuffled_records(self.files, self.rng, self.cycle_length, self.shuffle_buffer_size, self._stop)
         while not self._stop.is_set():
-            records, qs, skipped = take_answerable(recs, self.batch_size, self._parse, self.num_answers)
+            records, qs, skipped = take_answerable(recs, self.batch_size, self._parse, self.num_answers, self.TASK)
             self.skipped += skipped
             yield self._batch(records, lambda n: train_draws(self.rng, n), qs=qs)
 
