@@ -232,6 +232,15 @@ int merlot_ctr_split(const float* x, int rows, int C, int ldx, void* out, long l
                      void* stream);
 int merlot_ctr_dlogits(const float* logits, int ld, const int* labels, int rows, int C, const float* lse,
                        const float* coeff, float scale, void* dsh, int ld_h, void* dsv, int ld_v, void* stream);
+/* K17: exact rank and top-k of fp32 score rows (frame <-> transcript retrieval, merlot_b200/retrieval_validate.py).
+ * scores [rows, cols] with row stride ld >= cols; pos [rows] int32.  Per row r, with p = scores[r, pos[r]]:
+ *   greater[r] = #{j : s[r,j] > p};  ties[r] = #{j != pos[r] : s[r,j] == p};
+ *   topk_idx / topk_val [rows, k] (row stride k) = the k largest entries by (score descending, index ascending), 1 <= k <= 32.
+ * NaN is never greater, never equal and never in the top k; a NaN p sets greater = -1, a pos[r] outside [0, cols) sets
+ * greater = -2 (ties = 0 in both cases).  Top-k slots past the row's non-NaN entries hold index -1 and value NaN.
+ * Integer counts and a fixed-order merge: exact and deterministic. */
+int merlot_rank_topk(const float* scores, int rows, int cols, long long ld, const int* pos, int k, int* greater, int* ties,
+                     int* topk_idx, float* topk_val, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Transformer stack driver (utils/transformer.py:171-247 `transformer`, pre-LN; forward and explicit backward).

@@ -581,6 +581,26 @@ def ctr_dlogits(logits, labels, C, lse, coeff, scale, dsh, dsv):
                                coeff.data_ptr(), scale, dsh.data_ptr(), dsh.stride(0), dsv.data_ptr(), dsv.stride(0), _stream())
 
 
+def rank_topk(scores, pos, k, greater=None, ties=None, topk_idx=None, topk_val=None):
+    """K17: per row r of fp32 scores [rows, cols] (any row stride >= cols), with p = scores[r, pos[r]]: greater[r] (entries
+    > p; -1 when p is NaN, -2 when pos[r] is outside the row), ties[r] (other entries == p) and the k largest entries by
+    (score descending, index ascending) as topk_idx / topk_val [rows, k] (index -1, value NaN past the non-NaN entries).
+    Returns (greater, ties, topk_idx, topk_val)."""
+    _require_cuda(scores, pos, greater, ties, topk_idx, topk_val)
+    assert scores.dtype == torch.float32 and scores.dim() == 2 and scores.stride(1) == 1
+    assert pos.dtype == torch.int32 and pos.is_contiguous() and pos.numel() == scores.shape[0]
+    rows, dev = scores.shape[0], scores.device
+    greater = torch.empty(rows, dtype=torch.int32, device=dev) if greater is None else greater
+    ties = torch.empty(rows, dtype=torch.int32, device=dev) if ties is None else ties
+    topk_idx = torch.empty((rows, k), dtype=torch.int32, device=dev) if topk_idx is None else topk_idx
+    topk_val = torch.empty((rows, k), dtype=torch.float32, device=dev) if topk_val is None else topk_val
+    for t, dt in ((greater, torch.int32), (ties, torch.int32), (topk_idx, torch.int32), (topk_val, torch.float32)):
+        assert t.dtype == dt and t.is_contiguous() and t.numel() == rows * (1 if t.dim() == 1 else k)
+    L.lib().merlot_rank_topk(scores.data_ptr(), rows, scores.shape[1], max(scores.stride(0), scores.shape[1]), pos.data_ptr(), k,
+                             greater.data_ptr(), ties.data_ptr(), topk_idx.data_ptr(), topk_val.data_ptr(), _stream())
+    return greater, ties, topk_idx, topk_val
+
+
 def axpby(x, y, a=1.0, b=1.0):
     L.lib().merlot_axpby_f32(x.data_ptr(), y.data_ptr(), x.numel(), a, b, _stream())
 
