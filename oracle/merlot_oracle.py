@@ -874,6 +874,20 @@ class AdamOracle:
         self.v = {k: torch.zeros_like(v, dtype=dt) for k, v in params.items()}
         self.global_step = 0
 
+    @classmethod
+    def from_state(cls, params: Params, optimizer_cfg: dict, m: Params, v: Params, global_step: int):
+        """The optimizer of a run that has taken `global_step` steps: moments `m` and `v` per parameter, stored as
+        use_bfloat16_adam stores them (bf16 m and sign-packed bf16 v, or fp32).  The tensors are copied."""
+        opt = cls(params, optimizer_cfg)
+        for name, p in params.items():
+            for slot, src in ((opt.m, m), (opt.v, v)):
+                t = src[name]
+                if t.dtype != slot[name].dtype or tuple(t.shape) != tuple(p.shape):
+                    raise ValueError(f"{name}: moment {t.dtype} {tuple(t.shape)}, expected {slot[name].dtype} {tuple(p.shape)}")
+                slot[name] = t.detach().cpu().clone().contiguous()
+        opt.global_step = int(global_step)
+        return opt
+
     def step_scalars(self):
         c = self.cfg
         beta1, beta2 = np.float32(0.9), np.float32(c.get("beta_2", 0.98))

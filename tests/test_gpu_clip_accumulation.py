@@ -77,16 +77,16 @@ def capture_applied(fn, store):
     return seen
 
 
-def oracle_replica_gradients(cfg, params, data, mask_info):
+def oracle_replica_gradients(cfg, params, data, mask_info, dropouts=None):
     """g_v of every replica: each replica holds its own leaf copy of the parameters and the SUM of the per-replica losses is
     differentiated, so leaf_v.grad also carries what the other replicas' contrastive losses send into v's features.
-    Returns ([{name: g_v float64}], mean loss)."""
+    `dropouts`: each replica's oracle dropout hook (training mode), or None.  Returns ([{name: g_v float64}], mean loss)."""
     B, Lj = 2 * NC // cfg["num_chunks_in_group"], LC * cfg["num_chunks_in_group"]
     leaves = [{k: v.clone().requires_grad_(True) for k, v in params.items()} for _ in data]
     oms = []
-    for (im, ids, sh, _), mk, leaf in zip(data, mask_info, leaves):
+    for (im, ids, sh, _), mk, leaf, dropout in zip(data, mask_info, leaves, dropouts or [None] * len(data)):
         gm = {"masked_ids": mk["masked_ids"].cpu().reshape(B, Lj), "masked_idx": mk["masked_idx"].cpu().reshape(B, -1)}
-        oms.append(O.MerlotOracle(cfg, leaf, im, ids, mask_input=True, shuffled_idx_img=sh, mask_override=gm))
+        oms.append(O.MerlotOracle(cfg, leaf, im, ids, mask_input=True, shuffled_idx_img=sh, mask_override=gm, dropout=dropout))
     mean_loss, per = O.pretrain_losses_replicas(oms, [d[2] for d in data], [d[3] for d in data])
     sum(per).backward()
     return [{k: v.grad.double() for k, v in leaf.items() if v.grad is not None} for leaf in leaves], float(mean_loss.detach())
@@ -122,7 +122,17 @@ def run_clipped_step(cfg, A, which):
     fn = model_fn_builder(config, store=store, device=DEV, seed=3)
     data, feats = micro_batches(cfg, A)
     seen = capture_applied(fn, store)
-    snaps = []  # each micro-batch's gradient as clip_accumulate finds it in store.g
+    r = clipped_step(fn, cfg, params, data, feats, which)
+    assert store.global_step == 1 and len(r["snaps"]) == A
+    return dict(r, seen=seen)
+
+
+def clipped_step(fn, cfg, params, data, feats, which, dropouts=None):
+    """One optimizer step of fn (clip_norm > 0) over the micro-batches `feats`, whose host copies are `data`: pass 1 draws
+    the masks, the replica oracle's gradients at `params` (with `dropouts`) set clip_norm = choose_clip(norms, which), then
+    train_op.  Returns the spec, each micro-batch's gradient as clip_accumulate found it in store.g ("snaps"), the oracle's
+    gradients, norms and mean loss, and c; checks that both gradient arenas end zeroed."""
+    store, snaps = fn.store, []
     clip = fn.optimizer.clip_accumulate
 
     def snap():
@@ -132,15 +142,16 @@ def run_clipped_step(cfg, A, which):
 
     fn.optimizer.clip_accumulate = snap
     spec = fn(feats)  # pass 1 draws the masks the oracle needs
-    gs, ref_loss = oracle_replica_gradients(cfg, params, data, spec.mask_info)
+    gs, ref_loss = oracle_replica_gradients(cfg, params, data, spec.mask_info, dropouts)
     norms = [norm_of(g) for g in gs]
     c = choose_clip(norms, which)
     fn.optimizer.clip_norm = c
     spec.train_op()
     torch.cuda.synchronize()
-    assert store.global_step == 1 and len(snaps) == A
+    fn.optimizer.clip_accumulate = clip
+    assert len(snaps) == len(feats)
     assert store.g_acc is not None and float(store.g.abs().sum()) == 0.0 and float(store.g_acc.abs().sum()) == 0.0
-    return dict(spec=spec, seen=seen, snaps=snaps, gs=gs, norms=norms, c=c, ref_loss=ref_loss)
+    return dict(spec=spec, snaps=snaps, gs=gs, norms=norms, c=c, ref_loss=ref_loss)
 
 
 @pytest.mark.parametrize("A", [2, 3])

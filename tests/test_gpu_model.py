@@ -34,14 +34,17 @@ def synth(cfg, batch, nc, Lc, h0, w0, seed):
     return image, ids, shuf.int(), vid
 
 
-def build(cfg, seed=1):
+def bf16_operands(params):
+    """GEMM operands are the bf16 compute copies (bfloat16_getter): hand the oracle the same rounded matrices."""
+    return {k: (v.bfloat16().float() if (k.endswith("kernel") or k.endswith("word_embeddings")) else v) for k, v in params.items()}
+
+
+def build(cfg, seed=1, ocfg=None):
     from merlot_b200.params import ParamStore
-    params = O.init_params(cfg, seed=seed, perturb=0.05)
-    # GEMM operands are the bf16 compute copies (bfloat16_getter): hand the oracle the same rounded matrices
-    params = {k: (v.bfloat16().float() if (k.endswith("kernel") or k.endswith("word_embeddings")) else v) for k, v in params.items()}
-    ocfg = dict(type="adam_optimizer", learning_rate=3e-4, num_train_steps=1000, num_warmup_steps=10, weight_decay_rate=0.1,
-                beta_2=0.98, clip_norm=0.0, use_bfloat16_adam=True,
-                param_overrides=[[["LayerNorm", "layer_norm", "GroupNorm", "bias"], {"weight_decay_rate": 0}]])
+    params = bf16_operands(O.init_params(cfg, seed=seed, perturb=0.05))
+    ocfg = ocfg or dict(type="adam_optimizer", learning_rate=3e-4, num_train_steps=1000, num_warmup_steps=10, weight_decay_rate=0.1,
+                        beta_2=0.98, clip_norm=0.0, use_bfloat16_adam=True,
+                        param_overrides=[[["LayerNorm", "layer_norm", "GroupNorm", "bias"], {"weight_decay_rate": 0}]])
     store = ParamStore(cfg, device=DEV, optimizer_cfg=ocfg)
     store.load_tf_dict(params)
     return params, store, ocfg
@@ -96,17 +99,39 @@ def _step_parity(cfg, is_training=False, dropout_seed=0, oracle_dropout=None, wr
         if v.grad is None or float(v.grad.norm()) < 1e-7:  # key biases: softmax is shift invariant => exactly zero gradient
             continue
         assert rel(grads[k], v.grad) < 4e-2, k
-    # one AdamW step on those gradients vs the oracle optimizer fed the GPU gradients (isolates K10 from bf16 noise)
-    opt, _ = build_optimizer_from_config(None, ocfg, None, store=store)
+    # one AdamW step on those gradients vs the oracle optimizer fed the GPU gradients (isolates K10 from bf16 noise), taken at
+    # the end of the warm-up: at step 0 the learning rate is 0 and the parameters could not move on either side
+    check_adam_step(store, build_optimizer_from_config(None, ocfg, None, store=store)[0], ocfg, grads)
+    return m
+
+
+def check_adam_step(store, opt, ocfg, grads):
+    """opt.apply_gradients() at global_step num_warmup_steps against AdamOracle fed `grads` (the gradients in store.g):
+    parameters within 2e-6, the moments bit for bit; the parameters move by over 20x that bar (an Adam step from zero
+    moments moves a parameter by about 0.7 lr_t, 1.4e-4 at learning_rate 3e-4) and store.g ends zeroed."""
+    step = ocfg["num_warmup_steps"]
+    store.global_step = step
     p_before = {k: v.clone() for k, v in store.to_tf_dict("p").items()}
-    adam = O.AdamOracle(p_before, ocfg)
-    adam.apply_gradients(p_before, {k: v for k, v in grads.items()})
+    p_ref = {k: v.clone() for k, v in p_before.items()}
+    adam = O.AdamOracle(p_ref, ocfg)
+    adam.global_step = step
+    assert float(adam.step_scalars()["lr"]) > 0
+    adam.apply_gradients(p_ref, grads)
     opt.apply_gradients()
     after = store.to_tf_dict("p")
     for k in after:
-        assert (after[k] - p_before[k]).abs().max().item() < 2e-6, k
-    assert float(store.g.abs().max()) == 0.0 and store.global_step == 1
-    return m
+        assert (after[k] - p_ref[k]).abs().max().item() < 2e-6, k
+    assert max((after[k] - p_before[k]).abs().max().item() for k in after) > 20 * 2e-6
+    for buf, ref in ((store.m, adam.m), (store.v, adam.v)):
+        views = store.tf_views(buf)
+        assert len(views) == len(ref)
+        for _, nm, t in views:
+            assert t.dtype == ref[nm].dtype and torch.equal(bits(t.cpu().contiguous()), bits(ref[nm].contiguous())), nm
+    assert float(store.g.abs().max()) == 0.0 and store.global_step == step + 1
+
+
+def bits(t):
+    return t.view(torch.int16) if t.dtype == torch.bfloat16 else t.view(torch.int32)
 
 
 def test_pretrain_step_parity(tiny_cfg):

@@ -28,7 +28,7 @@ def vcr_cfg(tiny_cfg, **kw):
     return dict(tiny_cfg, num_texts=4, num_chunks_in_group=1, hidden_dropout_prob=0.1, **kw)
 
 
-def build(cfg, seed=1, tower_scale=3.0, encoder_scale=5.0, device=DEV):
+def build(cfg, seed=1, tower_scale=3.0, encoder_scale=5.0, device=DEV, ocfg=OCFG):
     """Oracle-initialised VCR variables, GEMM operands rounded to bf16, loaded into a ParamStore(task="vcr").  Two scalings
     keep the comparison meaningful.  The joint encoder's kernels are scaled so that a sequence's first token depends on its
     text: at the initialisers the four candidates' first tokens agree to a cosine of 0.9999, the tower gradients are then
@@ -43,7 +43,7 @@ def build(cfg, seed=1, tower_scale=3.0, encoder_scale=5.0, device=DEV):
         elif k.startswith("encoder/layer") and k.endswith("kernel"):
             params[k] = params[k] * encoder_scale
     params = {k: (v.bfloat16().float() if (k.endswith("kernel") or k.endswith("word_embeddings")) else v) for k, v in params.items()}
-    store = ParamStore(cfg, device=device, optimizer_cfg=OCFG, task="vcr")
+    store = ParamStore(cfg, device=device, optimizer_cfg=ocfg, task="vcr")
     store.load_tf_dict(params)
     return params, store
 
