@@ -459,18 +459,23 @@ def frame_table(plan, src_bytes: int) -> np.ndarray:
     return t
 
 
-def frames_prepare(src: torch.Tensor, plan, out_h: int, out_w: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+def frames_prepare(src: torch.Tensor, plan, out_h: int, out_w: int, out: Optional[torch.Tensor] = None,
+                   mean_ws: Optional[torch.Tensor] = None) -> torch.Tensor:
     """K14: bf16 [n, out_h, out_w, 3] <- convert, resize_and_pad, where(isfinite), augment and cast of n uint8 HWC frames packed
-    in `src` (a uint8 CUDA tensor), as `plan` (see frame_table) says.  Enqueued on the current stream."""
-    _require_cuda(src, out)
+    in `src` (a uint8 CUDA tensor), as `plan` (see frame_table) says.  Enqueued on the current stream.  `mean_ws`, a float32
+    CUDA tensor of n * 3 entries, receives the per-channel float32 mean of every contrast frame's padded image (the entries of
+    the other frames are left as they were); by default a scratch tensor does."""
+    _require_cuda(src, out, mean_ws)
     assert src.dtype == torch.uint8 and src.is_contiguous()
     table = frame_table(plan, src.numel())
     n = len(table)
     if out is None:
         out = torch.empty((n, out_h, out_w, 3), dtype=torch.bfloat16, device=src.device)
     assert out.dtype == torch.bfloat16 and out.is_contiguous() and tuple(out.shape) == (n, out_h, out_w, 3)
+    if mean_ws is None:
+        mean_ws = torch.empty(n * 3, dtype=torch.float32, device=src.device)
+    assert mean_ws.dtype == torch.float32 and mean_ws.is_contiguous() and mean_ws.numel() == n * 3
     table_dev = torch.from_numpy(table.view(np.uint8)).pin_memory().to(src.device, non_blocking=True)
-    mean_ws = torch.empty(n * 3, dtype=torch.float32, device=src.device)
     L.lib().merlot_frames_prepare(table_dev.data_ptr(), n, src.data_ptr(), out_h, out_w, mean_ws.data_ptr(), out.data_ptr(),
                                   _stream())
     return out

@@ -166,7 +166,8 @@ def resize_area(img, out_h, out_w):  # ResizeAreaOp::ComputeLoop, ComputePatchSu
         in_x, in_x1 = F(x) * ws, F(x + 1) * ws
         start, end = math.floor(in_x), math.ceil(in_x1)
         x_interps.append((start, end, cell_scale(start, in_x, in_x1, ws), cell_scale(end - 1, in_x, in_x1, ws)))
-    scale = F(1.0 / float(hs * ws))
+    with np.errstate(divide="ignore"):  # a 1-pixel side resized to more has scale 0: 1.0 / 0.0 is inf in C++
+        scale = F(np.float64(1.0) / np.float64(hs * ws))
     out = np.zeros((out_h, out_w, 3), F)
     for y in range(out_h):
         in_y, in_y1 = F(y) * hs, F(y + 1) * hs
@@ -181,7 +182,8 @@ def resize_area(img, out_h, out_w):  # ResizeAreaOp::ComputeLoop, ComputePatchSu
                             sum_y = sum_y + img[r, bound(xx, in_w), c]
                         sum_y = sum_y + img[r, bound(end - 1, in_w), c] * end_scale
                     total = total + sum_y * y_scale
-                out[y, x, c] = total * scale
+                with np.errstate(invalid="ignore"):  # 0 * inf when no row contributes: NaN, zeroed by where(isfinite)
+                    out[y, x, c] = total * scale
     return out
 
 

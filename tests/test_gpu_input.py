@@ -16,6 +16,7 @@ from merlot_b200 import dataloader as D
 from merlot_b200 import ops
 from merlot_b200.config import NeatConfig
 from oracle.oracle_np import process_example_np
+from tests import frames_exact_oracle as X
 from tests import input_oracle as O
 from tests import tfrecord_writer as W
 from tests.gemm_exact_oracle import bf16_ulps
@@ -24,17 +25,19 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _check(got, ref, method, transform, what):
-    d = bf16_ulps(got, ref)
-    if method == 1 and transform != 2:
-        # nearest copies one source value per pixel and the rest of the chain is elementwise: bit-exact
-        assert d.max() == 0, f"{what}: {int((d > 0).sum())} elements differ"
-    else:
-        # the other kernels sum in the source's order, but the contrast mean is a float32 sum whose order TensorFlow leaves
-        # unspecified (the oracle takes the float64 mean) and float libraries may round a product differently near a
-        # bf16 rounding boundary: at most 1 ulp, in at most 0.5% of the elements
-        assert d.max() <= 1, f"{what}: max {int(d.max())} ulp"
-        assert (d > 0).mean() <= 0.005, f"{what}: {(d > 0).mean():.4f} of the elements differ"
+def _check(got, ref, what):
+    # every operation of K14 and of the oracle is one float32 rounding in the TF source's order, so the outputs are equal
+    # bit for bit; contrast frames are checked against the oracle fed the kernel's own mean (_contrast_mean bounds it)
+    bad = got != ref
+    assert not bad.any(), f"{what}: {int(bad.sum())} elements differ, first at {np.argwhere(bad)[0].tolist()}"
+
+
+def _contrast_mean(mean, img, what):
+    """The kernel's float32 contrast mean against the float64 mean of the oracle's padded image, within the bound of its
+    reduction (tests/frames_exact_oracle.py:mean_bound)."""
+    err = np.abs(mean.astype(np.float64) - X.padded_mean(img))
+    assert (err <= X.mean_bound(img)).all(), f"{what}: mean {mean.tolist()} error {err.tolist()}"
+    return mean
 
 
 # ---- K14 against the oracle -------------------------------------------------------------------------------------------
@@ -71,17 +74,22 @@ def test_frames_prepare_matches_oracle():
     for m, t, si, sh, sw, oy, ox, fac in rows:
         for k, v in zip(ops.FRAME_FIELDS + ("factor",), (offs[si], *SOURCES[si], sh, sw, oy, ox, m, t, fac)):
             plan[k].append(v)
-    got = ops.frames_prepare(packed, plan, *OUT).float().cpu().numpy()
-    torch.cuda.synchronize()
+    mean_ws = torch.full((len(rows) * 3,), float("nan"), dtype=torch.float32, device="cuda")
+    got = ops.frames_prepare(packed, plan, *OUT, mean_ws=mean_ws).float().cpu().numpy()
+    means = mean_ws.cpu().numpy().reshape(-1, 3)
     assert got.shape == (len(rows),) + OUT + (3,)
     resized = {}
     for i, (m, t, si, sh, sw, oy, ox, fac) in enumerate(rows):
         key = (m, si, sh, sw, oy, ox)
         if key not in resized:
             resized[key] = O.resize_and_pad(srcs[si].astype(np.float32) * O.INV255, OUT, sh, sw, oy, ox, m)
-        ref = resized[key]
-        ref = O.bf16_round(O.augment(np.where(np.isfinite(ref), ref, np.float32(0)), t, fac))
-        _check(got[i], ref, m, t, f"{O.METHODS[m]} transform {t} source {SOURCES[si]} -> ({sh}, {sw}) at ({oy}, {ox})")
+        ref = np.where(np.isfinite(resized[key]), resized[key], np.float32(0))
+        what = f"{O.METHODS[m]} transform {t} source {SOURCES[si]} -> ({sh}, {sw}) at ({oy}, {ox})"
+        if t == 2:
+            ref = X.augment(ref, t, fac, _contrast_mean(means[i], ref, what))
+        else:
+            ref = O.augment(ref, t, fac)
+        _check(got[i], O.bf16_round(ref), what)
         if t == 0 and (sh < OUT[0] or sw < OUT[1]):
             assert (got[i][sh - oy:] == 0).all() and (got[i][:, sw - ox:] == 0).all()  # zero padding, bottom and right
 
@@ -130,12 +138,14 @@ def _oracle_batch(info, by_record, data, model):
             images.append(img)
     feats = {k: np.stack([t[k] for t in texts]) for k in texts[0]}
     feats["images"] = np.stack(images).reshape(len(texts), n, *out, 3)
+    feats["contrast"] = (np.asarray(fd["augment"]) == 2).reshape(len(texts), n)  # follows its frame through the shuffle
     pd = {k: v.numpy() for k, v in info["process_draws"].items()}
     idx, shuffled = process_example_np(feats["input_ids"], feats["video_src_ids"], pd["chunk_u"], pd["num_shuffle"], pd["pick_u"],
                                        pd["order_u"], model["num_chunks_in_group"], model["image_shuffle_prob"],
                                        data["shuffle_chunks"])
     feats = {k: np.take_along_axis(v, idx.reshape(idx.shape + (1,) * (v.ndim - 2)), 1) for k, v in feats.items()}
     feats["images"] = feats["images"].reshape(-1, *out, 3)
+    feats["contrast"] = feats["contrast"].reshape(-1)
     feats["shuffled_idx_img"] = shuffled
     return feats
 
@@ -156,7 +166,10 @@ def test_input_pipeline_batch_matches_oracle_and_trains(tmp_path, tiny_cfg):
             np.testing.assert_array_equal(feats[k].cpu().numpy(), ref[k], err_msg=k)
         got = feats["images"].float().cpu().numpy()
         d = bf16_ulps(got, ref["images"])
-        assert d.max() <= 1 and (d > 0).mean() <= 0.005, (int(d.max()), float((d > 0).mean()))  # as in the K14 test
+        c = ref["contrast"]
+        assert d[~c].max(initial=0) == 0, int((d[~c] > 0).sum())  # bit-exact, as in the K14 test
+        if c.any():  # the oracle's contrast mean is the float64 one, the kernel's a float32 sum
+            assert d[c].max() <= 1 and (d[c] > 0).mean() <= 0.005, (int(d[c].max()), float((d[c] > 0).mean()))
         model_fn = model_fn_builder(config, device="cuda")
         spec = model_fn(feats, None, "train", None)
         spec.train_op()

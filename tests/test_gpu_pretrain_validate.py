@@ -182,7 +182,10 @@ def test_eval_pipeline_images_match_oracle(tmp_path, tiny_cfg):
                     ref, _ = O.load_and_resize_img(u8, (64, 96), fd["scale"][i], fd["u_y"][i], fd["u_x"][i], fd["method"][i],
                                                    fd["augment"][i], fd["factor"][i])
                     d = bf16_ulps(got[i], ref)
-                    assert d.max() <= 1 and (d > 0).mean() <= 0.005, (int(d.max()), float((d > 0).mean()))  # the K14 bars
+                    if fd["augment"][i] != 2:
+                        assert d.max() == 0, int((d > 0).sum())  # bit-exact, the K14 bar
+                    else:  # the oracle's contrast mean is the float64 one, the kernel's a float32 sum
+                        assert d.max() <= 1 and (d > 0).mean() <= 0.005, (int(d.max()), float((d > 0).mean()))
             assert feats["shuffled_idx_img"].tolist() == [0, 1] * 4
 
 
